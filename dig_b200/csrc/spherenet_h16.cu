@@ -1,5 +1,10 @@
-// SphereNet / DimeNet++ dense edge-MLP chain, second generation: TWO 128-edge tiles in flight per CTA (one CTA per SM).
+// SphereNet / DimeNet++ dense chains on 3xFP16 wgmma.  Two engines:
+//   * update_e (parts A and B of an interaction block) runs on the register-accumulator engine (section "update_e:
+//     register-accumulator engine" below): activations stay in wgmma register fragments from layer to layer.
+//   * init_e, update_v and the generic linear run on the second-generation two-tile store engine: TWO 128-edge tiles in
+//     flight per CTA (one CTA per SM), accumulators handed to row-per-thread epilogues through the accumulator store.
 //
+// The two-tile store engine:
 // The first-generation chain (spherenet_tc.cu, 3xTF32) has fp32-sized operand planes (2 x 66 KB) and room for one
 // tile per CTA, so the tensor core waits during every epilogue.  Here:
 //
@@ -19,7 +24,8 @@
 //   * roles (640 threads): warpgroup 0 = weight ring (cp.async.bulk) + wgmma, warps 4..11 = epilogue of tile X,
 //     warps 12..19 = epilogue of tile Y (two warps per 32-row quarter, 64 columns each).
 //
-// Reference ops: update_e.forward spherenet.py:150-182 (dimenetpp.py:133-161), init.forward spherenet.py:79-91.
+// Reference ops: update_e.forward spherenet.py:150-182 (dimenetpp.py:133-161), init.forward spherenet.py:79-91,
+// update_v.forward spherenet.py:212-215.
 #include <cuda_fp16.h>
 #include "common.cuh"
 #define TC90_TM_COLS 512   // accumulator store columns per CTA slot
@@ -55,9 +61,6 @@ struct HSmem {
   unsigned char w[H_STAGES][H_STAGE_BYTES];
   float bias[8][128];
   float wr[128 * 8];
-  float wr1[64];
-  float wr2[128 * 8];                              // fused B + A(next block): lin_rbf2 of the NEXT block (wr is still lin_rbf of this one for the other tile)
-  float bias2[2][128];                             //                          b_ji (x 1), b_kj (x H_SA) of the next block
   int dst[2][H_M];
   int aux[2][2][H_M];                              // init_e: atomic numbers of the target / source node of each row
   // d_ready / d_free are indexed [tile][accumulator]: each barrier has ONE waiter that sees every phase in order
@@ -79,11 +82,9 @@ struct HGemm {
 
 static __device__ unsigned int g_h16_overflow = 0;
 static int h16_fast_swish = 1;
-static int h16_wide_epilogue = 0;   // update_e part B (+ A): 0 = eight epilogue warps per tile, 1 = all sixteen on the ready tile
-// optional timeline probe: CTA 0 of update_e part B records clock64() at protocol points (tools/gpu_h16_timeline.py)
+// optional timeline probe: CTA 0 of the update_e kernels records clock64() at protocol points (tools/gpu_h16_timeline.py)
 static __device__ long long g_h16_trace[128];
 static __device__ int g_h16_trace_on = 0;
-#define H_TRACE(slot) do { if (TRACE && g_h16_trace_on && blockIdx.x == 0) g_h16_trace[(slot)] = clock64(); } while (0)
 
 // x * sigmoid(x).  FAST (default): MUFU ex2 / rcp approximations in their flush-to-zero forms (the non-ftz forms
 // cost three extra instructions per element for denormal inputs that cannot occur here); the energy stays within the
@@ -130,7 +131,7 @@ __device__ __forceinline__ void h_produce(HSmem& s, const HGemm* g, int ng, int 
   ++it;
   if (++r.c == g[r.q].K / H_SLAB_K) { r.c = 0; if (++r.t == ntile) { r.t = 0; ++r.q; } }
 }
-template <bool TRACE, bool SHARED_A>
+template <bool SHARED_A>
 __device__ __forceinline__ void h_mma_n(HSmem& s, const HGemm* g, int ng, int ntile, uint32_t tmem) {
   const int wt = threadIdx.x;                            // 0..127
   HRing ring = {0, 0, 0};
@@ -148,7 +149,6 @@ __device__ __forceinline__ void h_mma_n(HSmem& s, const HGemm* g, int ng, int nt
         mbar_wait(&s.a_ready[SHARED_A ? 0 : t], q & 1);
         tc_fence_after();
       }
-      if (q < 8 && wt == 0) H_TRACE((q * 2 + t) * 2);
       const uint32_t a_hi = smem_u32(SHARED_A ? s.a[0][0] : s.a[t][0]), a_lo = smem_u32(SHARED_A ? s.a[1][0] : s.a[t][1]);
       for (int c = 0; c < nslab; c += 2, it += 2) {
         const int ab = ch & 1;
@@ -193,14 +193,9 @@ __device__ __forceinline__ void h_mma_n(HSmem& s, const HGemm* g, int ng, int nt
         if (ab) last1 = t; else last0 = t;
         ++ch;
       }
-      if (q < 8 && wt == 0) H_TRACE((q * 2 + t) * 2 + 1);
       if (SHARED_A && t == ntile - 1 && wt == 0) mbar_arrive(&s.l_done);
     }
   }
-}
-template <int NG, bool TRACE = false>
-__device__ __forceinline__ void h_mma(HSmem& s, const HGemm (&g)[NG], int ntile, uint32_t tmem) {
-  h_mma_n<TRACE, false>(s, g, NG, ntile, tmem);
 }
 
 // ---- epilogue context: thread = one row of its tile, NC = 64 (N = 128) or 32 (N = 64) columns
@@ -448,716 +443,485 @@ __global__ void h16_pack_kernel(HPackJobs jobs) {
   }
 }
 
-// ---------------------------------------------------------------------------------- update_e part B
-struct HBParams {
-  HGemm g[11];                 // lin_up, res0.lin1, res0.lin2, lin, res1.lin1, res1.lin2, res2.lin1, res2.lin2
-                               // FUSE: + lin_ji, lin_kj, lin_down of the NEXT block
-  const float* w_rbf;          // [128, 6]
-  const float *n_w_rbf1, *n_w_rbf2;     // FUSE: lin_rbf1 [8, 6], lin_rbf2 [128, 8] of the next block
-  float *n_x_ji, *n_x_down;             // FUSE: part-A outputs of the next block
+// ---------------------------------------------------------------------------------- update_e: register-accumulator engine
+// Part B of update_e (lin_up, the residual layers, lin; spherenet.py:172-179, edge -> node sum :211) and part A
+// (lin_ji, lin_kj, lin_down; spherenet.py:154-161) keep every activation of a 64-edge unit in wgmma register fragments:
+//
+//   * roles (384 threads): warpgroup 0 is the producer -- one thread streams the packed weight slabs of every layer
+//     through a ring of R_STAGES K = 32 slabs (cp.async.bulk, full / empty mbarriers; a stage is refilled once both
+//     consumers' MMAs that read it have completed).  Warpgroups 1 and 2 are consumers, each working on one 64-row unit
+//     at a time: a consumer issues its own wgmma with A FROM REGISTERS and B from the ring, then runs the layer's
+//     epilogue on the accumulator fragment while the other consumer's MMAs keep the tensor pipe busy (ping-pong).
+//     Consumer 1 starts after consumer 0 has issued its first layer; the stagger then persists because each consumer's
+//     MMAs queue behind the other's.
+//   * the m64nN accumulator fragment has the layout of the register A operand of the next layer's m64k16 steps
+//     (wgmma.cuh, frag_a_src): the epilogue splits each activated pair into the fp16 hi / lo registers of the next A in
+//     place -- no operand planes, no accumulator store, no handshakes inside a unit's chain.
+//   * the numerics are those of the two-tile store engine this replaces: operands pre-scaled by H_SA / H_SW and split
+//     hi / lo with round-to-nearest; K = 64 chunks, each started with scale-d = 0 (the tensor core truncates while it
+//     accumulates), summed with __fadd_rn in chunk order; the same product order inside a chunk (per K = 32 slab
+//     lo*W_hi and hi*W_lo for both k-steps, then hi*W_hi); the same epilogue arithmetic per element.
+//   * the fp32 skip / residual rows and then the e2 tile live in a [64][R_LDS] fp32 tile per consumer in shared memory;
+//     a thread touches only its own fragment elements there until e2 is summed by column.  Every output (e1, x_ji,
+//     x_down) is stored straight from the fragment: one warp store covers 8 rows x 32 bytes, whole sectors.
+//   * persistent grid of min(SMs, units / 2) CTAs: consumer w of CTA b takes units b + (2 k + w) gridDim.x, so the
+//     units beyond the last full round of pairs go to different SMs instead of a whole second CTA wave.
+constexpr int R_UNIT = 64;              // edges per consumer unit: the M of one wgmma
+constexpr int R_STAGES = 8;             // two K = 128, N = 128 layers: one consumer may hold a layer the other has left
+constexpr int R_LDS = 136;              // row stride (floats) of a consumer tile: 8-byte fragment accesses are conflict free
+constexpr int R_WG = 128;
+constexpr int R_THREADS = 3 * R_WG;     // producer warpgroup + two consumer warpgroups
+// setmaxnreg: the kernel is compiled for 168 registers (384 threads); the producer drops to 40 and the consumers grow to
+// 232 (128 x 40 + 256 x 232 <= 64 K): a consumer holds the A operand (64), the chunk-0 and chunk-1 accumulators (2 x 64).
+__device__ __forceinline__ void r_regs_producer() { asm volatile("setmaxnreg.dec.sync.aligned.u32 40;"); }
+__device__ __forceinline__ void r_regs_consumer() { asm volatile("setmaxnreg.inc.sync.aligned.u32 232;"); }
+
+struct RSmem {
+  unsigned char w[R_STAGES][H_STAGE_BYTES];
+  float tile[2][R_UNIT * R_LDS];        // per consumer: skip / residual rows (x H_SA), then e2
+  float rbf[2][R_UNIT * 6];             // per consumer: rbf0 rows of its unit
+  float bias[8][128];                   // part B biases (x H_SA)
+  float bias_a[2][128];                 // part A: b_ji (x 1), b_kj (x H_SA)
+  float wr[128 * 8];                    // part B: lin_rbf [128][6] padded to 8
+  float wr1[64];                        // part A: lin_rbf1 [8][6] padded to 8
+  float wr2[128 * 8];                   // part A: lin_rbf2 [128][8]
+  int dst[2][R_UNIT];
+  uint64_t full[R_STAGES], empty[R_STAGES];
+};
+static_assert(sizeof(RSmem) <= 227 * 1024, "RSmem exceeds the shared memory of an SM");
+
+enum { RE_B = 0, RE_BA = 1, RE_A = 2 };   // part B; part B + part A of the next block; part A
+struct REParams {
+  HGemm g[11];                          // B: lin_up, res0.lin1, res0.lin2, lin, res1.lin1, res1.lin2, res2.lin1, res2.lin2
+                                        // BA: + lin_ji, lin_kj, lin_down of the NEXT block;  A: lin_ji, lin_kj, lin_down
+  const float* w_rbf;                   // B: lin_rbf [128, 6]
+  const float *w_rbf1, *w_rbf2;         // A: lin_rbf1 [8, 6], lin_rbf2 [128, 8] (BA: of the next block)
+  float *x_ji, *x_down;                 // A: outputs (BA: of the next block)
 };
 
-// FUSE: part A of the NEXT interaction block (x_ji = act(lin_ji(e1)), x_kj = act(lin_kj(e1)) * gate,
-// x_down = act(lin_down(x_kj)); spherenet.py:154-161) is appended to this block's chain: its operand is the e1 tile
-// this kernel has just produced, so the three extra jobs continue on the same tiles -- one launch, one set-up and
-// one e1 read less per block (part A alone is 34 us for 2.5 layers, two thirds of it set-up and tail).
-template <bool FAST, bool FUSE>
-__global__ void __launch_bounds__(H_THREADS, 1)
-sphere_update_e_b_h16_kernel(const float* __restrict__ m, const float* __restrict__ x_ji,
-                             const float* __restrict__ e1_in, const float* __restrict__ rbf0,
-                             const int32_t* __restrict__ dst, int n_edges, HBParams P, float* __restrict__ e1_out,
-                             float* __restrict__ v_in) {
-  extern __shared__ __align__(1024) unsigned char h_raw[];
-  HSmem& s = *reinterpret_cast<HSmem*>(h_raw);
-  const int tid = threadIdx.x, warp = tid >> 5;
-  const int n_tiles = (n_edges + H_M - 1) / H_M, tile0 = blockIdx.x * 2, ntile = min(2, n_tiles - tile0);
-  if (tid == 0 && g_h16_trace_on && blockIdx.x == 0) { g_h16_trace[100] = clock64(); g_h16_trace[101] = (long long)global_ns(); }
-  HTileRegs<8> m_regs;                              // the m tile (K = 64) of this thread's tile, in flight during set-up
-  if (warp >= H_CTRL_WARPS) {
-    const int t = (warp - H_CTRL_WARPS) / H_TILE_WARPS, et = tid - H_CTRL_THREADS - t * H_TILE_THREADS;
-    const int e0 = (tile0 + t) * H_M;
-    if (t < ntile) h_tile_fetch<8>(m_regs, et, m + (size_t)e0 * 64, 64, min(H_M, n_edges - e0));
-  }
-  h_setup(s);
-  for (int i = tid; i < 8 * 128; i += H_THREADS) {
-    const float* b = P.g[i / 128].bias;
-    s.bias[i / 128][i % 128] = b ? H_SA * __ldg(b + i % 128) : 0.f;          // the chain runs pre-scaled by H_SA
-  }
-  for (int i = tid; i < 128 * 8; i += H_THREADS) s.wr[i] = (i % 8 < 6) ? __ldg(P.w_rbf + (i / 8) * 6 + i % 8) : 0.f;
-  for (int i = tid; i < 2 * H_M; i += H_THREADS) {
-    const int e = (tile0 + i / H_M) * H_M + i % H_M;
-    s.dst[i / H_M][i % H_M] = (e < n_edges) ? dst[e] : -1;
-  }
-  if (FUSE) {
-    for (int i = tid; i < 2 * 128; i += H_THREADS)     // lin_ji's output leaves unscaled, lin_kj's feeds an operand (x H_SA)
-      s.bias2[i / 128][i % 128] = (i / 128 ? H_SA : 1.0f) * __ldg(P.g[8 + i / 128].bias + i % 128);
-    for (int i = tid; i < 128 * 8; i += H_THREADS) s.wr2[i] = __ldg(P.n_w_rbf2 + i);      // [128][8]
-    for (int i = tid; i < 64; i += H_THREADS) s.wr1[i] = (i % 8 < 6) ? __ldg(P.n_w_rbf1 + (i / 8) * 6 + i % 8) : 0.f;
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  if (tid == 0 && g_h16_trace_on && blockIdx.x == 0) g_h16_trace[104] = clock64();
-  HCtx c;
-  bool epi = false;
-  constexpr int NG = FUSE ? 11 : 8;
-  if (warp < H_CTRL_WARPS) {
-    h_regs_ctrl();
-    h_mma_n<true, false>(s, P.g, NG, ntile, s.tmem_base);
-  } else if (h_regs_epi(), (c = h_ctx(s, ntile)).t < ntile) {
-    epi = true;
-    constexpr bool TRACE = true;
-    const bool probe = c.et == 0;
-    if (probe && c.t == 0) H_TRACE(105);
-    const int e0 = (tile0 + c.t) * H_M, rows = min(H_M, n_edges - e0);
-    const bool valid = c.row < rows;
-    const size_t ge = (size_t)(e0 + c.row);
-    const int col0 = c.half * 64;
-    const uint32_t stash = c.tl + 256u + 128u * c.t + col0;
-    // The fp32 skip rows (x_ji for q = 0, e1_in for q = 3) are fetched into the stash while this thread would
-    // otherwise wait for its tile's MMAs, so no global load sits on the critical path of an epilogue.
-    auto prefetch_skip = [&](const float* __restrict__ src) {
-      const float* gsrc = src + ge * 128 + col0;
+__device__ __forceinline__ void r_bar(int cw) { asm volatile("bar.sync %0, %1;" ::"r"(1 + cw), "n"(R_WG) : "memory"); }
+// 4 / 8-byte asynchronous copies global -> shared; a source size of 0 writes zeros (rows past the last edge)
+__device__ __forceinline__ void cp_async4(void* sm, const void* g, bool valid) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(smem_u32(sm)), "l"(g), "r"(valid ? 4 : 0) : "memory");
+}
+__device__ __forceinline__ void cp_async8(void* sm, const void* g, bool valid) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 8, %2;" ::"r"(smem_u32(sm)), "l"(g), "r"(valid ? 8 : 0) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
+
+// A pair of consecutive K elements, ALREADY multiplied by H_SA -> fp16 hi / lo registers (the split of h_store_ku).
+__device__ __forceinline__ void r_split(float x0, float x1, uint32_t& hi, uint32_t& lo) {
+  const __half2 hh = __floats2half2_rn(x0, x1);
+  const float2 hf = __half22float2(hh);
+  const __half2 ll = __floats2half2_rn(x0 - hf.x, x1 - hf.y);
+  hi = *reinterpret_cast<const uint32_t*>(&hh);
+  lo = *reinterpret_cast<const uint32_t*>(&ll);
+}
+struct RA { uint32_t hi[8][4], lo[8][4]; };   // register A operand of a K <= 128 layer: [k-step][register]
+// activated m64n128 fragment (x H_SA) -> A operand of the next layer
+__device__ __forceinline__ void r_acc_to_a(const float (&v)[64], RA& a, float scale = 1.0f) {
 #pragma unroll
-      for (int p = 0; p < 4; ++p) {
-        uint32_t r[16];
+  for (int s = 0; s < 8; ++s)
 #pragma unroll
-        for (int i = 0; i < 16; i += 4) {
-          const float4 x = valid ? __ldg(reinterpret_cast<const float4*>(gsrc + 16 * p + i)) : make_float4(0, 0, 0, 0);
-          r[i] = __float_as_uint(x.x * H_SA); r[i + 1] = __float_as_uint(x.y * H_SA);
-          r[i + 2] = __float_as_uint(x.z * H_SA); r[i + 3] = __float_as_uint(x.w * H_SA);
-        }
-        tmem_st16(stash + 16 * p, r);
-      }
-      tmem_st_wait();
-    };
-    // A0 = m tile (K = 64), fetched before the set-up barrier
-    h_tile_commit<8>(s, c, m_regs);
-    if (probe && c.t == 0) H_TRACE(106);
-    h_epi_done(s, c.t);
-    if (probe && c.t == 0) H_TRACE(107);
-    prefetch_skip(x_ji);
-    if (probe && c.t == 0) H_TRACE(108);
-    // The eight epilogues of the chain (spherenet.py:172-179); stash = the fp32 skip / residual row (x H_SA):
-    //   q=0: h = stash(x_ji) + act(lin_up(m))                -> A, stash
-    //   q=1,4,6: t = act(lin1(h))                            -> A
-    //   q=2,5: h = stash + act(lin2(t))                      -> A, stash      (q=2: then stash <- e1_in)
-    //   q=3: h = act(lin(h)) + stash(e1_in)                  -> A, stash
-    //   q=7: h = stash + act(lin2(t))                        -> e1_out, e2 tile
-    float acc_final[64];
-#pragma unroll 1
-    for (int q = 0; q < 8; ++q) {
-      float (&acc)[64] = acc_final;
-      if (probe) H_TRACE(32 + c.t * 32 + q * 4);
-      h_drain<4, true>(s, c, col0, q == 0 ? 1 : 2, acc);
-      if (probe) H_TRACE(32 + c.t * 32 + q * 4 + 1);
-      const bool add_stash = (q == 0 || q == 2 || q == 3 || q == 5 || q == 7);
-      const bool to_stash = (q == 0 || q == 3 || q == 5);
-      float rb[6];
-      if (q == 7) {
+    for (int r = 0; r < 4; ++r) r_split(v[frag_a_src(s, r)] * scale, v[frag_a_src(s, r) + 1] * scale, a.hi[s][r], a.lo[s][r]);
+}
+// rows [0, rows) of a row-major fp32 [64 x 16 KS] tile (leading dimension ld) -> A operand (x H_SA); other rows zero
+template <int KS>
+__device__ __forceinline__ void r_load_a(RA& a, const float* __restrict__ g, int ld, int rows, int wt) {
 #pragma unroll
-        for (int n = 0; n < 6; ++n) rb[n] = valid ? __ldg(rbf0 + ge * 6 + n) : 0.f;
-      }
+  for (int s = 0; s < KS; ++s)
 #pragma unroll
-      for (int p = 0; p < 4; ++p) {
-        const int col = col0 + 16 * p;
-        uint32_t r[16];
-        if (add_stash) tmem_ld16(stash + 16 * p, r);           // in flight under the 16 activations below
-        float* v = &acc[16 * p];                               // in place: v8 = H_SA * act(.)
-#pragma unroll
-        for (int i = 0; i < 16; i += 4) {
-          const float4 b = *reinterpret_cast<const float4*>(&s.bias[q][col + i]);
-          v[i] = hswish8<FAST>(fmaf(v[i], H_SA * H_INV, b.x));
-          v[i + 1] = hswish8<FAST>(fmaf(v[i + 1], H_SA * H_INV, b.y));
-          v[i + 2] = hswish8<FAST>(fmaf(v[i + 2], H_SA * H_INV, b.z));
-          v[i + 3] = hswish8<FAST>(fmaf(v[i + 3], H_SA * H_INV, b.w));
-        }
-        if (add_stash) {
-          tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 16; ++i) v[i] += __uint_as_float(r[i]);
-        }
-        if (q < 7) {
-          if (to_stash) {
-#pragma unroll
-            for (int i = 0; i < 16; ++i) r[i] = __float_as_uint(v[i]);
-            tmem_st16(stash + 16 * p, r);
-          }
-          float v16[16];
-#pragma unroll
-          for (int i = 0; i < 16; ++i) v16[i] = v[i];
-          h_store_a16(s, c, col, v16);
-        } else {
-          // e1 (unscaled, kept in the accumulator registers for the coalesced store below) and
-          // e2 = lin_rbf(rbf0) * e1, staged as a [128][H_LDS] tile over this tile's planes (all its MMAs are done)
-          float* e2t = reinterpret_cast<float*>(s.a[c.t][0]);
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            const float o = v[i] * (1.0f / H_SA);
-            c.bad |= !h_finite(o);
-            const float4 w0 = *reinterpret_cast<const float4*>(s.wr + (col + i) * 8);
-            const float2 w1 = *reinterpret_cast<const float2*>(s.wr + (col + i) * 8 + 4);
-            const float gsum = fmaf(w1.y, rb[5], fmaf(w1.x, rb[4], fmaf(w0.w, rb[3], fmaf(w0.z, rb[2],
-                               fmaf(w0.y, rb[1], w0.x * rb[0])))));
-            e2t[c.row * H_LDS + col + i] = gsum * o;
-            v[i] = o;
-          }
-        }
-      }
-      if (probe) H_TRACE(32 + c.t * 32 + q * 4 + 2);
-      if (q < 7) {
-        if (to_stash) tmem_st_wait();
-        h_epi_done(s, c.t);
-        if (q == 2) prefetch_skip(e1_in);     // the stash was consumed above; q = 3 adds e1_in from it
-      }
-      if (probe) H_TRACE(32 + c.t * 32 + q * 4 + 3);
+    for (int r = 0; r < 4; ++r) {
+      const int row = frag_a_row(wt, r), col = frag_a_col(wt, s, r);
+      const float2 x = row < rows ? __ldg(reinterpret_cast<const float2*>(g + (size_t)row * ld + col)) : make_float2(0.f, 0.f);
+      r_split(x.x * H_SA, x.y * H_SA, a.hi[s][r], a.lo[s][r]);
     }
-    h_tile_bar(c.t);
-    h_segment_sums(s, c, rows, v_in);   // spherenet.py:211
-    h_tile_bar(c.t);
-    h_store_tile_coalesced<128>(s, c, col0, acc_final, e1_out + (size_t)e0 * 128, rows);
-    if (probe) H_TRACE(96 + c.t);
-    if (FUSE) {
-      // ---- part A of the next block on the e1 tile still in this thread's registers
-      h_tile_bar(c.t);                               // every thread of the tile has read the staging overlay
+}
+// fp32 rows of a [E, 128] tensor -> this thread's fragment elements of the consumer tile (unscaled; zeros past `rows`)
+__device__ __forceinline__ void r_fetch_rows(float* tile, const float* __restrict__ src, int rows, int fr, int fc) {
 #pragma unroll
-      for (int p = 0; p < 4; ++p) {
-        float v16[16];
+  for (int j = 0; j < 16; ++j)
 #pragma unroll
-        for (int i = 0; i < 16; ++i) v16[i] = acc_final[16 * p + i] * H_SA;
-        h_store_a16(s, c, col0 + 16 * p, v16);
-      }
-      float r8[8];                                   // gate coefficients of this row: lin_rbf1(rbf0[row])   spherenet.py:157
-      {
-        float rb[6];
-#pragma unroll
-        for (int n = 0; n < 6; ++n) rb[n] = valid ? __ldg(rbf0 + ge * 6 + n) : 0.f;
-#pragma unroll
-        for (int mm = 0; mm < 8; ++mm) {
-          float a = 0.f;
-#pragma unroll
-          for (int n = 0; n < 6; ++n) a = fmaf(s.wr1[mm * 8 + n], rb[n], a);
-          r8[mm] = a;
-        }
-      }
-      h_epi_done(s, c.t);
-      float (&acc)[64] = acc_final;
-      // G0: x_ji = act(lin_ji(e1))                                                spherenet.py:154
-      h_drain<4, true>(s, c, col0, 2, acc);
-      h_epi_done(s, c.t);   // the operand (= e1) is reused unchanged by lin_kj
-      if (valid) {
-#pragma unroll
-        for (int i = 0; i < 64; i += 4) {
-          const float4 b = *reinterpret_cast<const float4*>(&s.bias2[0][col0 + i]);
-          float4 o;
-          o.x = hswish<FAST>(fmaf(acc[i], H_INV, b.x));
-          o.y = hswish<FAST>(fmaf(acc[i + 1], H_INV, b.y));
-          o.z = hswish<FAST>(fmaf(acc[i + 2], H_INV, b.z));
-          o.w = hswish<FAST>(fmaf(acc[i + 3], H_INV, b.w));
-          *reinterpret_cast<float4*>(P.n_x_ji + ge * 128 + col0 + i) = o;
-        }
-      }
-      // G1: x_kj = act(lin_kj(e1)) * lin_rbf2(r8)                                 spherenet.py:155-159
-      h_drain<4, true>(s, c, col0, 2, acc);
-#pragma unroll
-      for (int p = 0; p < 4; ++p) {
-        float v[16];
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          const int col = col0 + 16 * p + i;
-          const float4 w0 = *reinterpret_cast<const float4*>(s.wr2 + col * 8);
-          const float4 w1 = *reinterpret_cast<const float4*>(s.wr2 + col * 8 + 4);
-          const float gate = fmaf(w1.w, r8[7], fmaf(w1.z, r8[6], fmaf(w1.y, r8[5], fmaf(w1.x, r8[4],
-                             fmaf(w0.w, r8[3], fmaf(w0.z, r8[2], fmaf(w0.y, r8[1], w0.x * r8[0])))))));
-          v[i] = hswish8<FAST>(fmaf(acc[16 * p + i], H_SA * H_INV, s.bias2[1][col])) * gate;
-        }
-        h_store_a16(s, c, col0 + 16 * p, v);
-      }
-      h_epi_done(s, c.t);
-      // G2: x_down = act(lin_down(x_kj)), N = 64                                  spherenet.py:161
-      {
-        const int col = c.half * 32;
-        float a32[32];
-        h_drain<2, true>(s, c, col, 2, a32);
-#pragma unroll
-        for (int i = 0; i < 32; ++i) a32[i] = hswish<FAST>(a32[i] * H_INV);
-        h_store_tile_coalesced<64>(s, c, col, a32, P.n_x_down + (size_t)e0 * 64, rows);   // all MMAs of the tile are done
-      }
+    for (int h = 0; h < 2; ++h) {
+      const int row = fr + 8 * h, col = 8 * j + fc;
+      cp_async8(tile + row * R_LDS + col, src + (size_t)(row < rows ? row : 0) * 128 + col, row < rows);
     }
-  }
-  h_finish(s, epi ? &c : nullptr);
-  if (tid == 0 && g_h16_trace_on && blockIdx.x == 0) { g_h16_trace[102] = clock64(); g_h16_trace[103] = (long long)global_ns(); }
+  cp_async_commit();
 }
 
-// ---------------------------------------------------------------------------------- update_e part B (+ A), wide epilogue
-// Same chain, same jobs, same barriers as sphere_update_e_b_h16_kernel; the difference is WHO runs an epilogue.  There,
-// eight warps own a tile (64 columns per thread) and a tile's job cycle is its MMAs (~3.6 k cycles) PLUS its epilogue
-// (~5 k: 2 k of MUFU and 1.8 k of FP32 pipe per scheduler on two warps) -- the other tile fills the gaps and the tensor
-// pipe still idles a quarter of the time (DESIGN.md 4.5).  Here all SIXTEEN epilogue warps serve the tile whose
-// accumulators are ready (32 columns per thread, four warps per scheduler), then the other tile: an epilogue takes about
-// half as long, MMA(X, q+1) can follow MMA(Y, q) immediately, and the cycle becomes MMA-issue bound.  A thread walks the
-// jobs in the issuer's order (q, tile 0), (q, tile 1), (q + 1, tile 0), ...; nothing but barrier phases is kept per tile.
-constexpr int X_WARPS = 2 * H_TILE_WARPS;         // epilogue warps, all on one tile at a time
-constexpr int X_THREADS = X_WARPS * 32;
-
-struct XCtx {
-  int e, row, slice;        // index among the 512 epilogue threads, row of the tile, 32-column slice
-  uint32_t tl;              // accumulator-store address of this warp's row quarter, column 0
-  int ch;                   // accumulator-chunk counter (the issuer's sequence: q major, tile minor)
-  int use[2][2];            // chunks drained so far per [tile][accumulator]: barrier phases
-  bool bad;
-};
-__device__ __forceinline__ void x_bar() { asm volatile("bar.sync 1, %0;" ::"n"(X_THREADS) : "memory"); }
-__device__ __forceinline__ void x_epi_done(HSmem& s, int t) {
-  fence_async_smem();
-  tc_fence_before();
+// ---- weight ring, consumer side: `it` counts the slabs of the producer's sequence this consumer has passed
+__device__ __forceinline__ void r_release(RSmem& s, int it, int n) {   // the MMAs reading slabs it .. it + n - 1 are done
   __syncwarp();
-  if ((threadIdx.x & 31) == 0) mbar_arrive(&s.a_ready[t]);
+  if ((threadIdx.x & 31) == 0)
+    for (int i = 0; i < n; ++i) mbar_arrive(&s.empty[(it + i) % R_STAGES]);   // one arrival per consumer warp
 }
-// one k-unit (8 consecutive K elements, already x H_SA) of row `row` of tile t -> fp16 hi / lo planes
-__device__ __forceinline__ void x_store_ku(HSmem& s, int t, int row, int ku, const float (&x)[8]) {
-  uint32_t h[4], l[4];
+// chunk CH (K = 64: slabs it + 2 CH, + 1) of a layer with N output columns into t, the slab's corrections (2^-11 of the
+// main term) first, then its two hi*hi steps; the first product starts the chunk (scale-d = 0)
+template <int CH, int N>
+__device__ __forceinline__ void r_chunk(RSmem& s, const RA& a, float (&t)[N / 2], int it) {
 #pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const __half2 hh = __floats2half2_rn(x[2 * i], x[2 * i + 1]);
-    const float2 hf = __half22float2(hh);
-    const __half2 ll = __floats2half2_rn(x[2 * i] - hf.x, x[2 * i + 1] - hf.y);
-    h[i] = *reinterpret_cast<const uint32_t*>(&hh);
-    l[i] = *reinterpret_cast<const uint32_t*>(&ll);
-  }
-  const int o = (ku * H_AKU + row) * 16;
-  *reinterpret_cast<uint4*>(s.a[t][0] + o) = make_uint4(h[0], h[1], h[2], h[3]);
-  *reinterpret_cast<uint4*>(s.a[t][1] + o) = make_uint4(l[0], l[1], l[2], l[3]);
-}
-__device__ __forceinline__ void x_store_a16(HSmem& s, const XCtx& c, int t, int col, const float (&v8)[16]) {
-  float x[8];
+  for (int sl = 0; sl < 2; ++sl) {
+    const uint32_t w_hi = smem_u32(s.w[(it + 2 * CH + sl) % R_STAGES]), w_lo = w_hi + 4u * N * 16u;
 #pragma unroll
-  for (int u = 0; u < 2; ++u) {
-#pragma unroll
-    for (int i = 0; i < 8; ++i) x[i] = v8[8 * u + i];
-    x_store_ku(s, t, c.row, (col >> 3) + u, x);
-  }
-}
-// chunks of job (q, t) -> fp32 registers (round-to-nearest adds), NP 16-column pieces from column col0
-template <int NP>
-__device__ __forceinline__ void x_drain(HSmem& s, XCtx& c, int t, int col0, int chunks, float (&acc)[NP * 16]) {
-  for (int k = 0; k < chunks; ++k, ++c.ch) {
-    const int ab = c.ch & 1;
-    mbar_wait(&s.d_ready[t][ab], c.use[t][ab] & 1);
-    ++c.use[t][ab];
-    tc_fence_after();
-    const uint32_t ta = c.tl + 128u * ab + col0;
-    if (k == 0) {
-#pragma unroll
-      for (int p = 0; p < NP; ++p) tmem_ld16f(ta + 16 * p, &acc[p * 16]);
-      tmem_ld_wait();
-    } else {
-#pragma unroll
-      for (int p = 0; p < NP; ++p) {
-        uint32_t r[16];
-        tmem_ld16(ta + 16 * p, r);
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 16; ++i) acc[p * 16 + i] = __fadd_rn(acc[p * 16 + i], __uint_as_float(r[i]));
-      }
+    for (int ks = 0; ks < 2; ++ks) {
+      const int k = 4 * CH + 2 * sl + ks;
+      const uint32_t b_off = (uint32_t)(ks * 2 * N * 16);
+      mma_f16_rs(t, a.lo[k], smem_desc(w_hi + b_off, N * 16, 128), (sl | ks) != 0);
+      mma_f16_rs(t, a.hi[k], smem_desc(w_lo + b_off, N * 16, 128), 1);
     }
-    tc_fence_before();
-    __syncwarp();
-    if ((threadIdx.x & 31) == 0) mbar_arrive(&s.d_free[t][ab]);
-  }
-}
-// [rows x W] fp32 tile of tile t (every thread holds W / 4 values of its row from column col0) -> full-line stores
-template <int W>
-__device__ __forceinline__ void x_store_tile_coalesced(HSmem& s, const XCtx& c, int t, int col0, const float (&v)[W / 4],
-                                                       float* __restrict__ out, int rows) {
-  constexpr int LD = W + 1, RPW = 128 / W;
-  float* st = reinterpret_cast<float*>(s.a[t][0]);
 #pragma unroll
-  for (int i = 0; i < W / 4; ++i) st[c.row * LD + col0 + i] = v[i];
-  x_bar();
-  const int w = c.e >> 5, lane = c.e & 31;
-  for (int r0 = w * RPW; r0 < rows; r0 += X_WARPS * RPW) {
-    const int r = r0 + (RPW == 2 ? (lane >> 4) : 0), c4 = 4 * (RPW == 2 ? (lane & 15) : lane);
-    if (r < rows) {
-      const float* src = st + r * LD + c4;
-      *reinterpret_cast<float4*>(out + (size_t)r * W + c4) = make_float4(src[0], src[1], src[2], src[3]);
-    }
+    for (int ks = 0; ks < 2; ++ks)
+      mma_f16_rs(t, a.hi[4 * CH + 2 * sl + ks], smem_desc(w_hi + (uint32_t)(ks * 2 * N * 16), N * 16, 128), 1);
   }
 }
-// e2 tile of tile t (staged [128][H_LDS] over its planes) -> edge -> node sums: one column and one 32-row quarter per thread
-__device__ __forceinline__ void x_segment_sums(const HSmem& s, const XCtx& c, int t, int rows, float* __restrict__ v_in) {
-  const int col = c.e & 127, r0 = (c.e >> 7) * 32, r1 = min(rows, r0 + 32);
-  if (r0 >= r1) return;
-  const float* e2t = reinterpret_cast<const float*>(s.a[t][0]);
-  const int* dst = s.dst[t];
+// one layer (K = 64 NCH): chunk 0 -> acc, chunk 1 -> d; r_complete waits, frees the slabs and adds d to acc
+template <int NCH, int N>
+__device__ __forceinline__ void r_issue(RSmem& s, const RA& a, float (&acc)[N / 2], float (&d)[N / 2], int it) {
+#pragma unroll
+  for (int i = 0; i < 2 * NCH; ++i) mbar_wait(&s.full[(it + i) % R_STAGES], ((it + i) / R_STAGES) & 1);
+  wg_fence();
+  r_chunk<0, N>(s, a, acc, it);
+  if (NCH == 2) r_chunk<1, N>(s, a, d, it);
+  wg_commit();
+}
+template <int NCH, int N>
+__device__ __forceinline__ void r_complete(RSmem& s, float (&acc)[N / 2], const float (&d)[N / 2], int& it) {
+  wg_wait0();
+  r_release(s, it, 2 * NCH);
+  it += 2 * NCH;
+  if (NCH == 2) {
+#pragma unroll
+    for (int i = 0; i < N / 2; ++i) acc[i] = __fadd_rn(acc[i], d[i]);
+  }
+}
+// a consumer without a unit in this round still passes every slab of it (the ring counts both consumers per stage)
+__device__ __forceinline__ void r_skip(RSmem& s, int& it, int n) {
+  for (int i = 0; i < n; ++i, ++it) {
+    mbar_wait(&s.full[it % R_STAGES], (it / R_STAGES) & 1);
+    r_release(s, it, 1);
+  }
+}
+
+// e2 of a unit (staged [64][R_LDS] fp32) -> edge -> node sums; thread = column, rows in order.  Rows are target-sorted:
+// a segment touching the first or last row of the unit may continue in a neighbouring unit and is added with an
+// atomic, interior segments are plain stores (v_in is zeroed before the launch).  Every node's in-edge segment is split
+// across at most two writers: the radius graph caps the in-degree at 32, so a segment spans at most two 64-row units,
+// and two atomicAdds onto zero commute (0 + a + b == 0 + b + a) -- the sums are deterministic.
+__device__ __forceinline__ void r_segment_sums(const float* tile, const int* dst, int rows, int col,
+                                               float* __restrict__ v_in) {
   float run = 0.f;
-  int cur = dst[r0];
+  int cur = dst[0];
   bool first = true;
-  for (int r = r0; r < r1; ++r) {
+  for (int r = 0; r < rows; ++r) {
     const int d = dst[r];
     if (d != cur) {
       if (first) atomicAdd(v_in + (size_t)cur * 128 + col, run);
       else v_in[(size_t)cur * 128 + col] = run;
       first = false; run = 0.f; cur = d;
     }
-    run += e2t[r * H_LDS + col];
+    run += tile[r * R_LDS + col];
   }
   atomicAdd(v_in + (size_t)cur * 128 + col, run);
 }
 
-template <bool FAST, bool FUSE>
-__global__ void __launch_bounds__(H_THREADS, 1)
-sphere_update_e_b_x16_kernel(const float* __restrict__ m, const float* __restrict__ x_ji,
-                             const float* __restrict__ e1_in, const float* __restrict__ rbf0,
-                             const int32_t* __restrict__ dst, int n_edges, HBParams P, float* __restrict__ e1_out,
-                             float* __restrict__ v_in) {
+// MODE = RE_B: part B of a block; RE_BA: part B of block l, then part A of block l + 1 on the e1 fragment still in
+// registers (one launch, one e1 read less per block); RE_A: part A on e1 read from memory (layer 0).  Per element the
+// three compute what the store engine computed, so RE_BA == RE_B followed by RE_A bit for bit.
+template <bool FAST, int MODE>
+__global__ void __launch_bounds__(R_THREADS, 1)
+sphere_update_e_h16_kernel(const float* __restrict__ m, const float* __restrict__ x_ji,
+                           const float* __restrict__ e1_in, const float* __restrict__ rbf0,
+                           const int32_t* __restrict__ dst, int n_edges, REParams P, float* __restrict__ e1_out,
+                           float* __restrict__ v_in) {
+  constexpr int NG = MODE == RE_B ? 8 : MODE == RE_BA ? 11 : 3;   // layers per unit
   extern __shared__ __align__(1024) unsigned char h_raw[];
-  HSmem& s = *reinterpret_cast<HSmem*>(h_raw);
-  const int tid = threadIdx.x, warp = tid >> 5;
-  const int n_tiles = (n_edges + H_M - 1) / H_M, tile0 = blockIdx.x * 2, ntile = min(2, n_tiles - tile0);
-  // the m tiles (K = 64: 8 k-units per row) of both tiles, in flight during the set-up: 2 (row, k-unit) items per tile
-  float4 mreg[2][2][2];
-  if (warp >= H_CTRL_WARPS) {
-    const int e = tid - H_CTRL_THREADS;
-#pragma unroll
-    for (int t = 0; t < 2; ++t)
-#pragma unroll
-      for (int k = 0; k < 2; ++k) {
-        const int f = e + k * X_THREADS, row = f >> 3, ku = f & 7;
-        const int e0 = (tile0 + t) * H_M, rows = min(H_M, n_edges - e0);
-        if (t < ntile && row < rows) {
-          const float* g = m + (size_t)(e0 + row) * 64 + ku * 8;
-          mreg[t][k][0] = __ldg(reinterpret_cast<const float4*>(g));
-          mreg[t][k][1] = __ldg(reinterpret_cast<const float4*>(g + 4));
-        } else {
-          mreg[t][k][0] = mreg[t][k][1] = make_float4(0.f, 0.f, 0.f, 0.f);
-        }
-      }
+  RSmem& s = *reinterpret_cast<RSmem*>(h_raw);
+  const int tid = threadIdx.x, wg = tid / R_WG;
+  // (values live across setmaxnreg are recomputed after it: a register carried over would be spilled)
+  auto n_units = [&]() { return (n_edges + R_UNIT - 1) / R_UNIT; };
+  auto rounds = [&]() {   // units of consumer 0
+    return (n_units() - (int)blockIdx.x + 2 * (int)gridDim.x - 1) / (2 * (int)gridDim.x);
+  };
+  const bool trace = g_h16_trace_on && blockIdx.x == 0;
+  if (tid == 0 && trace) { g_h16_trace[100] = clock64(); g_h16_trace[101] = (long long)global_ns(); }
+  if (tid == 0) {
+    for (int i = 0; i < R_STAGES; ++i) { mbar_init(&s.full[i], 1); mbar_init(&s.empty[i], 8); }
+    mbar_fence_init();
   }
-  h_setup(s, X_WARPS, X_WARPS);
-  for (int i = tid; i < 8 * 128; i += H_THREADS) {
-    const float* b = P.g[i / 128].bias;
-    s.bias[i / 128][i % 128] = b ? H_SA * __ldg(b + i % 128) : 0.f;          // the chain runs pre-scaled by H_SA
+  if (MODE != RE_A) {
+    for (int i = tid; i < 8 * 128; i += R_THREADS) {
+      const float* b = P.g[i / 128].bias;
+      s.bias[i / 128][i % 128] = b ? H_SA * __ldg(b + i % 128) : 0.f;          // the chain runs pre-scaled by H_SA
+    }
+    for (int i = tid; i < 128 * 8; i += R_THREADS) s.wr[i] = (i % 8 < 6) ? __ldg(P.w_rbf + (i / 8) * 6 + i % 8) : 0.f;
   }
-  for (int i = tid; i < 128 * 8; i += H_THREADS) s.wr[i] = (i % 8 < 6) ? __ldg(P.w_rbf + (i / 8) * 6 + i % 8) : 0.f;
-  for (int i = tid; i < 2 * H_M; i += H_THREADS) {
-    const int e = (tile0 + i / H_M) * H_M + i % H_M;
-    s.dst[i / H_M][i % H_M] = (e < n_edges) ? dst[e] : -1;
+  if (MODE != RE_B) {
+    constexpr int GA = MODE == RE_A ? 0 : 8;
+    for (int i = tid; i < 2 * 128; i += R_THREADS)     // lin_ji's output leaves unscaled, lin_kj's feeds an operand (x H_SA)
+      s.bias_a[i / 128][i % 128] = (i / 128 ? H_SA : 1.0f) * __ldg(P.g[GA + i / 128].bias + i % 128);
+    for (int i = tid; i < 128 * 8; i += R_THREADS) s.wr2[i] = __ldg(P.w_rbf2 + i);
+    for (int i = tid; i < 64; i += R_THREADS) s.wr1[i] = (i % 8 < 6) ? __ldg(P.w_rbf1 + (i / 8) * 6 + i % 8) : 0.f;
   }
-  if (FUSE) {
-    for (int i = tid; i < 2 * 128; i += H_THREADS)     // lin_ji's output leaves unscaled, lin_kj's feeds an operand (x H_SA)
-      s.bias2[i / 128][i % 128] = (i / 128 ? H_SA : 1.0f) * __ldg(P.g[8 + i / 128].bias + i % 128);
-    for (int i = tid; i < 128 * 8; i += H_THREADS) s.wr2[i] = __ldg(P.n_w_rbf2 + i);      // [128][8]
-    for (int i = tid; i < 64; i += H_THREADS) s.wr1[i] = (i % 8 < 6) ? __ldg(P.n_w_rbf1 + (i / 8) * 6 + i % 8) : 0.f;
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  constexpr int NG = FUSE ? 11 : 8;
-  XCtx c;
-  bool epi = false;
-  if (warp < H_CTRL_WARPS) {
-    h_regs_ctrl();
-    h_mma_n<false, false>(s, P.g, NG, ntile, s.tmem_base);
-  } else {
-    h_regs_epi();
-    epi = true;
-    const int lane = tid & 31, ew = warp - H_CTRL_WARPS, quarter = warp & 3;
-    c.e = tid - H_CTRL_THREADS; c.row = 32 * quarter + lane; c.slice = ew >> 2;
-    c.tl = s.tmem_base + ((uint32_t)(32 * quarter) << 16);
-    c.ch = 0; c.use[0][0] = c.use[0][1] = c.use[1][0] = c.use[1][1] = 0; c.bad = false;
-    const int col0 = 32 * c.slice;
-    // skip rows (x_ji for q = 0, e1_in for q = 3) -> stash of tile t, x H_SA
-    auto prefetch_skip = [&](const float* __restrict__ src, int t) {
-      const int e0 = (tile0 + t) * H_M;
-      const bool valid = c.row < min(H_M, n_edges - e0);
-      const float* gsrc = src + (size_t)(e0 + c.row) * 128 + col0;
-      const uint32_t stash = c.tl + 256u + 128u * t + col0;
-#pragma unroll
-      for (int p = 0; p < 2; ++p) {
-        uint32_t r[16];
-#pragma unroll
-        for (int i = 0; i < 16; i += 4) {
-          const float4 x = valid ? __ldg(reinterpret_cast<const float4*>(gsrc + 16 * p + i)) : make_float4(0, 0, 0, 0);
-          r[i] = __float_as_uint(x.x * H_SA); r[i + 1] = __float_as_uint(x.y * H_SA);
-          r[i + 2] = __float_as_uint(x.z * H_SA); r[i + 3] = __float_as_uint(x.w * H_SA);
+  if (tid == 0 && trace) g_h16_trace[104] = clock64();
+
+  if (wg == 0) {
+    // ---- producer: every K = 32 slab of every layer, once per round (both consumers read each slab)
+    r_regs_producer();
+    if (tid == 0) {
+      int it = 0;
+      const int nr = rounds();
+      for (int k = 0; k < nr; ++k)
+        for (int q = 0; q < NG; ++q) {
+          const uint32_t bytes = 2u * 4u * (uint32_t)P.g[q].N * 16u;
+          for (int c = 0; c < P.g[q].K / H_SLAB_K; ++c, ++it) {
+            const int st = it % R_STAGES;
+            if (it >= R_STAGES) mbar_wait(&s.empty[st], ((it / R_STAGES) + 1) & 1);
+            mbar_arrive_expect_tx(&s.full[st], bytes);
+            bulk_g2s(s.w[st], P.g[q].w + (size_t)c * bytes, bytes, &s.full[st]);
+          }
         }
-        tmem_st16(stash + 16 * p, r);
-      }
-      tmem_st_wait();
-    };
-    // A0 = the m tiles
-    for (int t = 0; t < ntile; ++t) {
-#pragma unroll
-      for (int k = 0; k < 2; ++k) {
-        const int f = c.e + k * X_THREADS, row = f >> 3, ku = f & 7;
-        const float4 p0 = mreg[t][k][0], p1 = mreg[t][k][1];
-        const float x[8] = {p0.x * H_SA, p0.y * H_SA, p0.z * H_SA, p0.w * H_SA, p1.x * H_SA, p1.y * H_SA, p1.z * H_SA, p1.w * H_SA};
-        x_store_ku(s, t, row, ku, x);
-      }
-      x_epi_done(s, t);
     }
-    for (int t = 0; t < ntile; ++t) prefetch_skip(x_ji, t);
-    float acc[32];
+    return;
+  }
+
+  // ---- consumers
+  r_regs_consumer();
+  const int cw = threadIdx.x / R_WG - 1, wt = threadIdx.x & (R_WG - 1);
+  const int nu = n_units(), nr = rounds();
+  const int fr = frag_row(wt), fc = frag_col(wt);   // this thread's fragment rows fr, fr + 8 and columns 8 j + fc (+1)
+  float* tile = s.tile[cw];
+  const float* rbf = s.rbf[cw];
+  int slabs = 0;
+  for (int q = 0; q < NG; ++q) slabs += P.g[q].K / H_SLAB_K;
+  // timeline probe (tools/gpu_h16_timeline.py): CTA 0, first unit of each consumer, four points per layer
+  const bool probe = g_h16_trace_on && blockIdx.x == 0 && wt == 0;
+  int lq = 0;
+  auto tp = [&](bool on, int point) { if (on) g_h16_trace[cw * 48 + lq * 4 + point] = clock64(); };
+  bool staggered = cw == 1, bad = false;
+  auto stagger = [&]() {
+    if (!staggered) { asm volatile("bar.arrive 3, %0;" ::"n"(2 * R_WG) : "memory"); staggered = true; }
+  };
+  if (cw == 1) asm volatile("bar.sync 3, %0;" ::"n"(2 * R_WG) : "memory");   // after consumer 0's first layer is issued
+  int it = 0;
 #pragma unroll 1
-    for (int q = 0; q < 8; ++q) {
-      const bool add_stash = (q == 0 || q == 2 || q == 3 || q == 5 || q == 7);
-      const bool to_stash = (q == 0 || q == 3 || q == 5);
+  for (int k = 0; k < nr; ++k) {
+    const int unit = blockIdx.x + (2 * k + cw) * gridDim.x;
+    if (unit >= nu) { r_skip(s, it, slabs); continue; }
+    const int e0 = unit * R_UNIT, rows = min(R_UNIT, n_edges - e0);
+    const bool tr = probe && k == 0;
+    lq = 0;
+    r_bar(cw);   // the previous unit is done with tile / rbf / dst
+    for (int i = wt; i < R_UNIT * 6; i += R_WG)
+      cp_async4(&s.rbf[cw][i], rbf0 + (size_t)e0 * 6 + (i < rows * 6 ? i : 0), i < rows * 6);
+    RA a;
+    float acc[64], d[64];
+    if (MODE != RE_A) {
+      if (wt < R_UNIT) cp_async4(&s.dst[cw][wt], dst + e0 + (wt < rows ? wt : 0), wt < rows);
+      r_fetch_rows(tile, x_ji + (size_t)e0 * 128, rows, fr, fc);     // skip rows of q = 0
+      r_load_a<4>(a, m + (size_t)e0 * 64, 64, rows, wt);             // A0 = m (K = 64)
+      // The eight layers of the chain (spherenet.py:172-179), tile = the fp32 skip / residual row (x H_SA):
+      //   q=0: h = x_ji + act(lin_up(m))                       -> A, tile
+      //   q=1,4,6: t = act(lin1(h))                            -> A
+      //   q=2,5: h = tile + act(lin2(t))                       -> A, tile      (q=2: then tile <- e1_in)
+      //   q=3: h = act(lin(h)) + e1_in                         -> A, tile
+      //   q=7: e1 = tile + act(lin2(t))                        -> e1_out, e2 tile
 #pragma unroll 1
-      for (int t = 0; t < ntile; ++t) {
-        const int e0 = (tile0 + t) * H_M, rows = min(H_M, n_edges - e0);
-        const bool valid = c.row < rows;
-        const size_t ge = (size_t)(e0 + c.row);
-        const uint32_t stash = c.tl + 256u + 128u * t + col0;
-        x_drain<2>(s, c, t, col0, q == 0 ? 1 : 2, acc);
-        float rb[6];
-        if (q == 7) {
-#pragma unroll
-          for (int n = 0; n < 6; ++n) rb[n] = valid ? __ldg(rbf0 + ge * 6 + n) : 0.f;
-        }
-#pragma unroll
-        for (int p = 0; p < 2; ++p) {
-          const int col = col0 + 16 * p;
-          uint32_t r[16];
-          if (add_stash) tmem_ld16(stash + 16 * p, r);           // in flight under the 16 activations below
-          float* v = &acc[16 * p];                               // in place: v8 = H_SA * act(.)
-#pragma unroll
-          for (int i = 0; i < 16; i += 4) {
-            const float4 b = *reinterpret_cast<const float4*>(&s.bias[q][col + i]);
-            v[i] = hswish8<FAST>(fmaf(v[i], H_SA * H_INV, b.x));
-            v[i + 1] = hswish8<FAST>(fmaf(v[i + 1], H_SA * H_INV, b.y));
-            v[i + 2] = hswish8<FAST>(fmaf(v[i + 2], H_SA * H_INV, b.z));
-            v[i + 3] = hswish8<FAST>(fmaf(v[i + 3], H_SA * H_INV, b.w));
-          }
-          if (add_stash) {
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 16; ++i) v[i] += __uint_as_float(r[i]);
-          }
-          if (q < 7) {
-            if (to_stash) {
-#pragma unroll
-              for (int i = 0; i < 16; ++i) r[i] = __float_as_uint(v[i]);
-              tmem_st16(stash + 16 * p, r);
-            }
-            float v16[16];
-#pragma unroll
-            for (int i = 0; i < 16; ++i) v16[i] = v[i];
-            x_store_a16(s, c, t, col, v16);
-          } else {
-            // e1 (unscaled, kept in the accumulator registers for the coalesced store below) and e2 = lin_rbf(rbf0) * e1,
-            // staged as a [128][H_LDS] tile over this tile's planes (all its MMAs of part B are done)
-            float* e2t = reinterpret_cast<float*>(s.a[t][0]);
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              const float o = v[i] * (1.0f / H_SA);
-              c.bad |= !h_finite(o);
-              const float4 w0 = *reinterpret_cast<const float4*>(s.wr + (col + i) * 8);
-              const float2 w1 = *reinterpret_cast<const float2*>(s.wr + (col + i) * 8 + 4);
-              const float gsum = fmaf(w1.y, rb[5], fmaf(w1.x, rb[4], fmaf(w0.w, rb[3], fmaf(w0.z, rb[2],
-                                 fmaf(w0.y, rb[1], w0.x * rb[0])))));
-              e2t[c.row * H_LDS + col + i] = gsum * o;
-              v[i] = o;
-            }
-          }
-        }
-        if (q < 7) {
-          if (to_stash) tmem_st_wait();
-          x_epi_done(s, t);
-          if (q == 2) prefetch_skip(e1_in, t);    // the stash was consumed above; q = 3 adds e1_in from it
+      for (int q = 0; q < 7; ++q, ++lq) {
+        tp(tr, 0);
+        if (q == 0) {
+          r_issue<1, 128>(s, a, acc, d, it);
+          stagger();
+          tp(tr, 1);
+          r_complete<1, 128>(s, acc, d, it);
         } else {
-          x_bar();
-          x_segment_sums(s, c, t, rows, v_in);    // spherenet.py:211
-          x_bar();
-          x_store_tile_coalesced<128>(s, c, t, col0, acc, e1_out + (size_t)e0 * 128, rows);
-          if (FUSE) {
-            // operand of part A of the next block: H_SA * e1, from the registers
-            x_bar();                              // every thread has read the staging overlay
+          r_issue<2, 128>(s, a, acc, d, it);
+          tp(tr, 1);
+          r_complete<2, 128>(s, acc, d, it);
+        }
+        tp(tr, 2);
+        const bool add_tile = q == 0 || q == 2 || q == 3 || q == 5;
+        const bool to_tile = q == 0 || q == 3 || q == 5;
+        const float tile_scale = (q == 0 || q == 3) ? H_SA : 1.0f;   // x_ji / e1_in arrive unscaled (x H_SA is exact)
+        if (q == 0 || q == 3) cp_async_wait_all();
 #pragma unroll
-            for (int p = 0; p < 2; ++p) {
-              float v16[16];
+        for (int j = 0; j < 16; ++j)
 #pragma unroll
-              for (int i = 0; i < 16; ++i) v16[i] = acc[16 * p + i] * H_SA;
-              x_store_a16(s, c, t, col0 + 16 * p, v16);
+          for (int h = 0; h < 2; ++h) {
+            const int row = fr + 8 * h, col = 8 * j + fc, i = 4 * j + 2 * h;
+            const float2 b = *reinterpret_cast<const float2*>(&s.bias[q][col]);
+            float v0 = hswish8<FAST>(fmaf(acc[i], H_SA * H_INV, b.x));
+            float v1 = hswish8<FAST>(fmaf(acc[i + 1], H_SA * H_INV, b.y));
+            float2* tp2 = reinterpret_cast<float2*>(tile + row * R_LDS + col);
+            if (add_tile) {
+              const float2 r = *tp2;
+              v0 += r.x * tile_scale;
+              v1 += r.y * tile_scale;
             }
-            x_epi_done(s, t);
+            if (to_tile) *tp2 = make_float2(v0, v1);
+            acc[i] = v0;
+            acc[i + 1] = v1;
           }
-        }
+        r_acc_to_a(acc, a);
+        if (q == 0) r_bar(cw);                                            // rbf / dst of the unit: visible to all
+        if (q == 2) r_fetch_rows(tile, e1_in + (size_t)e0 * 128, rows, fr, fc);   // read above; q = 3 adds e1_in
+        tp(tr, 3);
       }
+      // q = 7: e1 = tile + act(lin2(t)); e2 = lin_rbf(rbf0) * e1 staged in the tile for the edge -> node sums
+      tp(tr, 0);
+      r_issue<2, 128>(s, a, acc, d, it);
+      tp(tr, 1);
+      r_complete<2, 128>(s, acc, d, it);
+      tp(tr, 2);
+      {
+        float rb[2][6];
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int n = 0; n < 6; ++n) rb[h][n] = rbf[(fr + 8 * h) * 6 + n];
+#pragma unroll
+        for (int j = 0; j < 16; ++j)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int row = fr + 8 * h, col = 8 * j + fc, i = 4 * j + 2 * h;
+            const float2 b = *reinterpret_cast<const float2*>(&s.bias[7][col]);
+            float2* tp2 = reinterpret_cast<float2*>(tile + row * R_LDS + col);
+            const float2 r = *tp2;
+            float e2[2];
+#pragma unroll
+            for (int u = 0; u < 2; ++u) {
+              const float v = hswish8<FAST>(fmaf(acc[i + u], H_SA * H_INV, u ? b.y : b.x)) + (u ? r.y : r.x);
+              const float o = v * (1.0f / H_SA);
+              bad |= !h_finite(o);
+              const float4 w0 = *reinterpret_cast<const float4*>(s.wr + (col + u) * 8);
+              const float2 w1 = *reinterpret_cast<const float2*>(s.wr + (col + u) * 8 + 4);
+              const float gsum = fmaf(w1.y, rb[h][5], fmaf(w1.x, rb[h][4], fmaf(w0.w, rb[h][3], fmaf(w0.z, rb[h][2],
+                                 fmaf(w0.y, rb[h][1], w0.x * rb[h][0])))));
+              e2[u] = gsum * o;
+              acc[i + u] = o;
+            }
+            *tp2 = make_float2(e2[0], e2[1]);
+          }
+      }
+      tp(tr, 3);
+      ++lq;
+      r_bar(cw);
+      r_segment_sums(tile, s.dst[cw], rows, wt, v_in);   // spherenet.py:211
+#pragma unroll
+      for (int j = 0; j < 16; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = fr + 8 * h, i = 4 * j + 2 * h;
+          if (row < rows)
+            *reinterpret_cast<float2*>(e1_out + (size_t)(e0 + row) * 128 + 8 * j + fc) = make_float2(acc[i], acc[i + 1]);
+        }
+      if (tr) g_h16_trace[96 + cw] = clock64();
+      if (MODE == RE_BA) r_acc_to_a(acc, a, H_SA);        // part A of the next block: operand H_SA * e1
+    } else {
+      cp_async_commit();
+      r_load_a<8>(a, e1_in + (size_t)e0 * 128, 128, rows, wt);
     }
-    if (FUSE) {
-      // ---- part A of the next block (spherenet.py:154-161): three more jobs per tile
-      // G0: x_ji = act(lin_ji(e1))
-#pragma unroll 1
-      for (int t = 0; t < ntile; ++t) {
-        const int e0 = (tile0 + t) * H_M, rows = min(H_M, n_edges - e0);
-        const bool valid = c.row < rows;
-        const size_t ge = (size_t)(e0 + c.row);
-        x_drain<2>(s, c, t, col0, 2, acc);
-        x_epi_done(s, t);     // the operand (= e1) is reused unchanged by lin_kj
-        if (valid) {
+    if (MODE != RE_B) {
+      // G0: x_ji = act(lin_ji(e1))                                                spherenet.py:154
+      tp(tr, 0);
+      r_issue<2, 128>(s, a, acc, d, it);
+      stagger();
+      tp(tr, 1);
+      r_complete<2, 128>(s, acc, d, it);
+      tp(tr, 2);
 #pragma unroll
-          for (int i = 0; i < 32; i += 4) {
-            const float4 b = *reinterpret_cast<const float4*>(&s.bias2[0][col0 + i]);
-            float4 o;
-            o.x = hswish<FAST>(fmaf(acc[i], H_INV, b.x));
-            o.y = hswish<FAST>(fmaf(acc[i + 1], H_INV, b.y));
-            o.z = hswish<FAST>(fmaf(acc[i + 2], H_INV, b.z));
-            o.w = hswish<FAST>(fmaf(acc[i + 3], H_INV, b.w));
-            *reinterpret_cast<float4*>(P.n_x_ji + ge * 128 + col0 + i) = o;
-          }
+      for (int j = 0; j < 16; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = fr + 8 * h, col = 8 * j + fc, i = 4 * j + 2 * h;
+          const float2 b = *reinterpret_cast<const float2*>(&s.bias_a[0][col]);
+          if (row < rows)
+            *reinterpret_cast<float2*>(P.x_ji + (size_t)(e0 + row) * 128 + col) =
+                make_float2(hswish<FAST>(fmaf(acc[i], H_INV, b.x)), hswish<FAST>(fmaf(acc[i + 1], H_INV, b.y)));
         }
-      }
-      // G1: x_kj = act(lin_kj(e1)) * lin_rbf2(lin_rbf1(rbf0))
-#pragma unroll 1
-      for (int t = 0; t < ntile; ++t) {
-        const int e0 = (tile0 + t) * H_M, rows = min(H_M, n_edges - e0);
-        const bool valid = c.row < rows;
-        const size_t ge = (size_t)(e0 + c.row);
-        float r8[8];
-        {
-          float rb[6];
+      if (MODE == RE_A) { cp_async_wait_all(); r_bar(cw); }   // rbf of the unit: visible to all
+      tp(tr, 3);
+      ++lq;
+      // G1: x_kj = act(lin_kj(e1)) * lin_rbf2(lin_rbf1(rbf0)), on the same operand    spherenet.py:155-159
+      tp(tr, 0);
+      r_issue<2, 128>(s, a, acc, d, it);
+      tp(tr, 1);
+      r_complete<2, 128>(s, acc, d, it);
+      tp(tr, 2);
+      {
+        float r8[2][8];                                // gate coefficients of the two rows: lin_rbf1(rbf0[row])
 #pragma unroll
-          for (int n = 0; n < 6; ++n) rb[n] = valid ? __ldg(rbf0 + ge * 6 + n) : 0.f;
+        for (int h = 0; h < 2; ++h)
 #pragma unroll
           for (int mm = 0; mm < 8; ++mm) {
-            float a = 0.f;
+            float x = 0.f;
 #pragma unroll
-            for (int n = 0; n < 6; ++n) a = fmaf(s.wr1[mm * 8 + n], rb[n], a);
-            r8[mm] = a;
+            for (int n = 0; n < 6; ++n) x = fmaf(s.wr1[mm * 8 + n], rbf[(fr + 8 * h) * 6 + n], x);
+            r8[h][mm] = x;
           }
-        }
-        x_drain<2>(s, c, t, col0, 2, acc);
 #pragma unroll
-        for (int p = 0; p < 2; ++p) {
-          float v[16];
+        for (int j = 0; j < 16; ++j)
 #pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            const int col = col0 + 16 * p + i;
-            const float4 w0 = *reinterpret_cast<const float4*>(s.wr2 + col * 8);
-            const float4 w1 = *reinterpret_cast<const float4*>(s.wr2 + col * 8 + 4);
-            const float gate = fmaf(w1.w, r8[7], fmaf(w1.z, r8[6], fmaf(w1.y, r8[5], fmaf(w1.x, r8[4],
-                               fmaf(w0.w, r8[3], fmaf(w0.z, r8[2], fmaf(w0.y, r8[1], w0.x * r8[0])))))));
-            v[i] = hswish8<FAST>(fmaf(acc[16 * p + i], H_SA * H_INV, s.bias2[1][col])) * gate;
-          }
-          x_store_a16(s, c, t, col0 + 16 * p, v);
-        }
-        x_epi_done(s, t);
+          for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int u = 0; u < 2; ++u) {
+              const int col = 8 * j + fc + u, i = 4 * j + 2 * h + u;
+              const float4 w0 = *reinterpret_cast<const float4*>(s.wr2 + col * 8);
+              const float4 w1 = *reinterpret_cast<const float4*>(s.wr2 + col * 8 + 4);
+              const float* g = r8[h];
+              const float gate = fmaf(w1.w, g[7], fmaf(w1.z, g[6], fmaf(w1.y, g[5], fmaf(w1.x, g[4],
+                                 fmaf(w0.w, g[3], fmaf(w0.z, g[2], fmaf(w0.y, g[1], w0.x * g[0])))))));
+              acc[i] = hswish8<FAST>(fmaf(acc[i], H_SA * H_INV, s.bias_a[1][col])) * gate;
+            }
       }
-      // G2: x_down = act(lin_down(x_kj)), N = 64: 16 columns per thread
-#pragma unroll 1
-      for (int t = 0; t < ntile; ++t) {
-        const int e0 = (tile0 + t) * H_M, rows = min(H_M, n_edges - e0);
-        const int col = 16 * c.slice;
-        float a16[16];
-        x_drain<1>(s, c, t, col, 2, a16);
+      r_acc_to_a(acc, a);
+      tp(tr, 3);
+      ++lq;
+      // G2: x_down = act(lin_down(x_kj)), N = 64                                  spherenet.py:161
+      {
+        float a64[32], d64[32];
+        tp(tr, 0);
+        r_issue<2, 64>(s, a, a64, d64, it);
+        tp(tr, 1);
+        r_complete<2, 64>(s, a64, d64, it);
+        tp(tr, 2);
 #pragma unroll
-        for (int i = 0; i < 16; ++i) a16[i] = hswish<FAST>(a16[i] * H_INV);
-        x_store_tile_coalesced<64>(s, c, t, col, a16, P.n_x_down + (size_t)e0 * 64, rows);   // all MMAs of the tile are done
-        x_bar();              // the staging overlay of tile t is read before anything else may touch shared memory
+        for (int j = 0; j < 8; ++j)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int row = fr + 8 * h, i = 4 * j + 2 * h;
+            if (row < rows)
+              *reinterpret_cast<float2*>(P.x_down + (size_t)(e0 + row) * 64 + 8 * j + fc) =
+                  make_float2(hswish<FAST>(a64[i] * H_INV), hswish<FAST>(a64[i + 1] * H_INV));
+          }
+        tp(tr, 3);
       }
     }
-    if (c.bad) atomicOr(&g_h16_overflow, 1u);
   }
-  (void)epi;
-  h_finish(s, nullptr);
+  stagger();   // consumer 0 of a CTA without units still meets consumer 1 at the start barrier
+  if (bad) atomicOr(&g_h16_overflow, 1u);
+  if (probe && cw == 0) { g_h16_trace[102] = clock64(); g_h16_trace[103] = (long long)global_ns(); }
 }
 
-// ---------------------------------------------------------------------------------- update_e part A
-struct HAParams {
-  HGemm g[3];                  // lin_ji, lin_kj, lin_down
-  const float *w_rbf1, *w_rbf2;
-};
-
-template <bool FAST>
-__global__ void __launch_bounds__(H_THREADS, 1)
-sphere_update_e_a_h16_kernel(const float* __restrict__ e1, const float* __restrict__ rbf0, int n_edges, HAParams P,
-                             float* __restrict__ x_ji, float* __restrict__ x_down) {
-  extern __shared__ __align__(1024) unsigned char h_raw[];
-  HSmem& s = *reinterpret_cast<HSmem*>(h_raw);
-  const int tid = threadIdx.x, warp = tid >> 5;
-  const int n_tiles = (n_edges + H_M - 1) / H_M, tile0 = blockIdx.x * 2, ntile = min(2, n_tiles - tile0);
-  h_setup(s);
-  for (int i = tid; i < 2 * 128; i += H_THREADS)     // lin_ji's output leaves unscaled, lin_kj's feeds an operand (x H_SA)
-    s.bias[i / 128][i % 128] = (i / 128 ? H_SA : 1.0f) * __ldg(P.g[i / 128].bias + i % 128);
-  for (int i = tid; i < 128 * 8; i += H_THREADS) s.wr[i] = __ldg(P.w_rbf2 + i);      // [128][8]
-  for (int i = tid; i < 64; i += H_THREADS) s.wr1[i] = (i % 8 < 6) ? __ldg(P.w_rbf1 + (i / 8) * 6 + i % 8) : 0.f;
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  HCtx c;
-  bool epi = false;
-  if (warp < H_CTRL_WARPS) {
-    h_regs_ctrl();
-    h_mma(s, P.g, ntile, s.tmem_base);
-  } else if (h_regs_epi(), (c = h_ctx(s, ntile)).t < ntile) {
-    epi = true;
-    const int e0 = (tile0 + c.t) * H_M, rows = min(H_M, n_edges - e0);
-    const bool valid = c.row < rows;
-    const size_t ge = (size_t)(e0 + c.row);
-    const int col0 = c.half * 64;
-    h_load_tile<16>(s, c, e1 + (size_t)e0 * 128, 128, rows);
-    // rbf gate coefficients of this row: r8 = lin_rbf1(rbf0[row])                spherenet.py:157
-    float r8[8];
-    {
-      float rb[6];
-#pragma unroll
-      for (int n = 0; n < 6; ++n) rb[n] = valid ? __ldg(rbf0 + ge * 6 + n) : 0.f;
-#pragma unroll
-      for (int mm = 0; mm < 8; ++mm) {
-        float a = 0.f;
-#pragma unroll
-        for (int n = 0; n < 6; ++n) a = fmaf(s.wr1[mm * 8 + n], rb[n], a);
-        r8[mm] = a;
-      }
-    }
-    h_epi_done(s, c.t);
-    {
-      float acc[64];
-      // G0: x_ji = act(lin_ji(e1))                                                spherenet.py:154
-      h_drain<4, true>(s, c, col0, 2, acc);
-      h_epi_done(s, c.t);   // A (= e1) is reused unchanged by lin_kj: its MMAs may run under this activation
-      if (valid) {
-#pragma unroll
-        for (int i = 0; i < 64; i += 4) {
-          const float4 b = *reinterpret_cast<const float4*>(&s.bias[0][col0 + i]);
-          float4 o;
-          o.x = hswish<FAST>(fmaf(acc[i], H_INV, b.x));
-          o.y = hswish<FAST>(fmaf(acc[i + 1], H_INV, b.y));
-          o.z = hswish<FAST>(fmaf(acc[i + 2], H_INV, b.z));
-          o.w = hswish<FAST>(fmaf(acc[i + 3], H_INV, b.w));
-          *reinterpret_cast<float4*>(x_ji + ge * 128 + col0 + i) = o;
-        }
-      }
-      // G1: x_kj = act(lin_kj(e1)) * lin_rbf2(r8)                                 spherenet.py:155-159
-      h_drain<4, true>(s, c, col0, 2, acc);
-#pragma unroll
-      for (int p = 0; p < 4; ++p) {
-        float v[16];
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          const int col = col0 + 16 * p + i;
-          const float4 w0 = *reinterpret_cast<const float4*>(s.wr + col * 8);
-          const float4 w1 = *reinterpret_cast<const float4*>(s.wr + col * 8 + 4);
-          const float gate = fmaf(w1.w, r8[7], fmaf(w1.z, r8[6], fmaf(w1.y, r8[5], fmaf(w1.x, r8[4],
-                             fmaf(w0.w, r8[3], fmaf(w0.z, r8[2], fmaf(w0.y, r8[1], w0.x * r8[0])))))));
-          v[i] = hswish8<FAST>(fmaf(acc[16 * p + i], H_SA * H_INV, s.bias[1][col])) * gate;
-        }
-        h_store_a16(s, c, col0 + 16 * p, v);
-      }
-      h_epi_done(s, c.t);
-    }
-    // G2: x_down = act(lin_down(x_kj)), N = 64                                    spherenet.py:161
-    {
-      const int col = c.half * 32;
-      float a32[32];
-      h_drain<2, true>(s, c, col, 2, a32);
-#pragma unroll
-      for (int i = 0; i < 32; ++i) a32[i] = hswish<FAST>(a32[i] * H_INV);
-      h_store_tile_coalesced<64>(s, c, col, a32, x_down + (size_t)e0 * 64, rows);   // all MMAs of the tile are done
-    }
+template <int MODE>
+static int launch_update_e_h16(const float* m, const float* x_ji, const float* e1_in, const float* rbf0,
+                               const int32_t* dst, int64_t n_edges, const REParams& P, float* e1_out, float* v_in,
+                               cudaStream_t st) {
+  auto kfn = h16_fast_swish ? sphere_update_e_h16_kernel<true, MODE> : sphere_update_e_h16_kernel<false, MODE>;
+  cudaError_t e = cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(RSmem));
+  if (e != cudaSuccess) {
+    set_error("cudaFuncSetAttribute(%zu): %s", sizeof(RSmem), cudaGetErrorString(e));
+    return DIG3D_ECUDA;
   }
-  h_finish(s, epi ? &c : nullptr);
+  int dev = 0, n_sm = 132;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
+  const int units = (int)ceil_div(n_edges, R_UNIT);
+  const int grid = min(n_sm, (units + 1) / 2);
+  kfn<<<grid, R_THREADS, sizeof(RSmem), st>>>(m, x_ji, e1_in, rbf0, dst, (int)n_edges, P, e1_out, v_in);
+  DIG3D_LAUNCH_CHECK();
+  return DIG3D_OK;
 }
 
 // ---------------------------------------------------------------------------------- init_e
@@ -1202,7 +966,7 @@ sphere_init_e_h16_kernel(const int64_t* __restrict__ z, const int32_t* __restric
   bool epi = false;
   if (warp < H_CTRL_WARPS) {
     h_regs_ctrl();
-    h_mma_n<false, false>(s, P.g, TABLE ? 1 : 3, ntile, s.tmem_base);
+    h_mma_n<false>(s, P.g, TABLE ? 1 : 3, ntile, s.tmem_base);
   } else if (h_regs_epi(), (c = h_ctx(s, ntile)).t < ntile) {
     epi = true;
     const int e0 = (tile0 + c.t) * H_M, rows = min(H_M, n_edges - e0);
@@ -1340,7 +1104,7 @@ sphere_update_v_h16_kernel(const float* __restrict__ v_in_all, int n_nodes, HVPa
   tc_fence_after();
   if (warp < H_CTRL_WARPS) {
     h_regs_ctrl();
-    h_mma_n<false, true>(s, g, ng, 2, s.tmem_base);
+    h_mma_n<true>(s, g, ng, 2, s.tmem_base);
   } else {
     h_regs_epi();
     HCtx c = h_ctx(s, 2);
@@ -1468,7 +1232,7 @@ linear_h16_kernel(const float* __restrict__ x, int n_rows, int ldx, HLinParams P
   bool epi = false;
   if (warp < H_CTRL_WARPS) {
     h_regs_ctrl();
-    h_mma_n<false, false>(s, P.g, NPANEL, ntile, s.tmem_base);
+    h_mma_n<false>(s, P.g, NPANEL, ntile, s.tmem_base);
   } else if (h_regs_epi(), (c = h_ctx(s, ntile)).t < ntile) {
     epi = true;
     const int r0 = (tile0 + c.t) * H_M, rows = min(H_M, n_rows - r0);
@@ -1790,8 +1554,10 @@ int dig3d_h16_set_fast_swish(int32_t on) {
   return DIG3D_OK;
 }
 
+// Selected between the eight- and sixteen-warp epilogues of the two-tile update_e kernels, which the register engine
+// replaced: accepted and ignored (the tests and the model forwards still call it).
 int dig3d_h16_set_wide_epilogue(int32_t on) {
-  h16_wide_epilogue = on ? 1 : 0;
+  (void)on;
   return DIG3D_OK;
 }
 
@@ -1864,18 +1630,22 @@ int dig3d_sphere_update_e_a_h16(const float* e1, const float* rbf0, int64_t n_ed
                                 float* x_ji, float* x_down, void* stream) {
   DIG3D_REQUIRE(e1 && rbf0 && w && x_ji && x_down, "sphere_update_e_a_h16: null pointer");
   if (n_edges == 0) return DIG3D_OK;
-  HAParams P;
+  REParams P = {};
   P.g[0] = {(const unsigned char*)w->p_ji, w->b_ji, 128, 128};
   P.g[1] = {(const unsigned char*)w->p_kj, w->b_kj, 128, 128};
   P.g[2] = {(const unsigned char*)w->p_down, nullptr, 128, 64};
   P.w_rbf1 = w->w_rbf1; P.w_rbf2 = w->w_rbf2;
-  auto kfn = h16_fast_swish ? sphere_update_e_a_h16_kernel<true> : sphere_update_e_a_h16_kernel<false>;
-  int rc = h_smem_attr((const void*)kfn);
-  if (rc) return rc;
-  const int pairs = ceil_div(ceil_div(n_edges, H_M), 2);
-  kfn<<<pairs, H_THREADS, sizeof(HSmem), (cudaStream_t)stream>>>(e1, rbf0, (int)n_edges, P, x_ji, x_down);
-  DIG3D_LAUNCH_CHECK();
-  return DIG3D_OK;
+  P.x_ji = x_ji; P.x_down = x_down;
+  return launch_update_e_h16<RE_A>(nullptr, nullptr, e1, rbf0, nullptr, n_edges, P, nullptr, nullptr,
+                                   (cudaStream_t)stream);
+}
+
+static void update_e_b_params(REParams& P, const dig3d_tc_update_e* w) {
+  P.g[0] = {(const unsigned char*)w->p_up, nullptr, 64, 128};
+  for (int i = 0; i < 2; ++i) P.g[1 + i] = {(const unsigned char*)w->p_res[i], w->b_res[i], 128, 128};
+  P.g[3] = {(const unsigned char*)w->p_lin, w->b_lin, 128, 128};
+  for (int i = 2; i < 6; ++i) P.g[2 + i] = {(const unsigned char*)w->p_res[i], w->b_res[i], 128, 128};
+  P.w_rbf = w->w_rbf;
 }
 
 int dig3d_sphere_update_e_b_h16(const float* m, const float* e1_in, const float* x_ji, const float* rbf0,
@@ -1883,23 +1653,9 @@ int dig3d_sphere_update_e_b_h16(const float* m, const float* e1_in, const float*
                                 float* v_in, void* stream) {
   DIG3D_REQUIRE(m && e1_in && x_ji && rbf0 && dst && w && e1_out && v_in, "sphere_update_e_b_h16: null pointer");
   if (n_edges == 0) return DIG3D_OK;
-  HBParams P;
-  P.g[0] = {(const unsigned char*)w->p_up, nullptr, 64, 128};
-  for (int i = 0; i < 2; ++i) P.g[1 + i] = {(const unsigned char*)w->p_res[i], w->b_res[i], 128, 128};
-  P.g[3] = {(const unsigned char*)w->p_lin, w->b_lin, 128, 128};
-  for (int i = 2; i < 6; ++i) P.g[2 + i] = {(const unsigned char*)w->p_res[i], w->b_res[i], 128, 128};
-  P.w_rbf = w->w_rbf;
-  P.n_w_rbf1 = P.n_w_rbf2 = nullptr; P.n_x_ji = P.n_x_down = nullptr;
-  auto kfn = h16_wide_epilogue
-                 ? (h16_fast_swish ? sphere_update_e_b_x16_kernel<true, false> : sphere_update_e_b_x16_kernel<false, false>)
-                 : (h16_fast_swish ? sphere_update_e_b_h16_kernel<true, false> : sphere_update_e_b_h16_kernel<false, false>);
-  int rc = h_smem_attr((const void*)kfn);
-  if (rc) return rc;
-  const int pairs = ceil_div(ceil_div(n_edges, H_M), 2);
-  kfn<<<pairs, H_THREADS, sizeof(HSmem), (cudaStream_t)stream>>>(m, x_ji, e1_in, rbf0, dst, (int)n_edges, P, e1_out,
-                                                                 v_in);
-  DIG3D_LAUNCH_CHECK();
-  return DIG3D_OK;
+  REParams P = {};
+  update_e_b_params(P, w);
+  return launch_update_e_h16<RE_B>(m, x_ji, e1_in, rbf0, dst, n_edges, P, e1_out, v_in, (cudaStream_t)stream);
 }
 
 int dig3d_sphere_update_e_ba_h16(const float* m, const float* e1_in, const float* x_ji, const float* rbf0,
@@ -1908,29 +1664,16 @@ int dig3d_sphere_update_e_ba_h16(const float* m, const float* e1_in, const float
                                  float* x_down_next, void* stream) {
   DIG3D_REQUIRE(m && e1_in && x_ji && rbf0 && dst && w && w_next && e1_out && v_in && x_ji_next && x_down_next,
                 "sphere_update_e_ba_h16: null pointer");
-  DIG3D_REQUIRE(x_ji_next != x_ji, "sphere_update_e_ba_h16: x_ji_next must not alias x_ji (other tiles still read it)");
+  DIG3D_REQUIRE(x_ji_next != x_ji, "sphere_update_e_ba_h16: x_ji_next must not alias x_ji (other units still read it)");
   if (n_edges == 0) return DIG3D_OK;
-  HBParams P;
-  P.g[0] = {(const unsigned char*)w->p_up, nullptr, 64, 128};
-  for (int i = 0; i < 2; ++i) P.g[1 + i] = {(const unsigned char*)w->p_res[i], w->b_res[i], 128, 128};
-  P.g[3] = {(const unsigned char*)w->p_lin, w->b_lin, 128, 128};
-  for (int i = 2; i < 6; ++i) P.g[2 + i] = {(const unsigned char*)w->p_res[i], w->b_res[i], 128, 128};
+  REParams P = {};
+  update_e_b_params(P, w);
   P.g[8] = {(const unsigned char*)w_next->p_ji, w_next->b_ji, 128, 128};
   P.g[9] = {(const unsigned char*)w_next->p_kj, w_next->b_kj, 128, 128};
   P.g[10] = {(const unsigned char*)w_next->p_down, nullptr, 128, 64};
-  P.w_rbf = w->w_rbf;
-  P.n_w_rbf1 = w_next->w_rbf1; P.n_w_rbf2 = w_next->w_rbf2;
-  P.n_x_ji = x_ji_next; P.n_x_down = x_down_next;
-  auto kfn = h16_wide_epilogue
-                 ? (h16_fast_swish ? sphere_update_e_b_x16_kernel<true, true> : sphere_update_e_b_x16_kernel<false, true>)
-                 : (h16_fast_swish ? sphere_update_e_b_h16_kernel<true, true> : sphere_update_e_b_h16_kernel<false, true>);
-  int rc = h_smem_attr((const void*)kfn);
-  if (rc) return rc;
-  const int pairs = ceil_div(ceil_div(n_edges, H_M), 2);
-  kfn<<<pairs, H_THREADS, sizeof(HSmem), (cudaStream_t)stream>>>(m, x_ji, e1_in, rbf0, dst, (int)n_edges, P, e1_out,
-                                                                 v_in);
-  DIG3D_LAUNCH_CHECK();
-  return DIG3D_OK;
+  P.w_rbf1 = w_next->w_rbf1; P.w_rbf2 = w_next->w_rbf2;
+  P.x_ji = x_ji_next; P.x_down = x_down_next;
+  return launch_update_e_h16<RE_BA>(m, x_ji, e1_in, rbf0, dst, n_edges, P, e1_out, v_in, (cudaStream_t)stream);
 }
 
 int dig3d_sphere_triplet_gather_tc(const float* x_down, const float* sbf_p, const float* t_p, int32_t ld_p,

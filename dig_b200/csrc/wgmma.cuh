@@ -7,11 +7,13 @@
 //     contiguous (128 B): SBO = 128 B (next 8 rows), LBO = the byte stride of one k-unit plane (next K elements);
 //   * one warpgroup (4 warps, 128 threads) issues the wgmma.mma_async instructions of a 128-row tile as two
 //     m64 halves and n64 column blocks, accumulating ONE K-chunk in registers (scale-d = 0 on its first product);
-//   * in the dense chains the finished chunk goes to the accumulator store: a slot of 128 rows x up to 512 fp32
-//     columns in global memory (L2-resident) that the CTA claims for its lifetime, addressed like tensor memory by
-//     (row << 16 | column).  The epilogue warps read whole 16-column row pieces of it (thread = row) while the
-//     warpgroup works on the next chunk, and the ready / free handshakes are mbarriers.  Kernels whose epilogue can
-//     work on the fragment layout directly (triplet gather, weight gradient) keep their accumulators in registers.
+//   * in the store-engine dense chains (init_e, update_v, the generic linear, the 3xTF32 chain) the finished chunk goes
+//     to the accumulator store: a slot of 128 rows x up to 512 fp32 columns in global memory (L2-resident) that the CTA
+//     claims for its lifetime, addressed like tensor memory by (row << 16 | column).  The epilogue warps read whole
+//     16-column row pieces of it (thread = row) while the warpgroup works on the next chunk, and the ready / free
+//     handshakes are mbarriers.  Kernels whose epilogue works on the fragment layout directly (update_e's register
+//     engine, triplet gather, weight gradient) keep their accumulators in registers; update_e also takes its A operand
+//     from registers (mma_f16_rs).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -130,9 +132,53 @@ __device__ __forceinline__ void mma_tf32(float (&d)[32], uint64_t a_desc, uint64
       : "memory");
 }
 // Register fragment of an m64n64 accumulator: thread t of the warpgroup holds rows 16 (t/32) + (t%32)/4 (+8) and
-// columns 8 j + 2 (t%4) (+1), j = 0..7: d[4j], d[4j+1] on the first row, d[4j+2], d[4j+3] on the second.
+// columns 8 j + 2 (t%4) (+1), j = 0..7: d[4j], d[4j+1] on the first row, d[4j+2], d[4j+3] on the second.  An m64n128
+// accumulator continues the same pattern with j = 0..15.
 __device__ __forceinline__ int frag_row(int wt) { return 16 * (wt >> 5) + ((wt & 31) >> 2); }
 __device__ __forceinline__ int frag_col(int wt) { return 2 * (wt & 3); }
+
+// ---- wgmma with A from registers
+// The A operand of m64nNk16 (fp16) held in registers: thread t owns four 32-bit registers per k-step, each an fp16 pair
+// of consecutive columns (lower column in the low half): a[0] = row frag_row(t), columns 2 (t%4) (+1); a[1] = row + 8,
+// same columns; a[2] / a[3] = the same rows at columns + 8.  These are exactly the rows and columns of accumulator
+// entries d[8 s + 2 r], d[8 s + 2 r + 1] of an m64nN fragment for k-step s (columns 16 s .. 16 s + 15): a layer's
+// accumulator becomes the next layer's A operand without leaving the thread.
+__device__ __forceinline__ constexpr int frag_a_src(int s, int r) { return 8 * s + 2 * r; }
+// Row / column of register r of k-step s in the A operand (first column of its pair).
+__device__ __forceinline__ int frag_a_row(int wt, int r) { return frag_row(wt) + 8 * (r & 1); }
+__device__ __forceinline__ int frag_a_col(int wt, int s, int r) { return 16 * s + 8 * (r >> 1) + frag_col(wt); }
+
+#define TC90_D64 "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"                                          \
+                 "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"                                  \
+                 "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,"                                  \
+                 "%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}"
+#define TC90_D64_OPS(d)                                                                                          \
+  TC90_D32_OPS(d), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]),    \
+      "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]),    \
+      "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]),    \
+      "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]),    \
+      "+f"(d[63])
+
+// D[64 x 64] (+)= A[64 x 16] (registers) * B[64 x 16]^T (shared memory), fp16 operands, fp32 accumulate.
+__device__ __forceinline__ void mma_f16_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t b_desc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 " TC90_D32 ", {%32,%33,%34,%35}, %36, p, 1, 1, 0;\n\t}"
+      : TC90_D32_OPS(d)
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate)
+      : "memory");
+}
+// D[64 x 128] (+)= A[64 x 16] (registers) * B[128 x 16]^T (shared memory).
+__device__ __forceinline__ void mma_f16_rs(float (&d)[64], const uint32_t (&a)[4], uint64_t b_desc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %69, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 " TC90_D64 ", {%64,%65,%66,%67}, %68, p, 1, 1, 0;\n\t}"
+      : TC90_D64_OPS(d)
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate)
+      : "memory");
+}
 
 // ---- accumulator store (see the header comment)
 // A translation unit that uses the store defines TC90_TM_COLS (columns per slot) before including this header.  The

@@ -671,7 +671,7 @@ def sphere_init_e_h16(z, g, rbf0, w, packed_lin, hidden, v_in=None, tables=None)
 
 
 def sphere_update_e_h16(e1, g, rbf0, sbf_p, t_p, col0, w, hidden, int_emb, v_in=None):
-    """update_e (A + triplet gather + B) with the dense chain on wgmma, two tiles in flight per SM (3xFP16)."""
+    """update_e (A + triplet gather + B) with the dense chain on wgmma, register-accumulator engine (3xFP16)."""
     dev = e1.device
     e = g.n_edges
     x_ji = torch.empty(max(e, 1), hidden, dtype=torch.float32, device=dev)[:e]
@@ -743,7 +743,8 @@ _H16_WIDE = [None]
 
 
 def h16_set_wide_epilogue(on):
-    """update_e part B (+ A): all sixteen epilogue warps on the ready tile (True) or eight per tile (False)."""
+    """No effect since update_e moved to the register-accumulator engine (it chose between the epilogue layouts of the
+    two-tile kernels); kept for existing callers."""
     call("dig3d_h16_set_wide_epilogue", int(bool(on)))
     _H16_WIDE[0] = bool(on)
 

@@ -314,13 +314,16 @@ int dig3d_sphere_init_e_h16(const int64_t* z, const int32_t* src, const int32_t*
 int dig3d_sphere_init_e_h16_tab(const int64_t* z, const int32_t* src, const int32_t* dst, const float* rbf0,
                                 int64_t n_edges, const dig3d_init_e_weights* w, const void* packed_rbf_panel,
                                 const float* tab_i, const float* tab_j, float* e1, float* v_in, void* stream);
+/* update_e part A (x_ji, x_down) and part B (e1_out, edge -> node sums added into v_in, which the caller zeroes) on
+ * the register-accumulator engine: persistent CTAs, two consumer warpgroups with one 64-edge unit each, activations
+ * kept in wgmma register fragments between layers.                               spherenet.py:150-182, 211 */
 int dig3d_sphere_update_e_a_h16(const float* e1, const float* rbf0, int64_t n_edges, const dig3d_tc_update_e* w,
                                 float* x_ji, float* x_down, void* stream);
 int dig3d_sphere_update_e_b_h16(const float* m, const float* e1_in, const float* x_ji, const float* rbf0,
                                 const int32_t* dst, int64_t n_edges, const dig3d_tc_update_e* w, float* e1_out,
                                 float* v_in, void* stream);
 /* dig3d_sphere_update_e_b_h16 of block l with part A of block l + 1 (dig3d_sphere_update_e_a_h16 on the e1 this kernel
- * produces) appended to the same tile chain: one launch, one set-up and one read of e1 less per block; bit-identical to
+ * produces) appended to the same unit chain: one launch, one set-up and one read of e1 less per block; bit-identical to
  * the two separate launches.  w_next: the next block's weights; x_ji_next [E, 128] (must not alias x_ji), x_down_next
  * [E, 64]: its part-A outputs.                                                  spherenet.py:150-182 */
 int dig3d_sphere_update_e_ba_h16(const float* m, const float* e1_in, const float* x_ji, const float* rbf0,
@@ -360,10 +363,8 @@ int dig3d_h16_timeouts(void);
 /* debugging probe: enable / read the clock64() timeline CTA 0 of update_e part B records (host buffer, 128 x i64) */
 int dig3d_h16_trace(int32_t on, long long* out128);
 int dig3d_h16_set_fast_swish(int32_t on);
-/* Process-wide switch of dig3d_sphere_update_e_b_h16 / _ba_h16: 0 = eight epilogue warps per tile (64 columns per
- * thread), 1 = all sixteen epilogue warps on the tile whose accumulators are ready (32 columns per thread): a shorter
- * epilogue per tile, so that the chain's cycle is bound by MMA issue.  Same jobs, same barriers; the edge -> node sums
- * are grouped in 32-row instead of 64-row parts (fp32 summation order only). */
+/* No effect: it selected between the eight- and sixteen-warp epilogues of the two-tile update_e kernels, which the
+ * register-accumulator engine replaced.  Kept so that existing callers still link; always returns DIG3D_OK. */
 int dig3d_h16_set_wide_epilogue(int32_t on);
 
 /* ------------------------------------------------------------------ SchNet

@@ -1,4 +1,5 @@
-"""Timeline of CTA 0 of sphere_update_e_b_h16_kernel (clock64 probes) -- test infrastructure."""
+"""Timeline of CTA 0 of the update_e register-accumulator engine (clock64 probes of the last update_e launch, part B
+here) -- test infrastructure."""
 import ctypes, os, sys
 import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -28,17 +29,11 @@ torch.cuda.synchronize()
 buf = (ctypes.c_longlong * 128)()
 lib.dig3d_h16_trace(0, buf)
 t = list(buf); t0 = t[100]
-print(f"kernel (CTA 0): {t[102] - t0} cycles, {t[103] - t[101]} ns -> {1e3 * (t[102] - t0) / max(1, t[103] - t[101]):.0f} MHz")
-print(f"startup: setup+sync +{t[104] - t0}, epilogue registers +{t[105] - t0}, m tile staged +{t[106] - t0}, "
-      f"A published +{t[107] - t0}, skip row prefetched +{t[108] - t0}")
-print("MMA issuer: job (layer q, tile t): A-ready .. all issued")
-for q in range(8):
-    for tt in range(2):
-        a, e = t[(q * 2 + tt) * 2] - t0, t[(q * 2 + tt) * 2 + 1] - t0
-        print(f"  q{q} t{tt}: +{a:7d} .. +{e:7d}  ({e - a:5d} issuing)")
-for tt in range(2):
-    print(f"epilogue tile {tt} (first thread): drain-wait start / drained / activated / signalled")
+print(f"consumer 0 of CTA 0: {t[102] - t0} cycles, {t[103] - t[101]} ns -> {1e3 * (t[102] - t0) / max(1, t[103] - t[101]):.0f} MHz")
+print(f"set-up (barriers, biases, gate weights) +{t[104] - t0}")
+for cw in range(2):
+    print(f"consumer {cw}, first unit: layer: slabs-wait start / issued / accumulators complete / epilogue done")
     for q in range(8):
-        s = [t[32 + tt * 32 + q * 4 + i] - t0 for i in range(4)]
-        print(f"  q{q}: +{s[0]:7d} +{s[1]:7d} +{s[2]:7d} +{s[3]:7d}   wait+drain {s[1] - s[0]:5d}  activation {s[2] - s[1]:5d}")
-    print(f"  segment sums done +{t[96 + tt] - t0}")
+        s = [t[cw * 48 + q * 4 + i] - t0 for i in range(4)]
+        print(f"  q{q}: +{s[0]:7d} +{s[1]:7d} +{s[2]:7d} +{s[3]:7d}   MMA wait {s[2] - s[1]:5d}  epilogue {s[3] - s[2]:5d}")
+    print(f"  edge -> node sums and e1 stored +{t[96 + cw] - t0}")
