@@ -124,6 +124,8 @@ SIGNATURES = {
     "dig3d_comenet_embed": [P, P, c_int64, P, P],
     "dig3d_pbc_edge_vectors": [P, P, P, P, P, c_int64, P, P, P],
     "dig3d_comenet_geometry_edges": [P, P, P, P, P, c_int64, c_int64, c_double, P, P, P, P, P, P],
+    "dig3d_radius_graph_pbc_count": [P, P, P, c_int64, c_int64, c_double, c_int32, P, P, P, P, P, P, P],
+    "dig3d_radius_graph_pbc_fill": [P, P, c_int64, c_int64, c_double, P, P, P, P, c_int64, P, P, P, P],
     "dig3d_comenet_block": [P, P, P, P, P, P, P, c_int64, c_int64, c_int64, POINTER(ComenetBlockWeights),
                             POINTER(ComenetHeadWeights), c_int32, P, P, P, P, P, P, P, P],
     "dig3d_edge_weighted_sum": [P, P, P, P, c_int64, c_int32, P, P],
@@ -175,7 +177,8 @@ _lib = None
 
 
 class Dig3dError(RuntimeError):
-    pass
+    """A non-zero return code of the library; `rc` holds it (DIG3D_EINVAL = -1: the arguments were rejected)."""
+    rc = None
 
 
 def load():
@@ -235,4 +238,6 @@ def call(name, *args):
     launch_count += 1
     if rc != 0:
         msg = lib.dig3d_last_error()
-        raise Dig3dError(f"{name} failed (rc={rc}): {msg.decode() if msg else ''}")
+        err = Dig3dError(f"{name} failed (rc={rc}): {msg.decode() if msg else ''}")
+        err.rc = rc
+        raise err

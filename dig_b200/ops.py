@@ -373,6 +373,51 @@ def schnet_readout(v, lin1, lin2, out_channels):
     return node_out
 
 
+def radius_graph_pbc(pos, cell, natoms, radius, max_num_neighbors_threshold):
+    """Periodic radius graph (ocpmodels' radius_graph_pbc, 2022): every periodic image of every atom of the same
+    structure within `radius` of each target atom, the image range per axis being the batch maximum of
+    ceil(radius / plane spacing); with max_num_neighbors_threshold > 0 each target keeps that many nearest (ties: first
+    in enumeration order), <= 0 keeps all.  pos [N, 3] fp32, cell [B, 3, 3] (rows = lattice vectors), natoms [B].
+
+    Returns (edge_index [2, E] int64 = (source j, target i), grouped by target, sources then image cells in the
+    reference's enumeration order; cell_offsets [E, 3] fp32 integer image cells; neighbors [B] int64 edges per
+    structure).  One host synchronisation (the edge total).  Raises ValueError for a cell of zero or non-finite volume,
+    natoms that do not sum to N, or more than 2^31 - 1 edges."""
+    if pos.dim() != 2 or pos.size(1) != 3:
+        raise ValueError(f"pos must be [N, 3], got {tuple(pos.shape)}")
+    if natoms.dim() != 1 or cell.shape != (natoms.numel(), 3, 3):
+        raise ValueError(f"cell must be [B, 3, 3] and natoms [B], got {tuple(cell.shape)} and {tuple(natoms.shape)}")
+    if not 0.0 < float(radius) < float("inf"):
+        raise ValueError(f"radius must be positive and finite, got {radius}")
+    pos = pos.detach()
+    dev = pos.device
+    n, nb = pos.size(0), natoms.numel()
+    cell = cell.detach().to(device=dev, dtype=torch.float32).contiguous()
+    natoms = natoms.to(device=dev, dtype=torch.int64).contiguous()
+    thr = int(max_num_neighbors_threshold)
+    st = _stream()
+    graph_ptr = torch.empty(nb + 1, dtype=torch.int32, device=dev)
+    counts = torch.empty(max(n, 1), dtype=torch.int32, device=dev)
+    select = torch.empty(2 * max(n, 1), dtype=torch.int32, device=dev)
+    row_ptr = torch.empty(n + 1, dtype=torch.int32, device=dev)
+    info = torch.empty(6, dtype=torch.int64, device=dev)
+    n_edges = ctypes.c_int64(0)
+    try:
+        call("dig3d_radius_graph_pbc_count", _p(pos, torch.float32, "pos"), _p(cell), _p(natoms), n, nb, float(radius),
+             thr, _p(graph_ptr), _p(counts), _p(select), _p(row_ptr), _p(info), ctypes.byref(n_edges), st)
+    except _lib.Dig3dError as exc:
+        if exc.rc == -1:                                   # DIG3D_EINVAL: the input was rejected
+            raise ValueError(str(exc)) from None
+        raise
+    e = n_edges.value
+    edge_index = torch.empty(2, e, dtype=torch.int64, device=dev)
+    cell_offsets = torch.empty(e, 3, dtype=torch.float32, device=dev)
+    neighbors = torch.empty(nb, dtype=torch.int64, device=dev)
+    call("dig3d_radius_graph_pbc_fill", _p(pos), _p(cell), n, nb, float(radius), _p(graph_ptr), _p(select),
+         _p(row_ptr), _p(info), e, _p(edge_index), _p(cell_offsets), _p(neighbors), st)
+    return edge_index, cell_offsets, neighbors
+
+
 # ----------------------------------------------------------------------------- ComENet
 def comenet_geometry(g, pos, cutoff, want_angles=False):
     dev = pos.device

@@ -3,10 +3,12 @@ precomputed edge lists with periodic images, optional per-tag ("hetero") weights
 
 Same constructor arguments as the reference class; `forward(data)` reads what the reference reads from an OCP batch:
 `atomic_numbers, pos, batch, tags, edge_index, cell, cell_offsets, neighbors` (use_pbc=True, otf_graph=False -- the
-shipped IS2RE configuration, ocp/comenet.yml).  The state_dict has the keys of the shipped checkpoint
+shipped IS2RE configuration, ocp/comenet.yml).  With otf_graph=True the batch needs only `atomic_numbers, pos, batch,
+cell, natoms`: the periodic graph is built on the GPU (radius_graph_pbc, cap 50) and written back onto `data` as
+`edge_index, cell_offsets, neighbors`, as the reference does (comenet-ocp.py:343-350).  The state_dict has the keys of the shipped checkpoint
 (`IS2RETrainedModelWeights.pt`, 125 tensors / 4 185 857 parameters, saved with a `module.` prefix).
 
-Kernels: get_pbc_distances -> dig3d_pbc_edge_vectors; the four scatter_min / argmin over the unsorted edge list and the
+Kernels: radius_graph_pbc -> dig3d_radius_graph_pbc_count / _fill; get_pbc_distances -> dig3d_pbc_edge_vectors; the four scatter_min / argmin over the unsorted edge list and the
 angle / basis features -> dig3d_comenet_geometry_edges; the interaction blocks run on the generic CUDA primitives of
 dig_b200.autograd (forward and backward), with the edges re-ordered by target once (stable: a segmented sum instead of
 atomics).  There is no fused block kernel for this variant yet (the fused ComENet block is compiled for middle = 64)."""
@@ -16,6 +18,7 @@ from torch import nn
 from ... import autograd as ag
 from ... import ops
 from ...ops import _p, _stream, call
+from ..utils.pbc import radius_graph_pbc
 from ._common import require_cuda
 from .comenet import EdgeGraphConv, EmbeddingBlock, GraphNorm, Linear
 
@@ -85,9 +88,10 @@ class ComENet(nn.Module):
             raise NotImplementedError(
                 "the ComENet geometry/basis kernel is generated for num_radial=3, num_spherical=2 (the shipped "
                 f"ocp/comenet.yml and dig_b200/codegen.py:CONFIGS); got {(num_radial, num_spherical)}")
-        if otf_graph or not use_pbc or regress_forces:
-            raise NotImplementedError("ComENet-OCP: only otf_graph=False, use_pbc=True, regress_forces=False "
-                                      "(the shipped IS2RE configuration) is implemented")
+        if not use_pbc or regress_forces:
+            raise NotImplementedError("ComENet-OCP: only use_pbc=True, regress_forces=False (the shipped IS2RE "
+                                      "configuration, with the graph precomputed or built with otf_graph=True) is "
+                                      "implemented")
         self.num_targets, self.regress_forces, self.use_pbc = num_targets, regress_forces, use_pbc
         self.cutoff, self.otf_graph, self.num_blocks, self.hetero = cutoff, otf_graph, num_blocks, hetero
         self.emb = EmbeddingBlock(hidden_channels)
@@ -173,6 +177,8 @@ class ComENet(nn.Module):
         flags = torch.zeros(1, dtype=torch.int32, device=dev)
         call("dig3d_validate_nodes", _p(batch), _p(z, torch.int64, "atomic_numbers"), n, num_graphs,
              self.emb.emb.num_embeddings, _p(flags), _stream())
+        if self.otf_graph:                                                   # comenet-ocp.py:343-350
+            data.edge_index, data.cell_offsets, data.neighbors = radius_graph_pbc(data, self.cutoff, 50)
         src, dst, row_ptr, f1, f2 = self._geometry(data)
         if int(flags.item()):
             raise ValueError("ComENet-OCP: batch ids / atomic numbers out of range")

@@ -1,3 +1,4 @@
 from .geometric_computing import radius_graph, xyz_to_dat
+from .pbc import radius_graph_pbc
 
-__all__ = ['xyz_to_dat', 'radius_graph']
+__all__ = ['xyz_to_dat', 'radius_graph', 'radius_graph_pbc']

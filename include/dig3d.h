@@ -7,7 +7,8 @@
  *
  * Conventions (all entry points):
  *   - plain pointers + sizes, no torch types; all pointers are DEVICE pointers unless named *_host;
- *   - caller owns every buffer (no allocation, no synchronisation inside; the only process-wide state are the
+ *   - caller owns every buffer (no allocation, no synchronisation inside except the one read-back of
+ *     dig3d_radius_graph_pbc_count; the only process-wide state are the
  *     experiment switches dig3d_tc_set_fast_swish / dig3d_tc_trace / dig3d_linear_set_config and a thread-local
  *     error string);
  *   - `stream` is a cudaStream_t passed as void*;
@@ -413,6 +414,25 @@ int dig3d_comenet_geometry_edges(const float* vec, const float* dist, const int6
                                  const int32_t* dst, int64_t n_nodes, int64_t n_edges, double cutoff, int32_t* refs,
                                  unsigned long long* keys, float* feature1, float* feature2, float* angles,
                                  void* stream);
+
+/* Periodic radius graph = ocpmodels' radius_graph_pbc(data, radius, max_num_neighbors) (2022), called by ComENet-OCP
+ * with otf_graph=True (comenet-ocp.py:343-350).  pos [N,3], cell [B,3,3] (rows = lattice vectors), natoms [B] int64.
+ * Image range per axis = ceil(radius * |a_k x a_l| / vol), maximum over the batch; candidates per target i: source j
+ * of the same structure, then image cell (cartesian product, last axis fastest); kept when d2 <= fp32(radius^2) and
+ * d2 > 1e-4; with max_num_neighbors > 0 each target keeps its max_num_neighbors smallest d2 (ties: first enumerated).
+ * Count pass: graph_ptr [B+1], counts [N], select [2N] and row_ptr [N+1] int32 and info [6] int64 are written
+ * (device); the stream is synchronised once and *n_edges_host receives E.  Returns DIG3D_EINVAL for a cell with
+ * zero or non-finite volume, natoms that do not sum to N, an image range above 2^31 candidates per atom, or E >= 2^31.
+ * Fill pass (after a successful count, same buffers): edge_index [2,E] int64 = (j, i) grouped by target in
+ * enumeration order, cell_offsets [E,3] fp32 = integer image cell, neighbors [B] int64 = edges per structure. */
+int dig3d_radius_graph_pbc_count(const float* pos, const float* cell, const int64_t* natoms, int64_t n_atoms,
+                                 int64_t n_graphs, double radius, int32_t max_num_neighbors, int32_t* graph_ptr,
+                                 int32_t* counts, uint32_t* select, int32_t* row_ptr, int64_t* info,
+                                 int64_t* n_edges_host, void* stream);
+int dig3d_radius_graph_pbc_fill(const float* pos, const float* cell, int64_t n_atoms, int64_t n_graphs, double radius,
+                                const int32_t* graph_ptr, const uint32_t* select, const int32_t* row_ptr,
+                                const int64_t* info, int64_t n_edges, int64_t* edge_index, float* cell_offsets,
+                                int64_t* neighbors, void* stream);
 
 /* x = act(emb(z))   EmbeddingBlock.forward, comenet.py:125-127 */
 int dig3d_comenet_embed(const int64_t* z, const float* emb, int64_t n_nodes, float* x, void* stream);
