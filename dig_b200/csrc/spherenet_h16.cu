@@ -53,7 +53,8 @@ __device__ __forceinline__ void h_regs_ctrl() { asm volatile("setmaxnreg.dec.syn
 __device__ __forceinline__ void h_regs_epi() { asm volatile("setmaxnreg.inc.sync.aligned.u32 104;"); }
 constexpr float H_SA = 8.0f, H_SW = 64.0f;
 constexpr float H_INV = 1.0f / (H_SA * H_SW);
-// |activation| limit of the chain: 65504 / H_SA = 8188
+// |activation| limit of the chain: the split rounds x * H_SA to fp16, which overflows to inf from 65520 (the midpoint
+// between 65504 and 2^16) on, so |x| must stay below 65520 / H_SA = 8190
 constexpr int H_LDS = 129;                         // row stride (floats) of the fp32 staging overlay of a tile's planes
 
 struct HSmem {
@@ -836,9 +837,11 @@ sphere_update_e_h16_kernel(const float* __restrict__ m, const float* __restrict_
         for (int h = 0; h < 2; ++h) {
           const int row = fr + 8 * h, col = 8 * j + fc, i = 4 * j + 2 * h;
           const float2 b = *reinterpret_cast<const float2*>(&s.bias_a[0][col]);
-          if (row < rows)
-            *reinterpret_cast<float2*>(P.x_ji + (size_t)(e0 + row) * 128 + col) =
-                make_float2(hswish<FAST>(fmaf(acc[i], H_INV, b.x)), hswish<FAST>(fmaf(acc[i + 1], H_INV, b.y)));
+          if (row < rows) {
+            const float2 o = make_float2(hswish<FAST>(fmaf(acc[i], H_INV, b.x)), hswish<FAST>(fmaf(acc[i + 1], H_INV, b.y)));
+            bad |= !(h_finite(o.x) && h_finite(o.y));   // e1 (part A's split operand) out of range: the flag of RE_A
+            *reinterpret_cast<float2*>(P.x_ji + (size_t)(e0 + row) * 128 + col) = o;
+          }
         }
       if (MODE == RE_A) { cp_async_wait_all(); r_bar(cw); }   // rbf of the unit: visible to all
       tp(tr, 3);
@@ -891,9 +894,11 @@ sphere_update_e_h16_kernel(const float* __restrict__ m, const float* __restrict_
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             const int row = fr + 8 * h, i = 4 * j + 2 * h;
-            if (row < rows)
-              *reinterpret_cast<float2*>(P.x_down + (size_t)(e0 + row) * 64 + 8 * j + fc) =
-                  make_float2(hswish<FAST>(a64[i] * H_INV), hswish<FAST>(a64[i + 1] * H_INV));
+            if (row < rows) {
+              const float2 o = make_float2(hswish<FAST>(a64[i] * H_INV), hswish<FAST>(a64[i + 1] * H_INV));
+              bad |= !(h_finite(o.x) && h_finite(o.y));   // x_kj's split (lin_down's operand) out of range
+              *reinterpret_cast<float2*>(P.x_down + (size_t)(e0 + row) * 64 + 8 * j + fc) = o;
+            }
           }
         tp(tr, 3);
       }
@@ -1246,7 +1251,10 @@ linear_h16_kernel(const float* __restrict__ x, int n_rows, int ldx, HLinParams P
       else h_drain<NC / 16, false>(s, c, col0, KU / 8, acc);
     }
 #pragma unroll
-    for (int i = 0; i < NC; ++i) acc[i] = fmaf(acc[i], H_INV, s.bias[0][col0 + i]);
+    for (int i = 0; i < NC; ++i) {
+      acc[i] = fmaf(acc[i], H_INV, s.bias[0][col0 + i]);
+      c.bad |= !h_finite(acc[i]);   // an element of x beyond the split's range poisons its row
+    }
     // outputs: y = x W^T + b (nullable) and / or act_out = swish(y); `residual` is added to the LAST of them (the skip
     // connection of a residual layer, or the second GEMM of a sum of two linears), y stays the pre-activation
     const float* res = residual ? residual + (size_t)r0 * ldy : nullptr;

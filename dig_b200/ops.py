@@ -776,7 +776,9 @@ def sphere_update_v_h16(v_in_all, holders, out_channels, v_out_all, cache):
 
 
 def h16_overflow(clear=True):
-    """True if an operand of the 3xFP16 chain left the fp16 range (|activation| >= 8190) since the last clear."""
+    """True if an operand of the 3xFP16 chain left the fp16 range (|activation| >= 8190) since the last clear.  Every
+    3xFP16 entry point (init_e, update_e parts A / B / BA, update_v, linear_h16) raises it in the launch whose outputs
+    the out-of-range operand turned into inf / NaN."""
     return bool(_lib.load().dig3d_h16_overflow(int(bool(clear))))
 
 

@@ -301,7 +301,9 @@ int dig3d_tc_set_fast_swish(int32_t on);
  * spherenet.py:150-182, init.forward spherenet.py:79-91); `w` is a dig3d_tc_update_e whose p_* members point to
  * dig3d_h16_pack output (4*N*K bytes per matrix: K/32 slabs of [hi|lo][4][N][8 halves], w*64 = hi + lo).
  * Activations must stay below 8190 in magnitude: larger values poison the affected energies with inf/NaN and
- * raise the flag returned by dig3d_h16_overflow (the *_tc chain has fp32 range and is the fallback). */
+ * raise the flag returned by dig3d_h16_overflow -- every 3xFP16 entry point (init_e, update_e parts A / B / BA,
+ * update_v, linear_h16) raises it in the launch whose outputs became non-finite (the *_tc chain has fp32 range and
+ * is the fallback). */
 int64_t dig3d_h16_packed_bytes(int32_t n, int32_t k);
 int dig3d_h16_pack(const float* const* weights, const int32_t* n, const int32_t* k, void* const* outs, int32_t count,
                    void* stream);
