@@ -106,6 +106,8 @@ SIGNATURES = {
     "dig3d_sphere_update_e_a_h16": [P, P, c_int64, POINTER(TcUpdateE), P, P, P],
     "dig3d_sphere_update_e_b_h16": [P, P, P, P, P, c_int64, POINTER(TcUpdateE), P, P, P],
     "dig3d_sphere_update_e_ba_h16": [P, P, P, P, P, c_int64, POINTER(TcUpdateE), POINTER(TcUpdateE), P, P, P, P, P],
+    "dig3d_sphere_init_update_e_a_h16": [P, P, P, P, c_int64, POINTER(InitEWeights), P, P, P, POINTER(TcUpdateE), P, P,
+                                         P, P, P],
     "dig3d_sphere_update_v_h16_supported": [c_int32, c_int32, c_int32, c_int32],
     "dig3d_sphere_update_v_h16": [P, c_int64, c_int32, c_int32, c_int32, P, P, P, P],
     "dig3d_h16_pack_t": [P, P, P, P, P, c_int32, P],

@@ -1,7 +1,8 @@
 // SphereNet / DimeNet++ dense chains on 3xFP16 wgmma.  Two engines:
-//   * update_e (parts A and B of an interaction block) runs on the register-accumulator engine (section "update_e:
-//     register-accumulator engine" below): activations stay in wgmma register fragments from layer to layer.
-//   * init_e, update_v and the generic linear run on the second-generation two-tile store engine: TWO 128-edge tiles in
+//   * init_e, update_e (parts A and B of an interaction block) and update_v run on the register-accumulator engine
+//     (section "update_e: register-accumulator engine" below): activations stay in wgmma register fragments (update_v:
+//     in per-consumer operand planes) from layer to layer.
+//   * the generic linear runs on the second-generation two-tile store engine: TWO 128-edge tiles in
 //     flight per CTA (one CTA per SM), accumulators handed to row-per-thread epilogues through the accumulator store.
 //
 // The two-tile store engine:
@@ -63,11 +64,9 @@ struct HSmem {
   float bias[8][128];
   float wr[128 * 8];
   int dst[2][H_M];
-  int aux[2][2][H_M];                              // init_e: atomic numbers of the target / source node of each row
   // d_ready / d_free are indexed [tile][accumulator]: each barrier has ONE waiter that sees every phase in order
   // (a parity wait may never lag or lead its barrier by two phases, which a barrier shared by the tiles allows)
   uint64_t full[H_STAGES], empty[H_STAGES], a_ready[2], d_ready[2][2], d_free[2][2];
-  uint64_t l_done;                                 // shared-A mode: every MMA of the layer has completed
   uint32_t tmem_base;
 };
 static_assert(sizeof(HSmem) <= 227 * 1024, "HSmem exceeds the shared memory of an SM");
@@ -78,7 +77,7 @@ struct HGemm {
   const unsigned char* w;   // packed slabs (dig3d_h16_pack)
   const float* bias;        // [N] or null
   int K, N;
-  int tile_stride;          // bytes added to `w` for the second job of a layer (shared-A mode: the other N half)
+  int tile_stride;          // bytes added to `w` for the second tile's job of a layer
 };
 
 static __device__ unsigned int g_h16_overflow = 0;
@@ -132,7 +131,6 @@ __device__ __forceinline__ void h_produce(HSmem& s, const HGemm* g, int ng, int 
   ++it;
   if (++r.c == g[r.q].K / H_SLAB_K) { r.c = 0; if (++r.t == ntile) { r.t = 0; ++r.q; } }
 }
-template <bool SHARED_A>
 __device__ __forceinline__ void h_mma_n(HSmem& s, const HGemm* g, int ng, int ntile, uint32_t tmem) {
   const int wt = threadIdx.x;                            // 0..127
   HRing ring = {0, 0, 0};
@@ -144,13 +142,9 @@ __device__ __forceinline__ void h_mma_n(HSmem& s, const HGemm* g, int ng, int nt
   for (int q = 0; q < ng; ++q) {
     const int nslab = g[q].K / H_SLAB_K, n = g[q].N;
     for (int t = 0; t < ntile; ++t) {
-      // SHARED_A: the two jobs of a layer are the two N halves of ONE operand tile (K up to 256: the hi plane spans
-      // s.a[0], the lo plane s.a[1]), published once per layer by all sixteen epilogue warps
-      if (!SHARED_A || t == 0) {
-        mbar_wait(&s.a_ready[SHARED_A ? 0 : t], q & 1);
-        tc_fence_after();
-      }
-      const uint32_t a_hi = smem_u32(SHARED_A ? s.a[0][0] : s.a[t][0]), a_lo = smem_u32(SHARED_A ? s.a[1][0] : s.a[t][1]);
+      mbar_wait(&s.a_ready[t], q & 1);
+      tc_fence_after();
+      const uint32_t a_hi = smem_u32(s.a[t][0]), a_lo = smem_u32(s.a[t][1]);
       for (int c = 0; c < nslab; c += 2, it += 2) {
         const int ab = ch & 1;
         const int lt = ab ? last1 : last0;
@@ -194,7 +188,6 @@ __device__ __forceinline__ void h_mma_n(HSmem& s, const HGemm* g, int ng, int nt
         if (ab) last1 = t; else last0 = t;
         ++ch;
       }
-      if (SHARED_A && t == ntile - 1 && wt == 0) mbar_arrive(&s.l_done);
     }
   }
 }
@@ -240,15 +233,6 @@ __device__ __forceinline__ void h_store_ku(HSmem& s, const HCtx& c, int row, int
   const int o = (ku * H_AKU + row) * 16;
   *reinterpret_cast<uint4*>(c.ahi + o) = make_uint4(h[0], h[1], h[2], h[3]);
   *reinterpret_cast<uint4*>(c.alo + o) = make_uint4(l[0], l[1], l[2], l[3]);
-}
-__device__ __forceinline__ void h_store_a16(HSmem& s, const HCtx& c, int col, const float (&v8)[16]) {
-  float x[8];
-#pragma unroll
-  for (int u = 0; u < 2; ++u) {
-#pragma unroll
-    for (int i = 0; i < 8; ++i) x[i] = v8[8 * u + i];
-    h_store_ku(s, c, c.row, (col >> 3) + u, x);
-  }
 }
 __device__ __forceinline__ bool h_finite(float x) { return fabsf(x) <= 3.402823466e38f; }
 // Cooperative load of a row-major [rows x KU*8] fp32 tile (leading dimension ld floats) into the tile's planes:
@@ -343,7 +327,6 @@ __device__ __forceinline__ void h_setup(HSmem& s, int a_ready_warps = H_TILE_WAR
       mbar_init(&s.a_ready[i], a_ready_warps);
       for (int j = 0; j < 2; ++j) { mbar_init(&s.d_ready[i][j], 1); mbar_init(&s.d_free[i][j], d_free_warps); }
     }
-    mbar_init(&s.l_done, 1);
     mbar_fence_init();
   }
   if ((threadIdx.x >> 5) == 0) tmem_alloc(&s.tmem_base, 512);
@@ -354,27 +337,6 @@ __device__ __forceinline__ void h_finish(HSmem& s, const HCtx* c) {
   __syncthreads();
   if ((threadIdx.x >> 5) == 0) tmem_dealloc(s.tmem_base, 512);
 }
-// Row-major [rows x W] fp32 tile (W = 128 or 64) -> global memory with full-line stores: every thread parks its W/2
-// values in a [128][W + 1] staging overlay of the tile's planes (lane = row: conflict free), then each warp writes
-// whole rows (a direct store from the row-per-thread layout touches 32 lines with 16 bytes each per instruction).
-template <int W>
-__device__ __forceinline__ void h_store_tile_coalesced(HSmem& s, const HCtx& c, int col0, const float (&v)[W / 2],
-                                                       float* __restrict__ out, int rows) {
-  constexpr int LD = W + 1, RPW = 128 / W;            // rows written per warp instruction (float4 per lane)
-  float* st = reinterpret_cast<float*>(s.a[c.t][0]);
-#pragma unroll
-  for (int i = 0; i < W / 2; ++i) st[c.row * LD + col0 + i] = v[i];
-  h_tile_bar(c.t);
-  const int w = c.et >> 5, lane = c.et & 31;
-  for (int r0 = w * RPW; r0 < rows; r0 += H_TILE_WARPS * RPW) {
-    const int r = r0 + (RPW == 2 ? (lane >> 4) : 0), c4 = 4 * (RPW == 2 ? (lane & 15) : lane);
-    if (r < rows) {
-      const float* src = st + r * LD + c4;
-      *reinterpret_cast<float4*>(out + (size_t)r * W + c4) = make_float4(src[0], src[1], src[2], src[3]);
-    }
-  }
-}
-
 // Same with an output leading dimension (the tile is a column slice of a wider row-major matrix).
 // `res` (nullable, same leading dimension): added to the tile in the coalesced store phase (fused residual / skip add).
 template <int W>
@@ -399,29 +361,6 @@ __device__ __forceinline__ void h_store_tile_strided(HSmem& s, const HCtx& c, in
       *reinterpret_cast<float4*>(out + (size_t)r * ld + c4) = o;
     }
   }
-}
-
-// e2 tile (staged as [128][H_LDS] fp32 over the tile's own planes) -> segmented edge -> node sums; the tile's 256
-// threads take one column and one half of the rows each.  Rows are target-sorted: only the first and the last
-// segment of a half can be shared with another half / tile (atomics), interior segments are plain stores.
-__device__ __forceinline__ void h_segment_sums(const HSmem& s, const HCtx& c, int rows, float* __restrict__ v_in) {
-  const int col = c.et & 127, r0 = (c.et >> 7) * 64, r1 = min(rows, r0 + 64);
-  if (r0 >= r1) return;
-  const float* e2t = reinterpret_cast<const float*>(s.a[c.t][0]);
-  const int* dst = s.dst[c.t];
-  float run = 0.f;
-  int cur = dst[r0];
-  bool first = true;
-  for (int r = r0; r < r1; ++r) {
-    const int d = dst[r];
-    if (d != cur) {
-      if (first) atomicAdd(v_in + (size_t)cur * 128 + col, run);
-      else v_in[(size_t)cur * 128 + col] = run;
-      first = false; run = 0.f; cur = d;
-    }
-    run += e2t[r * H_LDS + col];
-  }
-  atomicAdd(v_in + (size_t)cur * 128 + col, run);
 }
 
 // ---------------------------------------------------------------------------------- weight packing
@@ -491,13 +430,19 @@ struct RSmem {
 };
 static_assert(sizeof(RSmem) <= 227 * 1024, "RSmem exceeds the shared memory of an SM");
 
-enum { RE_B = 0, RE_BA = 1, RE_A = 2 };   // part B; part B + part A of the next block; part A
+// part B; part B + part A of the next block; part A; init_e; init_e + part A of block 0
+enum { RE_B = 0, RE_BA = 1, RE_A = 2, RE_I = 3, RE_IA = 4 };
 struct REParams {
   HGemm g[11];                          // B: lin_up, res0.lin1, res0.lin2, lin, res1.lin1, res1.lin2, res2.lin1, res2.lin2
                                         // BA: + lin_ji, lin_kj, lin_down of the NEXT block;  A: lin_ji, lin_kj, lin_down
-  const float* w_rbf;                   // B: lin_rbf [128, 6]
+                                        // I: init lin (K = 128 rbf panel, or K = 384 = three panels);  IA: + part A
+  const float* w_rbf;                   // B: lin_rbf [128, 6];  I: init lin_rbf_1 [128, 6]
   const float *w_rbf1, *w_rbf2;         // A: lin_rbf1 [8, 6], lin_rbf2 [128, 8] (BA: of the next block)
   float *x_ji, *x_down;                 // A: outputs (BA: of the next block)
+  const int64_t* z;                     // I: atomic numbers
+  const int32_t* src;                   // I: source node of each edge
+  const float *emb, *w_rbf0, *b_rbf0, *b_lin;   // I: init weights (emb: three-panel form)
+  const float *tab_i, *tab_j;           // I, table form: [emb rows, 128] = emb W[:, 0:128]^T and emb W[:, 128:256]^T
 };
 
 __device__ __forceinline__ void r_bar(int cw) { asm volatile("bar.sync %0, %1;" ::"r"(1 + cw), "n"(R_WG) : "memory"); }
@@ -596,6 +541,31 @@ __device__ __forceinline__ void r_complete(RSmem& s, float (&acc)[N / 2], const 
     for (int i = 0; i < N / 2; ++i) acc[i] = __fadd_rn(acc[i], d[i]);
   }
 }
+// a K = 128 panel issued into acc (chunk 0) and d (chunk 1) on top of the earlier panels' sum parked in the consumer
+// tile: acc = (tile + chunk 0) + chunk 1, the chunk order of the store engine's drains
+__device__ __forceinline__ void r_complete_onto(RSmem& s, float (&acc)[64], const float (&d)[64], const float* tile,
+                                                int fr, int fc, int& it) {
+  wg_wait0();
+  r_release(s, it, 4);
+  it += 4;
+#pragma unroll
+  for (int j = 0; j < 16; ++j)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int i = 4 * j + 2 * h;
+      const float2 t = *reinterpret_cast<const float2*>(tile + (fr + 8 * h) * R_LDS + 8 * j + fc);
+      acc[i] = __fadd_rn(__fadd_rn(t.x, acc[i]), d[i]);
+      acc[i + 1] = __fadd_rn(__fadd_rn(t.y, acc[i + 1]), d[i + 1]);
+    }
+}
+// the thread's fragment elements -> the consumer tile
+__device__ __forceinline__ void r_park(const float (&acc)[64], float* tile, int fr, int fc) {
+#pragma unroll
+  for (int j = 0; j < 16; ++j)
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+      *reinterpret_cast<float2*>(tile + (fr + 8 * h) * R_LDS + 8 * j + fc) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+}
 // a consumer without a unit in this round still passes every slab of it (the ring counts both consumers per stage)
 __device__ __forceinline__ void r_skip(RSmem& s, int& it, int n) {
   for (int i = 0; i < n; ++i, ++it) {
@@ -627,15 +597,18 @@ __device__ __forceinline__ void r_segment_sums(const float* tile, const int* dst
 }
 
 // MODE = RE_B: part B of a block; RE_BA: part B of block l, then part A of block l + 1 on the e1 fragment still in
-// registers (one launch, one e1 read less per block); RE_A: part A on e1 read from memory (layer 0).  Per element the
-// three compute what the store engine computed, so RE_BA == RE_B followed by RE_A bit for bit.
-template <bool FAST, int MODE>
+// registers (one launch, one e1 read less per block); RE_A: part A on e1 read from memory (layer 0); RE_I: init_e
+// (spherenet.py:79-91, edge -> node sum :211); RE_IA: init_e, then part A of block 0 on the e1 fragment.  Per element
+// the modes compute what the store engine computed, so RE_BA == RE_B followed by RE_A and RE_IA == RE_I followed by
+// RE_A bit for bit.  TABLE (RE_I / RE_IA): the embedding panels of init_e come from the tables (ops.init_e_tables).
+template <bool FAST, int MODE, bool TABLE = false>
 __global__ void __launch_bounds__(R_THREADS, 1)
 sphere_update_e_h16_kernel(const float* __restrict__ m, const float* __restrict__ x_ji,
                            const float* __restrict__ e1_in, const float* __restrict__ rbf0,
                            const int32_t* __restrict__ dst, int n_edges, REParams P, float* __restrict__ e1_out,
                            float* __restrict__ v_in) {
-  constexpr int NG = MODE == RE_B ? 8 : MODE == RE_BA ? 11 : 3;   // layers per unit
+  constexpr bool INIT = MODE == RE_I || MODE == RE_IA;
+  constexpr int NG = MODE == RE_B ? 8 : MODE == RE_BA ? 11 : MODE == RE_I ? 1 : MODE == RE_IA ? 4 : 3;   // layers per unit
   extern __shared__ __align__(1024) unsigned char h_raw[];
   RSmem& s = *reinterpret_cast<RSmem*>(h_raw);
   const int tid = threadIdx.x, wg = tid / R_WG;
@@ -650,15 +623,19 @@ sphere_update_e_h16_kernel(const float* __restrict__ m, const float* __restrict_
     for (int i = 0; i < R_STAGES; ++i) { mbar_init(&s.full[i], 1); mbar_init(&s.empty[i], 8); }
     mbar_fence_init();
   }
-  if (MODE != RE_A) {
+  if (INIT) {   // bias[0] = lin.bias, bias[1] = lin_rbf_0.bias (both unscaled), bias[2..7] = lin_rbf_0.weight [128][6]
+    for (int i = tid; i < 128; i += R_THREADS) { s.bias[0][i] = __ldg(P.b_lin + i); s.bias[1][i] = __ldg(P.b_rbf0 + i); }
+    for (int i = tid; i < 128 * 6; i += R_THREADS) (&s.bias[2][0])[i] = __ldg(P.w_rbf0 + i);
+  } else if (MODE != RE_A) {
     for (int i = tid; i < 8 * 128; i += R_THREADS) {
       const float* b = P.g[i / 128].bias;
       s.bias[i / 128][i % 128] = b ? H_SA * __ldg(b + i % 128) : 0.f;          // the chain runs pre-scaled by H_SA
     }
-    for (int i = tid; i < 128 * 8; i += R_THREADS) s.wr[i] = (i % 8 < 6) ? __ldg(P.w_rbf + (i / 8) * 6 + i % 8) : 0.f;
   }
-  if (MODE != RE_B) {
-    constexpr int GA = MODE == RE_A ? 0 : 8;
+  if (MODE != RE_A)
+    for (int i = tid; i < 128 * 8; i += R_THREADS) s.wr[i] = (i % 8 < 6) ? __ldg(P.w_rbf + (i / 8) * 6 + i % 8) : 0.f;
+  if (MODE != RE_B && MODE != RE_I) {
+    constexpr int GA = MODE == RE_A ? 0 : MODE == RE_IA ? 1 : 8;
     for (int i = tid; i < 2 * 128; i += R_THREADS)     // lin_ji's output leaves unscaled, lin_kj's feeds an operand (x H_SA)
       s.bias_a[i / 128][i % 128] = (i / 128 ? H_SA : 1.0f) * __ldg(P.g[GA + i / 128].bias + i % 128);
     for (int i = tid; i < 128 * 8; i += R_THREADS) s.wr2[i] = __ldg(P.w_rbf2 + i);
@@ -718,7 +695,126 @@ sphere_update_e_h16_kernel(const float* __restrict__ m, const float* __restrict_
       cp_async4(&s.rbf[cw][i], rbf0 + (size_t)e0 * 6 + (i < rows * 6 ? i : 0), i < rows * 6);
     RA a;
     float acc[64], d[64];
-    if (MODE != RE_A) {
+    if (INIT) {
+      // e1 = act(lin(cat[x_i, x_j, act(lin_rbf_0(rbf0))])), e2 = lin_rbf_1(rbf0) * e1          spherenet.py:79-91
+      if (wt < R_UNIT) cp_async4(&s.dst[cw][wt], dst + e0 + (wt < rows ? wt : 0), wt < rows);
+      cp_async_commit();
+      int zi[2], zj[2];   // atomic numbers of the target / source node of rows fr, fr + 8 (0 past the last edge)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int e = e0 + fr + 8 * h;
+        const bool ok = fr + 8 * h < rows;
+        zi[h] = ok ? (int)__ldg(P.z + __ldg(dst + e)) : 0;
+        zj[h] = ok ? (int)__ldg(P.z + __ldg(P.src + e)) : 0;
+      }
+      auto embedding_a = [&](const int (&zr)[2]) {   // A = H_SA * emb[z]
+#pragma unroll
+        for (int k = 0; k < 8; ++k)
+#pragma unroll
+          for (int r = 0; r < 4; ++r) {
+            const int h = r & 1, row = fr + 8 * h, col = frag_a_col(wt, k, r);
+            const float2 x = row < rows ? __ldg(reinterpret_cast<const float2*>(P.emb + (size_t)zr[h] * 128 + col))
+                                        : make_float2(0.f, 0.f);
+            r_split(x.x * H_SA, x.y * H_SA, a.hi[k][r], a.lo[k][r]);
+          }
+      };
+      auto rbf_a = [&]() {   // A = H_SA * act(lin_rbf_0(rbf0))                                     spherenet.py:87
+        const float* w0 = &s.bias[2][0];
+#pragma unroll
+        for (int k = 0; k < 8; ++k)
+#pragma unroll
+          for (int r = 0; r < 4; ++r) {
+            const int h = r & 1, row = fr + 8 * h, col = frag_a_col(wt, k, r);
+            float x[2];
+#pragma unroll
+            for (int u = 0; u < 2; ++u) {
+              float t = 0.f;
+#pragma unroll
+              for (int n = 0; n < 6; ++n) t = fmaf(w0[(col + u) * 6 + n], rbf[row * 6 + n], t);
+              x[u] = row < rows ? H_SA * hswish<FAST>(t + s.bias[1][col + u]) : 0.f;
+            }
+            r_split(x[0], x[1], a.hi[k][r], a.lo[k][r]);
+          }
+      };
+      if (TABLE) {
+        // W_i emb[z_i] + W_j emb[z_j] of the thread's elements (L2-resident tables) -> tile, while rbf0 arrives
+#pragma unroll
+        for (int j = 0; j < 16; ++j)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int row = fr + 8 * h, col = 8 * j + fc;
+            const float2 ti = __ldg(reinterpret_cast<const float2*>(P.tab_i + (size_t)zi[h] * 128 + col));
+            const float2 tj = __ldg(reinterpret_cast<const float2*>(P.tab_j + (size_t)zj[h] * 128 + col));
+            *reinterpret_cast<float2*>(tile + row * R_LDS + col) = make_float2(ti.x + tj.x, ti.y + tj.y);
+          }
+        cp_async_wait_all();
+        r_bar(cw);                                                   // rbf / dst of the unit: visible to all
+        rbf_a();
+        r_issue<2, 128>(s, a, acc, d, it);
+        stagger();
+        r_complete<2, 128>(s, acc, d, it);
+#pragma unroll
+        for (int j = 0; j < 16; ++j)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int row = fr + 8 * h, col = 8 * j + fc, i = 4 * j + 2 * h;
+            const float2 t = *reinterpret_cast<const float2*>(tile + row * R_LDS + col);
+            acc[i] = fmaf(acc[i], H_INV, t.x) * (H_SA * H_SW);
+            acc[i + 1] = fmaf(acc[i + 1], H_INV, t.y) * (H_SA * H_SW);
+          }
+      } else {   // K = 384 as three K = 128 panels, A rebuilt between them; six chunks summed in order
+        embedding_a(zi);                                             // panel 0: x_i
+        r_issue<2, 128>(s, a, acc, d, it);
+        stagger();
+        r_complete<2, 128>(s, acc, d, it);
+        r_park(acc, tile, fr, fc);                                   // (the running sum waits in the tile)
+        embedding_a(zj);                                             // panel 1: x_j
+        r_issue<2, 128>(s, a, acc, d, it);
+        r_complete_onto(s, acc, d, tile, fr, fc, it);
+        r_park(acc, tile, fr, fc);
+        cp_async_wait_all();
+        r_bar(cw);
+        rbf_a();                                                     // panel 2: act(lin_rbf_0(rbf0))
+        r_issue<2, 128>(s, a, acc, d, it);
+        r_complete_onto(s, acc, d, tile, fr, fc, it);
+      }
+      // e1 = act(. + b) and the e2 tile; edge -> node sums                                     spherenet.py:211
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int row = fr + 8 * h;
+        float rb[6];
+#pragma unroll
+        for (int n = 0; n < 6; ++n) rb[n] = rbf[row * 6 + n];
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          const int col = 8 * j + fc, i = 4 * j + 2 * h;
+          float e2[2];
+#pragma unroll
+          for (int u = 0; u < 2; ++u) {
+            const float o = hswish<FAST>(fmaf(acc[i + u], H_INV, s.bias[0][col + u]));
+            bad |= !h_finite(o);
+            const float4 w0 = *reinterpret_cast<const float4*>(s.wr + (col + u) * 8);
+            const float2 w1 = *reinterpret_cast<const float2*>(s.wr + (col + u) * 8 + 4);
+            const float gsum = fmaf(w1.y, rb[5], fmaf(w1.x, rb[4], fmaf(w0.w, rb[3], fmaf(w0.z, rb[2],
+                               fmaf(w0.y, rb[1], w0.x * rb[0])))));
+            e2[u] = gsum * o;
+            acc[i + u] = o;
+          }
+          *reinterpret_cast<float2*>(tile + row * R_LDS + col) = make_float2(e2[0], e2[1]);
+        }
+      }
+      r_bar(cw);
+      r_segment_sums(tile, s.dst[cw], rows, wt, v_in);
+#pragma unroll
+      for (int j = 0; j < 16; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = fr + 8 * h, i = 4 * j + 2 * h;
+          if (row < rows)
+            *reinterpret_cast<float2*>(e1_out + (size_t)(e0 + row) * 128 + 8 * j + fc) = make_float2(acc[i], acc[i + 1]);
+        }
+      if (MODE == RE_IA) r_acc_to_a(acc, a, H_SA);        // part A of block 0: operand H_SA * e1
+    } else if (MODE != RE_A) {
       if (wt < R_UNIT) cp_async4(&s.dst[cw][wt], dst + e0 + (wt < rows ? wt : 0), wt < rows);
       r_fetch_rows(tile, x_ji + (size_t)e0 * 128, rows, fr, fc);     // skip rows of q = 0
       r_load_a<4>(a, m + (size_t)e0 * 64, 64, rows, wt);             // A0 = m (K = 64)
@@ -823,7 +919,7 @@ sphere_update_e_h16_kernel(const float* __restrict__ m, const float* __restrict_
       cp_async_commit();
       r_load_a<8>(a, e1_in + (size_t)e0 * 128, 128, rows, wt);
     }
-    if (MODE != RE_B) {
+    if (MODE != RE_B && MODE != RE_I) {
       // G0: x_ji = act(lin_ji(e1))                                                spherenet.py:154
       tp(tr, 0);
       r_issue<2, 128>(s, a, acc, d, it);
@@ -909,11 +1005,11 @@ sphere_update_e_h16_kernel(const float* __restrict__ m, const float* __restrict_
   if (probe && cw == 0) { g_h16_trace[102] = clock64(); g_h16_trace[103] = (long long)global_ns(); }
 }
 
-template <int MODE>
+template <int MODE, bool TABLE = false>
 static int launch_update_e_h16(const float* m, const float* x_ji, const float* e1_in, const float* rbf0,
                                const int32_t* dst, int64_t n_edges, const REParams& P, float* e1_out, float* v_in,
                                cudaStream_t st) {
-  auto kfn = h16_fast_swish ? sphere_update_e_h16_kernel<true, MODE> : sphere_update_e_h16_kernel<false, MODE>;
+  auto kfn = h16_fast_swish ? sphere_update_e_h16_kernel<true, MODE, TABLE> : sphere_update_e_h16_kernel<false, MODE, TABLE>;
   cudaError_t e = cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(RSmem));
   if (e != cudaSuccess) {
     set_error("cudaFuncSetAttribute(%zu): %s", sizeof(RSmem), cudaGetErrorString(e));
@@ -929,159 +1025,17 @@ static int launch_update_e_h16(const float* m, const float* x_ji, const float* e
   return DIG3D_OK;
 }
 
-// ---------------------------------------------------------------------------------- init_e
-// e1 = act(lin(cat[x_i, x_j, act(lin_rbf_0(rbf))])), e2 = lin_rbf_1(rbf) * e1        spherenet.py:79-91
-// K = 384 as three K = 128 panels whose A operand is rebuilt between panels; the chunk sums keep accumulating in
-// the epilogue registers across the panels.
-struct HInitParams {
-  HGemm g[3];
-  const float *emb, *w_rbf0, *b_rbf0, *b_lin, *w_rbf1;
-  const float *tab_i, *tab_j;   // TABLE: [emb rows, 128] = emb W[:, 0:128]^T and emb W[:, 128:256]^T
-};
-
-// TABLE: lin(cat[x_i, x_j, rbf0]) = W_i emb[z_i] + W_j emb[z_j] + W_r rbf0 + b, and the first two terms depend on the
-// ATOMIC NUMBER only: they are two [emb rows, 128] tables computed once per parameter version in exact fp32
-// (ops.init_e_tables), gathered into the stash while the single remaining K = 128 panel (the rbf part) runs, and
-// added in the final epilogue -- one job per tile instead of three (a job of the two-tile chain is ~10 us, §4.5).
-template <bool FAST, bool TABLE>
-__global__ void __launch_bounds__(H_THREADS, 1)
-sphere_init_e_h16_kernel(const int64_t* __restrict__ z, const int32_t* __restrict__ src,
-                         const int32_t* __restrict__ dst, const float* __restrict__ rbf0, int n_edges, HInitParams P,
-                         float* __restrict__ e1, float* __restrict__ v_in) {
-  extern __shared__ __align__(1024) unsigned char h_raw[];
-  HSmem& s = *reinterpret_cast<HSmem*>(h_raw);
-  const int tid = threadIdx.x, warp = tid >> 5;
-  const int n_tiles = (n_edges + H_M - 1) / H_M, tile0 = blockIdx.x * 2, ntile = min(2, n_tiles - tile0);
-  float* w0 = &s.bias[2][0];   // lin_rbf_0.weight [128][6] parked in the unused bias rows
-  h_setup(s);
-  for (int i = tid; i < 128; i += H_THREADS) { s.bias[0][i] = __ldg(P.b_lin + i); s.bias[1][i] = __ldg(P.b_rbf0 + i); }
-  for (int i = tid; i < 128 * 6; i += H_THREADS) w0[i] = __ldg(P.w_rbf0 + i);
-  for (int i = tid; i < 128 * 8; i += H_THREADS) s.wr[i] = (i % 8 < 6) ? __ldg(P.w_rbf1 + (i / 8) * 6 + i % 8) : 0.f;
-  for (int i = tid; i < 2 * H_M; i += H_THREADS) {
-    const int t = i / H_M, r = i % H_M, e = (tile0 + t) * H_M + r;
-    const int d = (e < n_edges) ? dst[e] : -1, sj = (e < n_edges) ? src[e] : -1;
-    s.dst[t][r] = d;
-    s.aux[t][0][r] = d >= 0 ? (int)z[d] : 0;
-    s.aux[t][1][r] = sj >= 0 ? (int)z[sj] : 0;
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  HCtx c;
-  bool epi = false;
-  if (warp < H_CTRL_WARPS) {
-    h_regs_ctrl();
-    h_mma_n<false>(s, P.g, TABLE ? 1 : 3, ntile, s.tmem_base);
-  } else if (h_regs_epi(), (c = h_ctx(s, ntile)).t < ntile) {
-    epi = true;
-    const int e0 = (tile0 + c.t) * H_M, rows = min(H_M, n_edges - e0);
-    const bool valid = c.row < rows;
-    const size_t ge = (size_t)(e0 + c.row);
-    const int col0 = c.half * 64;
-    const uint32_t stash = c.tl + 256u + 128u * c.t + col0;      // TABLE: the row's table sums wait here
-    float rb[6];
-#pragma unroll
-    for (int n = 0; n < 6; ++n) rb[n] = valid ? __ldg(rbf0 + ge * 6 + n) : 0.f;
-    auto fill_embedding = [&](const int* zrow) {   // A = emb[z[node of row]]
-#pragma unroll
-      for (int k = 0; k < H_M * 16 / H_TILE_THREADS; ++k) {
-        const int f = c.et + k * H_TILE_THREADS, row = f >> 4, ku = f & 15;
-        float x[8];
-        if (row < rows) {
-          const float* er = P.emb + (size_t)zrow[row] * 128 + ku * 8;
-          const float4 p0 = __ldg(reinterpret_cast<const float4*>(er));
-          const float4 p1 = __ldg(reinterpret_cast<const float4*>(er + 4));
-          x[0] = p0.x * H_SA; x[1] = p0.y * H_SA; x[2] = p0.z * H_SA; x[3] = p0.w * H_SA;
-          x[4] = p1.x * H_SA; x[5] = p1.y * H_SA; x[6] = p1.z * H_SA; x[7] = p1.w * H_SA;
-        } else {
-#pragma unroll
-          for (int i = 0; i < 8; ++i) x[i] = 0.f;
-        }
-        h_store_ku(s, c, row, ku, x);
-      }
-    };
-    float acc[64];
-    if (!TABLE) {
-      fill_embedding(s.aux[c.t][0]);                  // panel 0: x_i
-      h_epi_done(s, c.t);
-      h_drain<4, true>(s, c, col0, 2, acc);
-      fill_embedding(s.aux[c.t][1]);                  // panel 1: x_j
-      h_epi_done(s, c.t);
-      h_drain<4, false>(s, c, col0, 2, acc);
-    }
-#pragma unroll
-    for (int p = 0; p < 4; ++p) {                   // panel 2: act(lin_rbf_0(rbf))        spherenet.py:87
-      float v[16];
-#pragma unroll
-      for (int i = 0; i < 16; ++i) {
-        const int col = col0 + 16 * p + i;
-        float a = 0.f;
-#pragma unroll
-        for (int n = 0; n < 6; ++n) a = fmaf(w0[col * 6 + n], rb[n], a);
-        v[i] = valid ? H_SA * hswish<FAST>(a + s.bias[1][col]) : 0.f;
-      }
-      h_store_a16(s, c, col0 + 16 * p, v);
-    }
-    h_epi_done(s, c.t);
-    if (TABLE) {
-      // W_i emb[z_i] + W_j emb[z_j] of this row (L2-resident tables) -> stash, under the panel's MMAs
-      const float* ti = P.tab_i + (size_t)s.aux[c.t][0][c.row] * 128 + col0;
-      const float* tj = P.tab_j + (size_t)s.aux[c.t][1][c.row] * 128 + col0;
-#pragma unroll
-      for (int p = 0; p < 4; ++p) {
-        uint32_t r[16];
-#pragma unroll
-        for (int i = 0; i < 16; i += 4) {
-          const float4 a = __ldg(reinterpret_cast<const float4*>(ti + 16 * p + i));
-          const float4 b = __ldg(reinterpret_cast<const float4*>(tj + 16 * p + i));
-          r[i] = __float_as_uint(a.x + b.x); r[i + 1] = __float_as_uint(a.y + b.y);
-          r[i + 2] = __float_as_uint(a.z + b.z); r[i + 3] = __float_as_uint(a.w + b.w);
-        }
-        tmem_st16(stash + 16 * p, r);
-      }
-      tmem_st_wait();
-      h_drain<4, true>(s, c, col0, 2, acc);
-#pragma unroll
-      for (int p = 0; p < 4; ++p) {
-        uint32_t r[16];
-        tmem_ld16(stash + 16 * p, r);
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 16; ++i) acc[16 * p + i] = fmaf(acc[16 * p + i], H_INV, __uint_as_float(r[i])) * (H_SA * H_SW);
-      }
-    } else {
-      h_drain<4, false>(s, c, col0, 2, acc);
-    }
-    // e1 = act(. + b), e2 = lin_rbf_1(rbf) * e1 (tile staged over the planes), edge -> node sums, coalesced e1 store
-    float* e2t = reinterpret_cast<float*>(s.a[c.t][0]);
-#pragma unroll
-    for (int i = 0; i < 64; ++i) {
-      const int col = col0 + i;
-      const float o = hswish<FAST>(fmaf(acc[i], H_INV, s.bias[0][col]));
-      c.bad |= !h_finite(o);
-      const float4 w0 = *reinterpret_cast<const float4*>(s.wr + col * 8);
-      const float2 w1 = *reinterpret_cast<const float2*>(s.wr + col * 8 + 4);
-      const float gsum = fmaf(w1.y, rb[5], fmaf(w1.x, rb[4], fmaf(w0.w, rb[3], fmaf(w0.z, rb[2],
-                         fmaf(w0.y, rb[1], w0.x * rb[0])))));
-      e2t[c.row * H_LDS + col] = gsum * o;
-      acc[i] = o;
-    }
-    h_tile_bar(c.t);
-    h_segment_sums(s, c, rows, v_in);
-    h_tile_bar(c.t);
-    h_store_tile_coalesced<128>(s, c, col0, acc, e1 + (size_t)e0 * 128, rows);
-  }
-  h_finish(s, epi ? &c : nullptr);
-}
-
 // ---------------------------------------------------------------------------------- update_v (node MLP)
 // v = lin_up(v_in) ; v = act(lins[l](v)) ... ; out = lin(v)                              spherenet.py:212-215
-// H = 128 -> O = 256 -> O ... -> out_channels on the same engine in SHARED-A mode: one 128-node tile per CTA whose
-// operand (K up to 256) spans both plane regions; the two jobs of a layer are the two 128-column halves of its
-// output, drained by the two epilogue groups.  Group X activates its half while the tensor core still runs group
-// Y's half; both write the next operand only after every MMA of the layer has completed (l_done).  The last linear
-// (out_channels <= 4) is a dot product over the activated row, reduced in a fixed order through shared memory.
-// All blocks (init_v + update_vs) run in one launch: blockIdx.y selects the block's weights.
+// H = 128 -> O = 256 -> O ... -> out_channels on the register-accumulator engine's roles (producer warpgroup with the
+// cp.async.bulk ring, two consumer warpgroups on 64-node units, setmaxnreg 40 / 232).  A K = 256 operand does not fit
+// in registers next to an m64n256 accumulator pair, so each consumer keeps its operand in shared memory as fp16 hi / lo
+// planes (64 rows x 256, wgmma with A from shared memory) and computes a 256-wide layer as two N = 128 halves: the first
+// half's activated values stay in registers while the second half runs, then both become the next operand.  The
+// per-element arithmetic is the store engine's (pre-scales, split, K = 64 chunks summed in order, bias / swish).  The
+// final 256 -> out_channels dot product: each thread sums its 64 columns of a row in column order, the four threads of
+// a row are added in a fixed butterfly order.  All blocks (init_v + update_vs) run in one launch: the units of a pair of
+// consumers belong to the same block (both read the same weight slabs), pairs are dealt round-robin over the grid.
 struct HVBlock {
   const unsigned char* p[9];     // packed lin_up [256 x 128], lins[l] [256 x 256] (rows 0..127 then 128..255)
   const float* b[9];             // biases [256]
@@ -1089,114 +1043,220 @@ struct HVBlock {
 };
 struct HVParams { HVBlock blk[8]; int n_lins, out_channels; };
 
-template <bool FAST>
-__global__ void __launch_bounds__(H_THREADS, 1)
-sphere_update_v_h16_kernel(const float* __restrict__ v_in_all, int n_nodes, HVParams P, float* __restrict__ v_out_all) {
-  extern __shared__ __align__(1024) unsigned char h_raw[];
-  HSmem& s = *reinterpret_cast<HSmem*>(h_raw);
-  const int tid = threadIdx.x, warp = tid >> 5;
-  const HVBlock& B = P.blk[blockIdx.y];
-  const int r0 = blockIdx.x * H_M, rows = min(H_M, n_nodes - r0);
-  const int ng = P.n_lins + 1, C = P.out_channels;
-  __shared__ HGemm g[9];
-  h_setup(s, 2 * H_TILE_WARPS);
-  if (tid < ng) g[tid] = {B.p[tid], nullptr, tid == 0 ? 128 : 256, 128, (tid == 0 ? 128 : 256) * 128 * 4};
-  // biases of the first four layers live in s.bias ([8][128] floats = 4 x 256), later ones are read from global
-  for (int i = tid; i < min(ng, 4) * 256; i += H_THREADS) (&s.bias[0][0])[i] = H_SA * __ldg(B.b[i / 256] + i % 256);
-  for (int i = tid; i < C * 256; i += H_THREADS) s.wr[i] = __ldg(B.w_out + i);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  if (warp < H_CTRL_WARPS) {
-    h_regs_ctrl();
-    h_mma_n<true>(s, g, ng, 2, s.tmem_base);
-  } else {
-    h_regs_epi();
-    HCtx c = h_ctx(s, 2);
-    c.ahi = s.a[0][0];
-    c.alo = s.a[1][0];
-    const int et2 = tid - H_CTRL_THREADS;           // 0 .. 511 over both groups
-    const int col0 = c.half * 64;                   // within this group's 128-column half
-    const int gcol0 = 128 * c.t + col0;             // output column of acc[0]
-    const float* vin = v_in_all + ((size_t)blockIdx.y * n_nodes + r0) * 128;
-    // A0 = v_in tile (K = 128), all 512 threads
+constexpr int V_STAGES = 6;                                  // K = 32 slabs in flight (N = 128)
+constexpr int V_PLANE = 32 * R_UNIT * 16;                    // bytes of one fp16 plane of a [64 x 256] operand
+struct VSmem {
+  unsigned char a[2][2][V_PLANE];                            // [consumer][hi | lo]: [k-unit][row][8 halves]
+  unsigned char w[V_STAGES][H_STAGE_BYTES];
+  uint64_t full[V_STAGES], empty[V_STAGES];
+};
+static_assert(sizeof(VSmem) <= 227 * 1024, "VSmem exceeds the shared memory of an SM");
+
+// chunk CH (K = 64) of an N = 128 layer half, A from the consumer's planes, slabs it + 2 CH, + 1; same product order as
+// r_chunk (corrections first, the first product starts the chunk)
+__device__ __forceinline__ void v_chunk(VSmem& s, uint32_t a_hi, uint32_t a_lo, int ch, float (&t)[64], int it) {
 #pragma unroll
-    for (int k = 0; k < H_M * 16 / (2 * H_TILE_THREADS); ++k) {
-      const int f = et2 + k * 2 * H_TILE_THREADS, row = f >> 4, ku = f & 15;
-      float x[8];
-      if (row < rows) {
-        const float4 p0 = __ldg(reinterpret_cast<const float4*>(vin + (size_t)row * 128 + ku * 8));
-        const float4 p1 = __ldg(reinterpret_cast<const float4*>(vin + (size_t)row * 128 + ku * 8 + 4));
-        x[0] = p0.x * H_SA; x[1] = p0.y * H_SA; x[2] = p0.z * H_SA; x[3] = p0.w * H_SA;
-        x[4] = p1.x * H_SA; x[5] = p1.y * H_SA; x[6] = p1.z * H_SA; x[7] = p1.w * H_SA;
-      } else {
+  for (int sl = 0; sl < 2; ++sl) {
+    const uint32_t w_hi = smem_u32(s.w[(it + 2 * ch + sl) % V_STAGES]), w_lo = w_hi + 4u * 128 * 16u;
 #pragma unroll
-        for (int i = 0; i < 8; ++i) x[i] = 0.f;
-      }
-      h_store_ku(s, c, row, ku, x);
+    for (int ks = 0; ks < 2; ++ks) {
+      const uint32_t a_off = (uint32_t)((4 * ch + 2 * sl + ks) * 2 * R_UNIT * 16), b_off = (uint32_t)(ks * 2 * 128 * 16);
+      const uint64_t bh = smem_desc(w_hi + b_off, 128 * 16, 128), bl = smem_desc(w_lo + b_off, 128 * 16, 128);
+      mma_f16_ss(t, smem_desc(a_lo + a_off, R_UNIT * 16, 128), bh, (sl | ks) != 0);
+      mma_f16_ss(t, smem_desc(a_hi + a_off, R_UNIT * 16, 128), bl, 1);
     }
-    fence_async_smem();
-    tc_fence_before();
-    __syncwarp();
-    if ((tid & 31) == 0) mbar_arrive(&s.a_ready[0]);
-    float acc[64];
+#pragma unroll
+    for (int ks = 0; ks < 2; ++ks) {
+      const uint32_t a_off = (uint32_t)((4 * ch + 2 * sl + ks) * 2 * R_UNIT * 16), b_off = (uint32_t)(ks * 2 * 128 * 16);
+      mma_f16_ss(t, smem_desc(a_hi + a_off, R_UNIT * 16, 128), smem_desc(w_hi + b_off, 128 * 16, 128), 1);
+    }
+  }
+}
+__device__ __forceinline__ void v_wait_slabs(VSmem& s, int it, int n) {
+  for (int i = 0; i < n; ++i) mbar_wait(&s.full[(it + i) % V_STAGES], ((it + i) / V_STAGES) & 1);
+}
+__device__ __forceinline__ void v_release(VSmem& s, int it, int n) {
+  __syncwarp();
+  if ((threadIdx.x & 31) == 0)
+    for (int i = 0; i < n; ++i) mbar_arrive(&s.empty[(it + i) % V_STAGES]);
+}
+// one N = 128 half of a layer with NCH K = 64 chunks: acc = c0, acc += c1, ... (fp32, round to nearest, in order)
+__device__ __forceinline__ void v_half(VSmem& s, uint32_t a_hi, uint32_t a_lo, int nch, float (&acc)[64],
+                                      float (&d)[64], int& it) {
+  v_wait_slabs(s, it, 2);
+  wg_fence();
+  v_chunk(s, a_hi, a_lo, 0, acc, it);
+  wg_commit();
+  wg_wait0();
+  v_release(s, it, 2);
 #pragma unroll 1
-    for (int q = 0; q < ng; ++q) {
-      h_drain<4, true>(s, c, col0, q == 0 ? 2 : 4, acc);
-      // v8 = H_SA * (acc / (H_SA H_SW) + b) ; layers >= 1 apply the activation
+  for (int ch = 1; ch < nch; ++ch) {
+    v_wait_slabs(s, it + 2 * ch, 2);
+    wg_fence();
+    v_chunk(s, a_hi, a_lo, ch, d, it);
+    wg_commit();
+    wg_wait0();
+    v_release(s, it + 2 * ch, 2);
 #pragma unroll
-      for (int i = 0; i < 64; i += 4) {
-        float4 b;
-        if (q < 4) b = *reinterpret_cast<const float4*>(&(&s.bias[0][0])[q * 256 + gcol0 + i]);
-        else {
-          b = __ldg(reinterpret_cast<const float4*>(B.b[q] + gcol0 + i));
-          b.x *= H_SA; b.y *= H_SA; b.z *= H_SA; b.w *= H_SA;
-        }
-        acc[i] = fmaf(acc[i], H_SA * H_INV, b.x); acc[i + 1] = fmaf(acc[i + 1], H_SA * H_INV, b.y);
-        acc[i + 2] = fmaf(acc[i + 2], H_SA * H_INV, b.z); acc[i + 3] = fmaf(acc[i + 3], H_SA * H_INV, b.w);
-        if (q > 0) {
-          acc[i] = hswish8<FAST>(acc[i]); acc[i + 1] = hswish8<FAST>(acc[i + 1]);
-          acc[i + 2] = hswish8<FAST>(acc[i + 2]); acc[i + 3] = hswish8<FAST>(acc[i + 3]);
+    for (int i = 0; i < 64; ++i) acc[i] = __fadd_rn(acc[i], d[i]);
+  }
+  it += 2 * nch;
+}
+// this thread's fragment elements (x H_SA) of columns [col0, col0 + 128) -> fp16 hi / lo planes
+__device__ __forceinline__ void v_store_a(unsigned char* hi, unsigned char* lo, const float (&v)[64], int col0, int fr,
+                                         int fc) {
+#pragma unroll
+  for (int j = 0; j < 16; ++j)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int col = col0 + 8 * j + fc, i = 4 * j + 2 * h;
+      uint32_t xh, xl;
+      r_split(v[i], v[i + 1], xh, xl);
+      const int o = ((col >> 3) * R_UNIT + fr + 8 * h) * 16 + (col & 7) * 2;
+      *reinterpret_cast<uint32_t*>(hi + o) = xh;
+      *reinterpret_cast<uint32_t*>(lo + o) = xl;
+    }
+}
+
+template <bool FAST>
+__global__ void __launch_bounds__(R_THREADS, 1)
+sphere_update_v_h16_kernel(const float* __restrict__ v_in_all, int n_nodes, int n_blocks, HVParams P,
+                           float* __restrict__ v_out_all) {
+  extern __shared__ __align__(1024) unsigned char h_raw[];
+  VSmem& s = *reinterpret_cast<VSmem*>(h_raw);
+  const int tid = threadIdx.x, wg = tid / R_WG;
+  // (values live across setmaxnreg are recomputed after it)
+  auto upb = [&]() { return (n_nodes + R_UNIT - 1) / R_UNIT; };             // units per block
+  auto ppb = [&]() { return (upb() + 1) / 2; };                              // unit pairs per block
+  auto rounds = [&]() { return (n_blocks * ppb() - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x; };
+  if (tid == 0) {
+    for (int i = 0; i < V_STAGES; ++i) { mbar_init(&s.full[i], 1); mbar_init(&s.empty[i], 8); }
+    mbar_fence_init();
+  }
+  __syncthreads();
+  const int ng = P.n_lins + 1;
+
+  if (wg == 0) {
+    // ---- producer: per pair, every K = 32 slab of both N halves of every layer of the pair's block
+    r_regs_producer();
+    if (tid == 0) {
+      int it = 0;
+      const int nr = rounds(), np = ppb();
+      const uint32_t bytes = 2u * 4u * 128u * 16u;
+      for (int k = 0; k < nr; ++k) {
+        const HVBlock& B = P.blk[(blockIdx.x + k * gridDim.x) / np];
+        for (int q = 0; q < ng; ++q) {
+          const int K = q ? 256 : 128;
+          for (int t = 0; t < 2; ++t)
+            for (int c = 0; c < K / H_SLAB_K; ++c, ++it) {
+              const int st = it % V_STAGES;
+              if (it >= V_STAGES) mbar_wait(&s.empty[st], ((it / V_STAGES) + 1) & 1);
+              mbar_arrive_expect_tx(&s.full[st], bytes);
+              bulk_g2s(s.w[st], B.p[q] + (size_t)t * K * 128 * 4 + (size_t)c * bytes, bytes, &s.full[st]);
+            }
         }
       }
-      mbar_wait(&s.l_done, q & 1);          // every MMA that reads the current operand has completed
-      tc_fence_after();
-      if (q + 1 < ng) {
-#pragma unroll
-        for (int p = 0; p < 4; ++p) {
-          float v16[16];
-#pragma unroll
-          for (int i = 0; i < 16; ++i) v16[i] = acc[16 * p + i];
-          h_store_a16(s, c, gcol0 + 16 * p, v16);
-        }
-        fence_async_smem();
-        tc_fence_before();
-        __syncwarp();
-        if ((tid & 31) == 0) mbar_arrive(&s.a_ready[0]);
-      }
     }
-    // out[row][o] = sum_c v[row][c] * w_out[o][c]: partial sums of this thread's 64 columns, fixed-order reduction
-    float* red = reinterpret_cast<float*>(s.a[0][0]);        // [128][4 slots][C], the operand planes are free now
-    const int slot = 2 * c.t + c.half;
-    for (int o = 0; o < C; ++o) {
-      float part = 0.f;
-#pragma unroll
-      for (int i = 0; i < 64; ++i) part = fmaf(acc[i], s.wr[o * 256 + gcol0 + i], part);
-      red[(c.row * 4 + slot) * C + o] = part * (1.0f / H_SA);
-      c.bad |= !h_finite(part);
-    }
-    asm volatile("bar.sync 3, %0;" ::"n"(2 * H_TILE_THREADS) : "memory");
-    if (slot == 0 && c.row < rows) {
-      float* out = v_out_all + ((size_t)blockIdx.y * n_nodes + r0 + c.row) * C;
-      for (int o = 0; o < C; ++o) {
-        const float* rr = red + (c.row * 4) * C + o;
-        out[o] = ((rr[0] + rr[C]) + rr[2 * C]) + rr[3 * C];
-      }
-    }
-    h_finish(s, &c);
     return;
   }
-  h_finish(s, nullptr);
+
+  // ---- consumers
+  r_regs_consumer();
+  const int cw = threadIdx.x / R_WG - 1, wt = threadIdx.x & (R_WG - 1);
+  const int fr = frag_row(wt), fc = frag_col(wt), C = P.out_channels;
+  const int nr = rounds(), np = ppb(), nu = upb();
+  unsigned char *ahi = s.a[cw][0], *alo = s.a[cw][1];
+  const uint32_t a_hi = smem_u32(ahi), a_lo = smem_u32(alo);
+  int slabs = 2 * 128 / H_SLAB_K + 2 * (ng - 1) * 256 / H_SLAB_K;
+  bool staggered = cw == 1, bad = false;
+  auto stagger = [&]() {
+    if (!staggered) { asm volatile("bar.arrive 3, %0;" ::"n"(2 * R_WG) : "memory"); staggered = true; }
+  };
+  if (cw == 1) asm volatile("bar.sync 3, %0;" ::"n"(2 * R_WG) : "memory");   // after consumer 0's first half is issued
+  int it = 0;
+#pragma unroll 1
+  for (int k = 0; k < nr; ++k) {
+    const int pair = blockIdx.x + k * gridDim.x, blk = pair / np, unit = 2 * (pair % np) + cw;
+    if (unit >= nu) {   // passes every slab of the round (the ring counts both consumers per stage)
+      for (int i = 0; i < slabs; ++i, ++it) {
+        mbar_wait(&s.full[it % V_STAGES], (it / V_STAGES) & 1);
+        v_release(s, it, 1);
+      }
+      continue;
+    }
+    const HVBlock& B = P.blk[blk];
+    const int r0 = unit * R_UNIT, rows = min(R_UNIT, n_nodes - r0);
+    const float* vin = v_in_all + ((size_t)blk * n_nodes + r0) * 128;
+    float h0[64], acc[64], d[64];
+    r_bar(cw);   // the previous unit's MMAs have read the planes
+#pragma unroll
+    for (int j = 0; j < 16; ++j)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int row = fr + 8 * h, i = 4 * j + 2 * h;
+        const float2 x = row < rows ? __ldg(reinterpret_cast<const float2*>(vin + (size_t)row * 128 + 8 * j + fc))
+                                    : make_float2(0.f, 0.f);
+        acc[i] = x.x * H_SA;
+        acc[i + 1] = x.y * H_SA;
+      }
+    v_store_a(ahi, alo, acc, 0, fr, fc);                                 // A0 = v_in (K = 128)
+#pragma unroll 1
+    for (int q = 0; q < ng; ++q) {
+      fence_async_smem();
+      r_bar(cw);                                                           // the operand is complete
+      const int nch = q ? 4 : 2;
+#pragma unroll
+      for (int t = 0; t < 2; ++t) {
+        float* v = t ? acc : h0;
+        v_half(s, a_hi, a_lo, nch, acc, d, it);
+        if (t == 0) stagger();
+        // v8 = H_SA * (acc / (H_SA H_SW) + b) ; layers >= 1 apply the activation
+#pragma unroll
+        for (int j = 0; j < 16; ++j)
+#pragma unroll
+          for (int u = 0; u < 2; ++u) {
+            const float b = H_SA * __ldg(B.b[q] + 128 * t + 8 * j + fc + u);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int i = 4 * j + 2 * h + u;
+              const float x = fmaf(acc[i], H_SA * H_INV, b);
+              v[i] = q > 0 ? hswish8<FAST>(x) : x;
+            }
+          }
+      }
+      if (q + 1 < ng) {
+        r_bar(cw);                                                         // every MMA of the layer has completed
+        v_store_a(ahi, alo, h0, 0, fr, fc);
+        v_store_a(ahi, alo, acc, 128, fr, fc);
+      }
+    }
+    // out[row][o] = sum_c v[row][c] * w_out[o][c]: this thread's 64 columns of each of its two rows in column order,
+    // then the four threads of the row in a fixed order
+    for (int o = 0; o < C; ++o) {
+      float part[2] = {0.f, 0.f};
+#pragma unroll
+      for (int t = 0; t < 2; ++t)
+#pragma unroll
+        for (int j = 0; j < 16; ++j)
+#pragma unroll
+          for (int u = 0; u < 2; ++u) {
+            const float w = __ldg(B.w_out + o * 256 + 128 * t + 8 * j + fc + u);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) part[h] = fmaf(t ? acc[4 * j + 2 * h + u] : h0[4 * j + 2 * h + u], w, part[h]);
+          }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        part[h] += __shfl_xor_sync(0xffffffffu, part[h], 1);
+        part[h] += __shfl_xor_sync(0xffffffffu, part[h], 2);
+        const float y = part[h] * (1.0f / H_SA);
+        bad |= !h_finite(y);
+        const int row = fr + 8 * h;
+        if ((wt & 3) == 0 && row < rows) v_out_all[((size_t)blk * n_nodes + r0 + row) * C + o] = y;
+      }
+    }
+  }
+  stagger();   // consumer 0 of a CTA without units still meets consumer 1 at the start barrier
+  if (bad) atomicOr(&g_h16_overflow, 1u);
 }
 
 // ---------------------------------------------------------------------------------- generic linear (training path)
@@ -1237,7 +1297,7 @@ linear_h16_kernel(const float* __restrict__ x, int n_rows, int ldx, HLinParams P
   bool epi = false;
   if (warp < H_CTRL_WARPS) {
     h_regs_ctrl();
-    h_mma_n<false>(s, P.g, NPANEL, ntile, s.tmem_base);
+    h_mma_n(s, P.g, NPANEL, ntile, s.tmem_base);
   } else if (h_regs_epi(), (c = h_ctx(s, ntile)).t < ntile) {
     epi = true;
     const int r0 = (tile0 + c.t) * H_M, rows = min(H_M, n_rows - r0);
@@ -1592,24 +1652,27 @@ int dig3d_h16_timeouts(void) {
   return (int)v;
 }
 
+// init_e on the register engine: tab_i / tab_j null = the three-panel form (packed = lin.weight [128, 384]), else the
+// table form (packed = its rbf panel W[:, 256:384])
+static void init_e_params(REParams& P, const int64_t* z, const int32_t* src, const dig3d_init_e_weights* w,
+                          const void* packed, const float* tab_i, const float* tab_j) {
+  P.g[0] = {(const unsigned char*)packed, nullptr, tab_i ? 128 : 384, 128};
+  P.w_rbf = w->w_rbf1;
+  P.z = z; P.src = src;
+  P.emb = w->emb; P.w_rbf0 = w->w_rbf0; P.b_rbf0 = w->b_rbf0; P.b_lin = w->b_lin;
+  P.tab_i = tab_i; P.tab_j = tab_j;
+}
+
 int dig3d_sphere_init_e_h16(const int64_t* z, const int32_t* src, const int32_t* dst, const float* rbf0,
                             int64_t n_edges, const dig3d_init_e_weights* w, const void* packed_lin, float* e1,
                             float* v_in, void* stream) {
   DIG3D_REQUIRE(z && src && dst && rbf0 && w && packed_lin && e1 && v_in, "sphere_init_e_h16: null pointer");
   DIG3D_REQUIRE(w->emb && w->w_rbf0 && w->b_rbf0 && w->b_lin && w->w_rbf1, "sphere_init_e_h16: null weight");
   if (n_edges == 0) return DIG3D_OK;
-  HInitParams P;
-  const size_t panel = (size_t)4 * 2 * 4 * 128 * 16;   // four K=32 slabs
-  for (int p = 0; p < 3; ++p) P.g[p] = {(const unsigned char*)packed_lin + p * panel, nullptr, 128, 128};
-  P.emb = w->emb; P.w_rbf0 = w->w_rbf0; P.b_rbf0 = w->b_rbf0; P.b_lin = w->b_lin; P.w_rbf1 = w->w_rbf1;
-  P.tab_i = P.tab_j = nullptr;
-  auto kfn = h16_fast_swish ? sphere_init_e_h16_kernel<true, false> : sphere_init_e_h16_kernel<false, false>;
-  int rc = h_smem_attr((const void*)kfn);
-  if (rc) return rc;
-  const int pairs = ceil_div(ceil_div(n_edges, H_M), 2);
-  kfn<<<pairs, H_THREADS, sizeof(HSmem), (cudaStream_t)stream>>>(z, src, dst, rbf0, (int)n_edges, P, e1, v_in);
-  DIG3D_LAUNCH_CHECK();
-  return DIG3D_OK;
+  REParams P = {};
+  init_e_params(P, z, src, w, packed_lin, nullptr, nullptr);
+  return launch_update_e_h16<RE_I, false>(nullptr, nullptr, nullptr, rbf0, dst, n_edges, P, e1, v_in,
+                                          (cudaStream_t)stream);
 }
 
 int dig3d_sphere_init_e_h16_tab(const int64_t* z, const int32_t* src, const int32_t* dst, const float* rbf0,
@@ -1620,18 +1683,34 @@ int dig3d_sphere_init_e_h16_tab(const int64_t* z, const int32_t* src, const int3
   DIG3D_REQUIRE(w->w_rbf0 && w->b_rbf0 && w->b_lin && w->w_rbf1, "sphere_init_e_h16_tab: null weight");
   DIG3D_REQUIRE((((uintptr_t)tab_i | (uintptr_t)tab_j) & 15) == 0, "sphere_init_e_h16_tab: tables must be 16-byte aligned");
   if (n_edges == 0) return DIG3D_OK;
-  HInitParams P;
-  P.g[0] = {(const unsigned char*)packed_rbf_panel, nullptr, 128, 128};
-  P.g[1] = P.g[2] = P.g[0];
-  P.emb = w->emb; P.w_rbf0 = w->w_rbf0; P.b_rbf0 = w->b_rbf0; P.b_lin = w->b_lin; P.w_rbf1 = w->w_rbf1;
-  P.tab_i = tab_i; P.tab_j = tab_j;
-  auto kfn = h16_fast_swish ? sphere_init_e_h16_kernel<true, true> : sphere_init_e_h16_kernel<false, true>;
-  int rc = h_smem_attr((const void*)kfn);
-  if (rc) return rc;
-  const int pairs = ceil_div(ceil_div(n_edges, H_M), 2);
-  kfn<<<pairs, H_THREADS, sizeof(HSmem), (cudaStream_t)stream>>>(z, src, dst, rbf0, (int)n_edges, P, e1, v_in);
-  DIG3D_LAUNCH_CHECK();
-  return DIG3D_OK;
+  REParams P = {};
+  init_e_params(P, z, src, w, packed_rbf_panel, tab_i, tab_j);
+  return launch_update_e_h16<RE_I, true>(nullptr, nullptr, nullptr, rbf0, dst, n_edges, P, e1, v_in,
+                                         (cudaStream_t)stream);
+}
+
+int dig3d_sphere_init_update_e_a_h16(const int64_t* z, const int32_t* src, const int32_t* dst, const float* rbf0,
+                                     int64_t n_edges, const dig3d_init_e_weights* w_init, const void* packed_init,
+                                     const float* tab_i, const float* tab_j, const dig3d_tc_update_e* w, float* e1,
+                                     float* v_in, float* x_ji, float* x_down, void* stream) {
+  DIG3D_REQUIRE(z && src && dst && rbf0 && w_init && packed_init && w && e1 && v_in && x_ji && x_down,
+                "sphere_init_update_e_a_h16: null pointer");
+  DIG3D_REQUIRE(w_init->w_rbf0 && w_init->b_rbf0 && w_init->b_lin && w_init->w_rbf1 && (tab_i || w_init->emb),
+                "sphere_init_update_e_a_h16: null weight");
+  DIG3D_REQUIRE(!tab_i == !tab_j, "sphere_init_update_e_a_h16: tab_i and tab_j must agree");
+  DIG3D_REQUIRE((((uintptr_t)tab_i | (uintptr_t)tab_j) & 15) == 0,
+                "sphere_init_update_e_a_h16: tables must be 16-byte aligned");
+  if (n_edges == 0) return DIG3D_OK;
+  REParams P = {};
+  init_e_params(P, z, src, w_init, packed_init, tab_i, tab_j);
+  P.g[1] = {(const unsigned char*)w->p_ji, w->b_ji, 128, 128};
+  P.g[2] = {(const unsigned char*)w->p_kj, w->b_kj, 128, 128};
+  P.g[3] = {(const unsigned char*)w->p_down, nullptr, 128, 64};
+  P.w_rbf1 = w->w_rbf1; P.w_rbf2 = w->w_rbf2;
+  P.x_ji = x_ji; P.x_down = x_down;
+  cudaStream_t st = (cudaStream_t)stream;
+  return tab_i ? launch_update_e_h16<RE_IA, true>(nullptr, nullptr, nullptr, rbf0, dst, n_edges, P, e1, v_in, st)
+               : launch_update_e_h16<RE_IA, false>(nullptr, nullptr, nullptr, rbf0, dst, n_edges, P, e1, v_in, st);
 }
 
 int dig3d_sphere_update_e_a_h16(const float* e1, const float* rbf0, int64_t n_edges, const dig3d_tc_update_e* w,
@@ -1781,10 +1860,17 @@ int dig3d_sphere_update_v_h16(const float* v_in_all, int64_t n_nodes, int32_t n_
     P.blk[b].w_out = w[b].w_out;
   }
   auto kfn = h16_fast_swish ? sphere_update_v_h16_kernel<true> : sphere_update_v_h16_kernel<false>;
-  int rc = h_smem_attr((const void*)kfn);
-  if (rc) return rc;
-  dim3 grid(ceil_div(n_nodes, H_M), n_blocks);
-  kfn<<<grid, H_THREADS, sizeof(HSmem), (cudaStream_t)stream>>>(v_in_all, (int)n_nodes, P, v_out_all);
+  cudaError_t e = cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(VSmem));
+  if (e != cudaSuccess) {
+    set_error("cudaFuncSetAttribute(%zu): %s", sizeof(VSmem), cudaGetErrorString(e));
+    return DIG3D_ECUDA;
+  }
+  int dev = 0, n_sm = 132;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
+  const int pairs = n_blocks * (int)ceil_div(ceil_div(n_nodes, R_UNIT), 2);
+  kfn<<<min(n_sm, pairs), R_THREADS, sizeof(VSmem), (cudaStream_t)stream>>>(v_in_all, (int)n_nodes, n_blocks, P,
+                                                                             v_out_all);
   DIG3D_LAUNCH_CHECK();
   return DIG3D_OK;
 }

@@ -180,6 +180,17 @@ __device__ __forceinline__ void mma_f16_rs(float (&d)[64], const uint32_t (&a)[4
       : "memory");
 }
 
+// D[64 x 128] (+)= A[64 x 16] * B[128 x 16]^T, both from shared memory.
+__device__ __forceinline__ void mma_f16_ss(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 " TC90_D64 ", %64, %65, p, 1, 1, 0, 0;\n\t}"
+      : TC90_D64_OPS(d)
+      : "l"(a_desc), "l"(b_desc), "r"(accumulate)
+      : "memory");
+}
+
 // ---- accumulator store (see the header comment)
 // A translation unit that uses the store defines TC90_TM_COLS (columns per slot) before including this header.  The
 // store is static device memory of the library (TM_SLOTS slots of 128 rows x TC90_TM_COLS fp32), so no host-side
@@ -247,14 +258,6 @@ __device__ __forceinline__ void tmem_ld16f(uint32_t taddr, float* r) {
   }
 }
 __device__ __forceinline__ void tmem_ld_wait() {}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&r)[16]) {
-  float4* p = reinterpret_cast<float4*>(tm_ptr(taddr, threadIdx.x & 31));
-#pragma unroll
-  for (int i = 0; i < 4; ++i)
-    __stcg(p + i, make_float4(__uint_as_float(r[4 * i]), __uint_as_float(r[4 * i + 1]), __uint_as_float(r[4 * i + 2]),
-                              __uint_as_float(r[4 * i + 3])));
-}
-__device__ __forceinline__ void tmem_st_wait() {}
 
 // Warpgroup (thread wt = 0..127) writes its m64n64 fragment to the 64 x 64 block whose top-left corner is taddr.
 __device__ __forceinline__ void tm_store_frag(const float (&d)[32], int wt, uint32_t taddr) {

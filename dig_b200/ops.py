@@ -765,7 +765,7 @@ def pack_update_v_h16(holders, cache):
 
 
 def sphere_update_v_h16(v_in_all, holders, out_channels, v_out_all, cache):
-    """All node MLPs of a forward in one launch on the two-tile tensor-core engine (3xFP16 operands).
+    """All node MLPs of a forward in one launch on the register-accumulator engine (3xFP16 operands).
     v_in_all [NB, N, 128], holders: NB update_v modules (128 -> 256 -> ... -> out_channels)."""
     nb, n, _ = v_in_all.shape
     parr, arr, n_lins = pack_update_v_h16(holders, cache)

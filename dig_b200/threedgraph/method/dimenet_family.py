@@ -409,21 +409,30 @@ class _DimeNetFamily(nn.Module):
             call("dig3d_triplet_basis_project_lists", a["bess"], a["angle"], a["torsion"] if tors else None, src, dst,
                  row_ptr, trip_ptr, graph_ptr, batch, E, T, int(self._basis_id), 4, 8, plan["w_s"].data_ptr(),
                  plan["w_t"].data_ptr() if tors else None, a["sbf_p"], a["t_p"] if tors else None, *ops._out_lists(g), st)
+        # Part A of block l + 1 rides on the unit chain of part B of block l (dig3d_sphere_update_e_ba_h16), and part A of
+        # block 0 on init_e's (dig3d_sphere_init_update_e_a_h16): two launches per interaction block (gather, dense chain)
+        # instead of three; DIG3D_FUSE_BA=0 keeps them apart (same results).
+        fuse = os.environ.get("DIG3D_FUSE_BA", "1") != "0"
+        zp = ops._p(z, torch.int64, "z")
         if plan["init_tables"] is not None:
             tab_i, tab_j, packed_rbf = plan["init_tables"]
-            call("dig3d_sphere_init_e_h16_tab", ops._p(z, torch.int64, "z"), src, dst, a["rbf0"], E, byref(plan["init_w"]),
-                 packed_rbf.data_ptr(), tab_i.data_ptr(), tab_j.data_ptr(), a["e1a"], v_in, st)
+            init_args = (packed_rbf.data_ptr(), tab_i.data_ptr(), tab_j.data_ptr())
         else:
-            call("dig3d_sphere_init_e_h16", ops._p(z, torch.int64, "z"), src, dst, a["rbf0"], E, byref(plan["init_w"]),
-                 plan["init_packed"].data_ptr(), a["e1a"], v_in, st)
-        # Part A of block l + 1 rides on the tile chain of part B of block l (dig3d_sphere_update_e_ba_h16): two launches per
-        # interaction block (gather, dense chain) instead of three; DIG3D_FUSE_BA=0 keeps them apart (same results).
-        fuse = os.environ.get("DIG3D_FUSE_BA", "1") != "0"
+            init_args = (plan["init_packed"].data_ptr(), None, None)
+        if fuse and L:
+            call("dig3d_sphere_init_update_e_a_h16", zp, src, dst, a["rbf0"], E, byref(plan["init_w"]), *init_args,
+                 byref(plan["layers"][0]), a["e1a"], v_in, a["x_ji"], a["x_down"], st)
+        elif plan["init_tables"] is not None:
+            call("dig3d_sphere_init_e_h16_tab", zp, src, dst, a["rbf0"], E, byref(plan["init_w"]), *init_args,
+                 a["e1a"], v_in, st)
+        else:
+            call("dig3d_sphere_init_e_h16", zp, src, dst, a["rbf0"], E, byref(plan["init_w"]), init_args[0],
+                 a["e1a"], v_in, st)
         e1, e1_next = a["e1a"], a["e1b"]
         x_ji, x_ji_next = a["x_ji"], a["x_ji2"]
         for l in range(L):
             w = plan["layers"][l]
-            if l == 0 or not fuse:
+            if not fuse:
                 call("dig3d_sphere_update_e_a_h16", e1, a["rbf0"], E, byref(w), x_ji, a["x_down"], st)
             sp = ctypes.c_void_p(a["sbf_p"] + 4 * 8 * T * l)
             tp = ctypes.c_void_p(a["t_p"] + 4 * 8 * T * l) if tors else None

@@ -333,8 +333,18 @@ int dig3d_sphere_update_e_ba_h16(const float* m, const float* e1_in, const float
                                  const int32_t* dst, int64_t n_edges, const dig3d_tc_update_e* w,
                                  const dig3d_tc_update_e* w_next, float* e1_out, float* v_in, float* x_ji_next,
                                  float* x_down_next, void* stream);
-/* update_v.forward after the scatter (spherenet.py:212-215) for ALL blocks of a forward on the same engine (one
- * 128-node tile per CTA, the two 128-column halves of every 256-wide layer in flight); H = 128, O = 256,
+/* init_e (dig3d_sphere_init_e_h16_tab with tab_i / tab_j and packed_init = the rbf panel, or dig3d_sphere_init_e_h16 with
+ * both tables null and packed_init = the packed lin) with part A of block 0 (dig3d_sphere_update_e_a_h16, weights w) on
+ * the e1 fragment in registers: one launch and one read of e1 less; bit-identical to the two launches.  Writes e1,
+ * adds the edge -> node sums into v_in (zeroed by the caller), writes x_ji [E, 128] and x_down [E, 64].
+ *                                                                          spherenet.py:79-91, 150-161 */
+int dig3d_sphere_init_update_e_a_h16(const int64_t* z, const int32_t* src, const int32_t* dst, const float* rbf0,
+                                     int64_t n_edges, const dig3d_init_e_weights* w_init, const void* packed_init,
+                                     const float* tab_i, const float* tab_j, const dig3d_tc_update_e* w, float* e1,
+                                     float* v_in, float* x_ji, float* x_down, void* stream);
+/* update_v.forward after the scatter (spherenet.py:212-215) for ALL blocks of a forward on the register-accumulator
+ * engine's roles (64-node units, operands in per-consumer fp16 planes, every 256-wide layer as two 128-column halves,
+ * unit pairs of one block dealt over the grid); H = 128, O = 256,
  * out_channels <= 4.  packed[b * (n_lins + 1) + l] = dig3d_h16_pack of block b's lin_up (l = 0) / lins[l - 1]
  * as TWO [128, K] matrices back to back (output rows 0..127, then 128..255). */
 int dig3d_sphere_update_v_h16_supported(int32_t hidden, int32_t out_emb, int32_t out_channels, int32_t n_lins);

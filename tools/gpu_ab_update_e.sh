@@ -39,6 +39,11 @@ import glob, json, os, statistics, sys
 import numpy as np
 out = sys.argv[1]
 CHAIN = ("sphere_update_e_ba_h16", "sphere_update_e_b_h16", "sphere_update_e_a_h16")
+# init_e (either form), part A of block 0 (alone, or fused into init_e) and update_v, per step
+OTHER = {"init_e": ("sphere_init_e_h16_tab", "sphere_init_e_h16"),
+         "init_e+part_a": ("sphere_init_update_e_a_h16",),
+         "part_a": ("sphere_update_e_a_h16",),
+         "update_v": ("sphere_update_v_h16",)}
 
 def load(tag):
     with open(os.path.join(out, tag + ".json")) as fh:
@@ -53,6 +58,8 @@ for tree in ("parent", "new"):
           f"| serial {[round(r['serial']['value']) for r in runs]} "
           f"| update_e chain ms/step {[round(sum(r['roofline']['per_step_ms'].get(k, 0) for k in CHAIN), 4) for r in runs]} "
           f"| full run value {full['value']:.0f} serial {full['serial']['value']:.0f} parity {full.get('parity')}")
+    for name, keys in OTHER.items():
+        print(f"  {name} ms/step {[round(sum(r['roofline']['per_step_ms'].get(k, 0) for k in keys), 4) for r in runs]}")
     print(f"  per_step_ms {runs[0]['roofline']['per_step_ms']}")
 a = np.load(os.path.join(out, "dump_parent", "energies.npy"))
 b = np.load(os.path.join(out, "dump_new", "energies.npy"))
