@@ -117,7 +117,6 @@ SIGNATURES = {
     "dig3d_h16_timeouts": [],
     "dig3d_h16_trace": [c_int32, P],
     "dig3d_h16_set_fast_swish": [c_int32],
-    "dig3d_h16_set_wide_epilogue": [c_int32],
     "dig3d_tc_trace": [c_int32, P],
     "dig3d_schnet_block": [P, c_int64, P, P, P, c_int64, P, c_int32, c_double, c_double, c_int32, c_int32,
                            POINTER(SchnetBlockWeights), P, P, P, P],

@@ -460,7 +460,7 @@ static int smem_attr(K kernel, size_t bytes) {
 
 // ---------------------------------------------------------------------------------- EdgeGraphConv aggregation
 // agg[i][c] = sum_{e = (j -> i)} w[e][c] * x[j][c]       (comenet.py:66-73: message x_j * edge_weight, aggr = 'add')
-// for the tensor-engine forward (ComENet._forward_h16): w = lin_feature(feat) comes out of a GEMM on the dense engine as an
+// for an edge filter that is already materialised: w = lin_feature(feat) comes out of a GEMM on the dense engine as an
 // [E, W] matrix; one warp per target node streams its (contiguous, CSR-sorted) rows of w and gathers the source rows of x
 // from L2; lanes own float4 columns, the sum stays in registers, one coalesced row store.  No atomics, no zero fill.
 template <int W4>

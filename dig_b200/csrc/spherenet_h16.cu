@@ -1622,13 +1622,6 @@ int dig3d_h16_set_fast_swish(int32_t on) {
   return DIG3D_OK;
 }
 
-// Selected between the eight- and sixteen-warp epilogues of the two-tile update_e kernels, which the register engine
-// replaced: accepted and ignored (the tests and the model forwards still call it).
-int dig3d_h16_set_wide_epilogue(int32_t on) {
-  (void)on;
-  return DIG3D_OK;
-}
-
 int dig3d_h16_overflow(int32_t clear) {
   unsigned int v = 0;
   cudaMemcpyFromSymbol(&v, g_h16_overflow, sizeof(v));

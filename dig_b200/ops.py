@@ -293,6 +293,11 @@ def pack_update_v(m):
     return w
 
 
+def pack_update_v_array(holders):
+    """UpdateVWeights[len(holders)]: the node-MLP weight structs of a forward, one per block."""
+    return (_lib.UpdateVWeights * len(holders))(*[pack_update_v(h) for h in holders])
+
+
 def sphere_init_e(z, g, rbf0, w, hidden, v_in=None):
     e1 = torch.empty(max(g.n_edges, 1), hidden, dtype=torch.float32, device=rbf0.device)[:g.n_edges]
     if v_in is None:
@@ -325,7 +330,7 @@ def sphere_update_e(e1, g, rbf0, sbf_p, t_p, col0, w, hidden, int_emb, v_in=None
 def sphere_update_v_batched(v_in_all, holders, out_channels, v_out_all):
     """All node MLPs of a forward in one launch.  v_in_all [NB, N, H], holders: NB update_v modules."""
     nb, n, _ = v_in_all.shape
-    arr = (_lib.UpdateVWeights * nb)(*[pack_update_v(h) for h in holders])
+    arr = pack_update_v_array(holders)
     if n:
         call("dig3d_sphere_update_v_batched", _p(v_in_all, torch.float32, "v_in_all", 16), n, nb, int(out_channels),
              arr, _p(v_out_all, align=4), _stream())
@@ -661,7 +666,7 @@ def gather_split(g):
 
 
 def _ptr(x):
-    """Device pointer argument: a raw address (int, internal workspace of the lean inference path) or a validated tensor."""
+    """Device pointer argument: a raw address (int, workspace of the planned inference forward) or a validated tensor."""
     return x if type(x) is int else _p(x)
 
 
@@ -760,8 +765,7 @@ def pack_update_v_h16(holders, cache):
         _, buf, offs = hit
         ptrs += [buf.data_ptr() + offs[2 * l] for l in range(n_lins + 1)]
     parr = (ctypes.c_void_p * len(ptrs))(*ptrs)
-    arr = (_lib.UpdateVWeights * len(holders))(*[pack_update_v(h) for h in holders])
-    return parr, arr, n_lins
+    return parr, pack_update_v_array(holders), n_lins
 
 
 def sphere_update_v_h16(v_in_all, holders, out_channels, v_out_all, cache):
@@ -784,24 +788,6 @@ def h16_overflow(clear=True):
 
 def h16_set_fast_swish(on):
     call("dig3d_h16_set_fast_swish", int(bool(on)))
-
-
-_H16_WIDE = [None]
-
-
-def h16_set_wide_epilogue(on):
-    """No effect since update_e moved to the register-accumulator engine (it chose between the epilogue layouts of the
-    two-tile kernels); kept for existing callers."""
-    call("dig3d_h16_set_wide_epilogue", int(bool(on)))
-    _H16_WIDE[0] = bool(on)
-
-
-def h16_wide_from_env():
-    """Apply DIG3D_H16_WIDE (default 1) once per change; called by the model forwards."""
-    import os
-    want = os.environ.get("DIG3D_H16_WIDE", "1") != "0"
-    if _H16_WIDE[0] is not want:
-        h16_set_wide_epilogue(want)
 
 
 def tc_set_fast_swish(on):

@@ -206,9 +206,7 @@ class ComENet(nn.Module):
         if dense not in ("h16", "simt"):
             raise ValueError(f"DIG3D_COMENET_DENSE={dense!r}: expected h16 or simt")
         if dense == "h16":
-            if os.environ.get("DIG3D_LEAN", "1") != "0" and g.n_nodes and g.n_edges:
-                return self._forward_lean(self._inference_plan(), z, g, f1, f2)
-            return self._forward_h16(z, g, f1, f2)
+            return self._forward_plan(self._inference_plan(), z, g, f1, f2)
         x = ops.comenet_embed(z, self.emb.emb.weight)
         no_head = ops.pack_comenet_head([], None)
         head = ops.pack_comenet_head(self.lins, self.lin_out)
@@ -245,42 +243,15 @@ class ComENet(nn.Module):
             cache[id(blk)] = hit
         return hit[1], hit[2]
 
-    def _forward_h16(self, z, g, f1, f2):
-        """Inference forward (reference comenet.py:386-399, SimpleInteractionBlock.forward :195-215) with every
-        hidden x hidden linear on the two-tile wgmma engine (3xFP16 operands, `dig3d_linear_h16`, swish fused where the
-        reference applies it) and the two EdgeGraphConv aggregations as `dig3d_comenet_filter_sum` (edge filter folded to
-        one [Q, hidden] matrix).  VERDICT r1 item 4; `DIG3D_COMENET_DENSE=simt` selects round 1's fused FFMA block kernel."""
-        lin = ops.linear_h16
-        x = ops.comenet_embed(z, self.emb.emb.weight)                               # swish(emb[z])
-        for blk in self.interaction_blocks:
-            x = lin(x, blk.lin.weight, blk.lin.bias, want_act=True, act_only=True)
-            hs = []
-            for conv, lf, l, feat in ((blk.conv1, blk.lin_feature1, blk.lin1, f1),
-                                      (blk.conv2, blk.lin_feature2, blk.lin2, f2)):
-                agg = ops.comenet_filter_sum(feat, self._filter_t(lf), x, g)
-                # GraphConv: lin_rel(agg) + lin_root(x) -- the second GEMM adds the first in its epilogue
-                h = lin(agg, conv.lin_rel.weight, conv.lin_rel.bias, residual=lin(x, conv.lin_root.weight, None))
-                hs.append(lin(h, l.weight, l.bias, want_act=True, act_only=True))
-            wa, wb = self._cat_halves(blk)
-            # lin_cat(cat[h1, h2]) + x = h1 Wa^T + b + (h2 Wb^T + x)
-            h = lin(hs[0], wa, blk.lin_cat.bias, residual=lin(hs[1], wb, None, residual=x))
-            for l in blk.lins:
-                h = lin(h, l.weight, l.bias, want_act=True, act_only=True, residual=h)      # swish(l(h)) + h
-            h, _, _ = ops.graphnorm(h, g.graph_ptr, blk.norm.weight.detach(), blk.norm.bias.detach(),
-                                    blk.norm.mean_scale.detach(), blk.norm.eps)
-            x = lin(h, blk.final.weight, blk.final.bias)
-        for l in self.lins:
-            x = lin(x, l.weight, l.bias, want_act=True, act_only=True)
-        x = ops.linear(x, self.lin_out.weight.detach(), self.lin_out.bias.detach())
-        return ops.segment_sum(x, g.graph_ptr)
-
-    # ------------------------------------------------------------------ lean inference path (host overhead)
-    # `_forward_h16` is 77 launches of ~20 us kernels behind ~18 us of Python each (module attribute walks, packed-weight
-    # registry look-ups, one or two allocations and six pointer validations per linear): host-bound.  As for the DimeNet
-    # family (DESIGN.md 4.5) everything that depends only on the parameters is resolved once into a plan -- per linear
-    # (packed weight address, bias address, K, N) -- and a forward is the same launch sequence over 256-wide slots of one
-    # workspace with raw addresses.  Bit-identical to `_forward_h16` (DIG3D_LEAN=0;
-    # tests/test_gpu_parity.py::test_comenet_lean_inference_path_is_bit_identical).
+    # ------------------------------------------------------------------ inference on the tensor engine, from a cached plan
+    # Inference forward (reference comenet.py:386-399, SimpleInteractionBlock.forward :195-215) with every hidden x hidden
+    # linear on the two-tile wgmma engine (3xFP16 operands, `dig3d_linear_h16`, swish fused where the reference applies
+    # it) and the two EdgeGraphConv aggregations as `dig3d_comenet_filter_sum` (edge filter folded to one [Q, hidden]
+    # matrix).  The forward is 77 launches of ~20 us kernels; issued op by op through the tensor wrappers, each would sit
+    # behind ~18 us of Python (module attribute walks, packed-weight registry look-ups, allocations, pointer validations).
+    # So, as for the DimeNet family, everything that depends only on the parameters is resolved once into a plan -- per
+    # linear (packed weight address, bias address, K, N) -- and a forward is the launch sequence over 256-wide slots of one
+    # workspace with raw addresses.
     def _inference_plan(self):
         key = ops.plan_key(self)
         plan = self.__dict__.get("_plan")
@@ -318,7 +289,7 @@ class ComENet(nn.Module):
         self.__dict__["_plan"] = plan
         return plan
 
-    def _forward_lean(self, plan, z, g, f1, f2):
+    def _forward_plan(self, plan, z, g, f1, f2):
         call = ops.call
         n, hdim, dev = g.n_nodes, self.emb.emb.weight.size(1), z.device
         ng, oc = g.n_graphs, self.out_channels

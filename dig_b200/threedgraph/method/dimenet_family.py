@@ -275,12 +275,15 @@ class _DimeNetFamily(nn.Module):
                                             lambda p, c: self._exact(self._forward_dual, z, p, c, g, nf),
                                             pos, tuple(self.parameters()))
             return self._exact(self._forward_train, z, pos, g, nf, exact=bool(pos.requires_grad))
-        ops.h16_wide_from_env()
-        if (os.environ.get("DIG3D_DENSE", "h16") == "h16" and g.n_edges and self.num_layers <= 4
-                and os.environ.get("DIG3D_LEAN", "1") != "0"):
-            plan = self._inference_plan()
-            if plan is not None:
-                return self._forward_lean(plan, z, pos, g)
+        # dense edge-MLP chain: "h16" (default) = register-accumulator engine, 3xFP16 operands (csrc/spherenet_h16.cu),
+        # run from the cached plan below; "tc" = first-generation 3xTF32 chain with fp32 operand range
+        # (csrc/spherenet_tc.cu); "simt" = exact-fp32 FFMA twin (csrc/spherenet.cu).  All three are sm_90a kernels of
+        # libdig3d.so.
+        dense = os.environ.get("DIG3D_DENSE", "h16")
+        if dense not in ("h16", "tc", "simt"):
+            raise ValueError(f"DIG3D_DENSE={dense!r}: expected h16, tc or simt")
+        if dense == "h16":
+            return self._forward_plan(self._inference_plan(), z, pos, g)
         ops.triplet_geometry(g, pos, use_torsion=self._torsion, want_idx=False)
         rbf0, bess = ops.edge_basis(g.dist, self.cutoff, self.envelope_exponent, self.emb.dist_emb.freq,
                                     self._basis_id, envelope_on_bessel=not self._torsion, num_radial=nr,
@@ -297,20 +300,8 @@ class _DimeNetFamily(nn.Module):
         dev = pos.device
         v_in_all = torch.zeros(L + 1, g.n_nodes, self.hidden_channels, dtype=torch.float32, device=dev)
         v_all = torch.empty(L + 1, g.n_nodes, self.out_channels, dtype=torch.float32, device=dev)
-        # dense edge-MLP chain: "h16" (default) = two tiles in flight per SM, 3xFP16 operands (csrc/spherenet_h16.cu);
-        # "tc" = first-generation 3xTF32 chain with fp32 operand range (csrc/spherenet_tc.cu); "simt" = exact-fp32 FFMA
-        # twin (csrc/spherenet.cu).  All three are sm_90a kernels of libdig3d.so.
-        dense = os.environ.get("DIG3D_DENSE", "h16")
-        if dense not in ("h16", "tc", "simt"):
-            raise ValueError(f"DIG3D_DENSE={dense!r}: expected h16, tc or simt")
-        tc_cache = self.__dict__.setdefault("_tc_cache", {})
-        if dense == "h16":
-            packed = ops.tc_pack_matrix(self.init_e.lin.weight, tc_cache, "init_e.lin", kind="h16")
-            tables = (ops.init_e_tables(self.init_e, tc_cache)
-                      if os.environ.get("DIG3D_INIT_TABLES", "1") != "0" and self.hidden_channels == 128 else None)
-            e1, _ = ops.sphere_init_e_h16(z, g, rbf0, ops.pack_init_e(self.init_e), packed, self.hidden_channels,
-                                          v_in=v_in_all[0], tables=tables)
-        elif dense == "tc":
+        if dense == "tc":
+            tc_cache = self.__dict__.setdefault("_tc_cache", {})
             packed = ops.tc_pack_matrix(self.init_e.lin.weight, tc_cache, "init_e.lin")
             e1, _ = ops.sphere_init_e_tc(z, g, rbf0, ops.pack_init_e(self.init_e), packed, self.hidden_channels,
                                          v_in=v_in_all[0])
@@ -319,11 +310,7 @@ class _DimeNetFamily(nn.Module):
                                       v_in=v_in_all[0])
         for l in range(L):
             sbf_p, t_p = proj[l // 4]
-            if dense == "h16":
-                wt = ops.tc_pack_update_e(self.update_es[l], self._torsion, tc_cache, kind="h16")
-                e1, _, _, _ = ops.sphere_update_e_h16(e1, g, rbf0, sbf_p, t_p, 8 * (l % 4), wt,
-                                                      self.hidden_channels, self.int_emb_size, v_in=v_in_all[l + 1])
-            elif dense == "tc":
+            if dense == "tc":
                 wt = ops.tc_pack_update_e(self.update_es[l], self._torsion, tc_cache)
                 e1, _, _, _ = ops.sphere_update_e_tc(e1, g, rbf0, sbf_p, t_p, 8 * (l % 4), wt,
                                                      self.hidden_channels, self.int_emb_size, v_in=v_in_all[l + 1])
@@ -332,50 +319,47 @@ class _DimeNetFamily(nn.Module):
                                             ops.pack_update_e(self.update_es[l], self._torsion),
                                             self.hidden_channels, self.int_emb_size, v_in=v_in_all[l + 1])
         holders = [self.init_v] + list(self.update_vs)
-        if dense == "h16" and ops.update_v_h16_supported(self.init_v, self.out_channels):
-            ops.sphere_update_v_h16(v_in_all, holders, self.out_channels, v_all, tc_cache)
-        else:                                  # exact-fp32 FFMA engine (other widths, DIG3D_DENSE=tc / simt)
-            ops.sphere_update_v_batched(v_in_all, holders, self.out_channels, v_all)
+        ops.sphere_update_v_batched(v_in_all, holders, self.out_channels, v_all)      # exact-fp32 FFMA engine
         return ops.graph_readout(v_all, g.graph_ptr, g.n_graphs, g.n_nodes)
 
 
-    # ------------------------------------------------------------------ lean inference path (host overhead)
-    # The launch sequence above spends ~0.85 ms of Python per forward (weight-pointer structs rebuilt and validated for
-    # every layer, ~35 allocations, ~240 pointer validations) -- more than the GPU
-    # needs for the batch once three batches are in flight.  Everything that depends only on the PARAMETERS lives in a
-    # plan that is rebuilt when a parameter changes (same rules as the packed-weight caches: tensor._version / storage
-    # address / invalidate_packed()); per forward the host then allocates one workspace and makes the ~25 C calls with
-    # raw addresses.  Same kernels, same arguments, same order: the energies are bit-identical to the path above
-    # (DIG3D_LEAN=0 selects it; tests/test_gpu_parity.py::test_lean_inference_path_is_bit_identical).
+    # ------------------------------------------------------------------ 3xFP16 inference from a cached plan
+    # Building the launches op by op spends ~0.85 ms of Python per forward (weight-pointer structs rebuilt and validated
+    # for every layer, ~35 allocations, ~240 pointer validations) -- more than the GPU needs for the batch once three
+    # batches are in flight.  Everything that depends only on the PARAMETERS lives in a plan that is rebuilt when a
+    # parameter changes (same rules as the packed-weight caches: tensor._version / storage address / invalidate_packed());
+    # per forward the host then allocates one workspace and makes the ~25 C calls with raw addresses.
     def _inference_plan(self):
-        tables = os.environ.get("DIG3D_INIT_TABLES", "1")
+        tables = os.environ.get("DIG3D_INIT_TABLES", "1") != "0"
         key = ops.plan_key(self, tables)
         plan = self.__dict__.get("_plan")
         if plan is not None and plan["key"] == key:
             return plan
         key = ops.plan_key_refresh(self, tables)
         holders = [self.init_v] + list(self.update_vs)
-        if not ops.update_v_h16_supported(self.init_v, self.out_channels):
-            return None
         tc_cache = self.__dict__.setdefault("_tc_cache", {})
         L = self.num_layers
-        w_s, w_t = self._projection_rows(0, L)
-        parr, varr, n_lins = ops.pack_update_v_h16(holders, tc_cache)
+        if ops.update_v_h16_supported(self.init_v, self.out_channels):
+            parr, varr, n_lins = ops.pack_update_v_h16(holders, tc_cache)
+        else:            # out_channels > 4: update_v runs on the exact-fp32 FFMA engine (parr None)
+            parr, varr, n_lins = None, ops.pack_update_v_array(holders), None
         plan = {
             "key": key,
             "init_w": ops.pack_init_e(self.init_e),
-            "init_packed": ops.tc_pack_matrix(self.init_e.lin.weight, tc_cache, "init_e.lin", kind="h16"),
-            "init_tables": (ops.init_e_tables(self.init_e, tc_cache)
-                            if os.environ.get("DIG3D_INIT_TABLES", "1") != "0" and self.hidden_channels == 128 else None),
+            "init_packed": None if tables else ops.tc_pack_matrix(self.init_e.lin.weight, tc_cache, "init_e.lin",
+                                                                  kind="h16"),
+            "init_tables": ops.init_e_tables(self.init_e, tc_cache) if tables else None,
             "layers": [ops.tc_pack_update_e(self.update_es[l], self._torsion, tc_cache, kind="h16") for l in range(L)],
-            "w_s": w_s, "w_t": w_t, "parr": parr, "varr": varr, "n_lins": n_lins,
+            # basis projection rows, one [32, C] block per group of four layers
+            "proj": [self._projection_rows(first, min(4, L - first)) for first in range(0, L, 4)],
+            "parr": parr, "varr": varr, "n_lins": n_lins,
             "freq": self.emb.dist_emb.freq.detach(),
             "emb_rows": self.init_e.emb.num_embeddings if self.init_e.use_node_features else 0,
         }
         self.__dict__["_plan"] = plan
         return plan
 
-    def _forward_lean(self, plan, z, pos, g):
+    def _forward_plan(self, plan, z, pos, g):
         import ctypes
         call, byref = ops.call, ctypes.byref
         tors = self._torsion
@@ -383,9 +367,10 @@ class _DimeNetFamily(nn.Module):
         H, I, O = self.hidden_channels, self.int_emb_size, self.out_channels
         nb_s = self.num_spherical * self.num_radial
         dev = pos.device
-        # one workspace (floats), every buffer on a 256-byte boundary
+        # one workspace (floats), every buffer on a 256-byte boundary; layer l's projections sit at 8 * T * l
+        n_proj = 32 * T * len(plan["proj"])
         sizes = (("angle", T), ("torsion", T if tors else 0), ("rbf0", E * self.num_radial), ("bess", E * nb_s),
-                 ("sbf_p", 32 * T), ("t_p", 32 * T if tors else 0), ("e1a", E * H), ("e1b", E * H), ("x_ji", E * H),
+                 ("sbf_p", n_proj), ("t_p", n_proj if tors else 0), ("e1a", E * H), ("e1b", E * H), ("x_ji", E * H),
                  ("x_ji2", E * H), ("x_down", E * I), ("m", E * I), ("v_all", (L + 1) * N * O))
         off, total = {}, 0
         for name, n in sizes:
@@ -399,58 +384,63 @@ class _DimeNetFamily(nn.Module):
         st = ops._stream()
         src, dst, row_ptr, trip_ptr = g.src.data_ptr(), g.dst.data_ptr(), g.row_ptr.data_ptr(), g.trip_ptr.data_ptr()
         graph_ptr, batch = g.graph_ptr.data_ptr(), ops._p(g.batch, torch.int64, "batch")
-        pos_p = ops._p(pos.detach(), torch.float32, "pos")
-        if T:
-            call("dig3d_triplet_geometry", pos_p, src, dst, row_ptr, trip_ptr, E, int(tors), a["angle"],
-                 a["torsion"] if tors else None, None, None, None, None, st)
-        call("dig3d_edge_basis", g.dist.data_ptr(), E, float(self.cutoff), int(self.envelope_exponent),
-             ops._p(plan["freq"], torch.float32, "freq"), int(self._basis_id), int(not tors), a["rbf0"], a["bess"], st)
-        if T:
-            call("dig3d_triplet_basis_project_lists", a["bess"], a["angle"], a["torsion"] if tors else None, src, dst,
-                 row_ptr, trip_ptr, graph_ptr, batch, E, T, int(self._basis_id), 4, 8, plan["w_s"].data_ptr(),
-                 plan["w_t"].data_ptr() if tors else None, a["sbf_p"], a["t_p"] if tors else None, *ops._out_lists(g), st)
-        # Part A of block l + 1 rides on the unit chain of part B of block l (dig3d_sphere_update_e_ba_h16), and part A of
-        # block 0 on init_e's (dig3d_sphere_init_update_e_a_h16): two launches per interaction block (gather, dense chain)
-        # instead of three; DIG3D_FUSE_BA=0 keeps them apart (same results).
-        fuse = os.environ.get("DIG3D_FUSE_BA", "1") != "0"
-        zp = ops._p(z, torch.int64, "z")
-        if plan["init_tables"] is not None:
-            tab_i, tab_j, packed_rbf = plan["init_tables"]
-            init_args = (packed_rbf.data_ptr(), tab_i.data_ptr(), tab_j.data_ptr())
-        else:
-            init_args = (plan["init_packed"].data_ptr(), None, None)
-        if fuse and L:
-            call("dig3d_sphere_init_update_e_a_h16", zp, src, dst, a["rbf0"], E, byref(plan["init_w"]), *init_args,
-                 byref(plan["layers"][0]), a["e1a"], v_in, a["x_ji"], a["x_down"], st)
-        elif plan["init_tables"] is not None:
-            call("dig3d_sphere_init_e_h16_tab", zp, src, dst, a["rbf0"], E, byref(plan["init_w"]), *init_args,
-                 a["e1a"], v_in, st)
-        else:
-            call("dig3d_sphere_init_e_h16", zp, src, dst, a["rbf0"], E, byref(plan["init_w"]), init_args[0],
-                 a["e1a"], v_in, st)
-        e1, e1_next = a["e1a"], a["e1b"]
-        x_ji, x_ji_next = a["x_ji"], a["x_ji2"]
-        for l in range(L):
-            w = plan["layers"][l]
-            if not fuse:
-                call("dig3d_sphere_update_e_a_h16", e1, a["rbf0"], E, byref(w), x_ji, a["x_down"], st)
-            sp = ctypes.c_void_p(a["sbf_p"] + 4 * 8 * T * l)
-            tp = ctypes.c_void_p(a["t_p"] + 4 * 8 * T * l) if tors else None
-            ops.triplet_gather(a["x_down"], sp, tp, g, w.w_sbf2, w.w_t2, a["m"], st)
-            if fuse and l + 1 < L:        # x_down is free again: the gather that read it has completed (stream order)
-                call("dig3d_sphere_update_e_ba_h16", a["m"], e1, x_ji, a["rbf0"], dst, E, byref(w),
-                     byref(plan["layers"][l + 1]), e1_next, v_in + 4 * (l + 1) * N * H, x_ji_next, a["x_down"], st)
-                x_ji, x_ji_next = x_ji_next, x_ji
+        if E:                   # without edges every v_in stays zero: only update_v and the readout run
+            pos_p = ops._p(pos.detach(), torch.float32, "pos")
+            if T:
+                call("dig3d_triplet_geometry", pos_p, src, dst, row_ptr, trip_ptr, E, int(tors), a["angle"],
+                     a["torsion"] if tors else None, None, None, None, None, st)
+            call("dig3d_edge_basis", g.dist.data_ptr(), E, float(self.cutoff), int(self.envelope_exponent),
+                 ops._p(plan["freq"], torch.float32, "freq"), int(self._basis_id), int(not tors), a["rbf0"], a["bess"],
+                 st)
+            if T:
+                for k, (w_s, w_t) in enumerate(plan["proj"]):          # layers 4k .. 4k + 3
+                    call("dig3d_triplet_basis_project_lists", a["bess"], a["angle"], a["torsion"] if tors else None,
+                         src, dst, row_ptr, trip_ptr, graph_ptr, batch, E, T, int(self._basis_id), 4, 8, w_s.data_ptr(),
+                         w_t.data_ptr() if tors else None, a["sbf_p"] + 4 * 32 * T * k,
+                         a["t_p"] + 4 * 32 * T * k if tors else None, *ops._out_lists(g), st)
+            # Part A of block l + 1 rides on the unit chain of part B of block l (dig3d_sphere_update_e_ba_h16), and part
+            # A of block 0 on init_e's (dig3d_sphere_init_update_e_a_h16): two launches per interaction block (gather,
+            # dense chain) instead of three.
+            zp = ops._p(z, torch.int64, "z")
+            if plan["init_tables"] is not None:
+                tab_i, tab_j, packed_rbf = plan["init_tables"]
+                init_args = (packed_rbf.data_ptr(), tab_i.data_ptr(), tab_j.data_ptr())
             else:
-                call("dig3d_sphere_update_e_b_h16", a["m"], e1, x_ji, a["rbf0"], dst, E, byref(w), e1_next,
-                     v_in + 4 * (l + 1) * N * H, st)
-            e1, e1_next = e1_next, e1
-        call("dig3d_sphere_update_v_h16", v_in, N, L + 1, int(O), plan["n_lins"], plan["parr"], plan["varr"], a["v_all"], st)
+                init_args = (plan["init_packed"].data_ptr(), None, None)
+            if L:
+                call("dig3d_sphere_init_update_e_a_h16", zp, src, dst, a["rbf0"], E, byref(plan["init_w"]), *init_args,
+                     byref(plan["layers"][0]), a["e1a"], v_in, a["x_ji"], a["x_down"], st)
+            elif plan["init_tables"] is not None:
+                call("dig3d_sphere_init_e_h16_tab", zp, src, dst, a["rbf0"], E, byref(plan["init_w"]), *init_args,
+                     a["e1a"], v_in, st)
+            else:
+                call("dig3d_sphere_init_e_h16", zp, src, dst, a["rbf0"], E, byref(plan["init_w"]), init_args[0],
+                     a["e1a"], v_in, st)
+            e1, e1_next = a["e1a"], a["e1b"]
+            x_ji, x_ji_next = a["x_ji"], a["x_ji2"]
+            for l in range(L):
+                w = plan["layers"][l]
+                sp = ctypes.c_void_p(a["sbf_p"] + 4 * 8 * T * l)
+                tp = ctypes.c_void_p(a["t_p"] + 4 * 8 * T * l) if tors else None
+                ops.triplet_gather(a["x_down"], sp, tp, g, w.w_sbf2, w.w_t2, a["m"], st)
+                if l + 1 < L:        # x_down is free again: the gather that read it has completed (stream order)
+                    call("dig3d_sphere_update_e_ba_h16", a["m"], e1, x_ji, a["rbf0"], dst, E, byref(w),
+                         byref(plan["layers"][l + 1]), e1_next, v_in + 4 * (l + 1) * N * H, x_ji_next, a["x_down"], st)
+                    x_ji, x_ji_next = x_ji_next, x_ji
+                else:
+                    call("dig3d_sphere_update_e_b_h16", a["m"], e1, x_ji, a["rbf0"], dst, E, byref(w), e1_next,
+                         v_in + 4 * (l + 1) * N * H, st)
+                e1, e1_next = e1_next, e1
+        if plan["parr"] is not None:
+            call("dig3d_sphere_update_v_h16", v_in, N, L + 1, int(O), plan["n_lins"], plan["parr"], plan["varr"],
+                 a["v_all"], st)
+        else:
+            call("dig3d_sphere_update_v_batched", v_in, N, L + 1, int(O), plan["varr"], a["v_all"], st)
         u = torch.empty(g.n_graphs, O, dtype=torch.float32, device=dev)
         if g.n_graphs:
             call("dig3d_graph_readout", a["v_all"], graph_ptr, g.n_graphs, N, L + 1, O, u.data_ptr(), st)
         # ws / v_in_all are released here: the caching allocator hands them out again in stream order, after the kernels
-        # above, exactly like the per-tensor buffers of the general path
+        # above
         return u
 
     @staticmethod

@@ -376,9 +376,6 @@ int dig3d_h16_timeouts(void);
 /* debugging probe: enable / read the clock64() timeline CTA 0 of update_e part B records (host buffer, 128 x i64) */
 int dig3d_h16_trace(int32_t on, long long* out128);
 int dig3d_h16_set_fast_swish(int32_t on);
-/* No effect: it selected between the eight- and sixteen-warp epilogues of the two-tile update_e kernels, which the
- * register-accumulator engine replaced.  Kept so that existing callers still link; always returns DIG3D_OK. */
-int dig3d_h16_set_wide_epilogue(int32_t on);
 
 /* ------------------------------------------------------------------ SchNet
  * One interaction (update_e + update_v, schnet.py:29-35,53-59) for hidden_channels == num_filters in

@@ -205,14 +205,14 @@ def test_out_edge_lists_of_the_graph_build():
 
 
 @pytest.mark.parametrize("cls_name", ["SphereNet", "DimeNetPP"])
-def test_inference_paths_with_isolated_atoms_and_an_empty_graph_slot(cls_name, monkeypatch):
-    """The lean inference path (cached plan, fused chain, wide epilogue, out-edge lists) on a batch with an isolated atom, a
-    two-atom molecule without triplets and an empty graph slot: bit-identical to the general path and within 1e-5 of the
+def test_inference_paths_with_isolated_atoms_and_an_empty_graph_slot(cls_name):
+    """The inference forward (cached plan, fused chain, out-edge lists) on a batch with an isolated atom, a two-atom
+    molecule without triplets and an empty graph slot: bit-identical to the op-by-op chain and within 1e-5 of the
     oracle."""
     from dig_b200 import ops
     from dig_b200.data import synthetic_molecules, collate, Molecule
     from dig_b200.threedgraph import method
-    from helpers import formula_state_dict, rel_err
+    from helpers import formula_state_dict, rel_err, sphere_forward_op_by_op
     from oracle import restated
     dev = torch.device("cuda:0")
     m0, m1 = synthetic_molecules(2, "qm9", seed=11, variable=True)
@@ -226,10 +226,8 @@ def test_inference_paths_with_isolated_atoms_and_an_empty_graph_slot(cls_name, m
     model.load_state_dict(sd)
     model = model.to(dev).eval()
     with torch.no_grad():
-        monkeypatch.setenv("DIG3D_LEAN", "1")
         lean = model(b)
-        monkeypatch.setenv("DIG3D_LEAN", "0")
-        general = model(b)
+        general = sphere_forward_op_by_op(model, b)
         ref = restated.dimenet_family_forward({k: v.to(dev) for k, v in sd.items()}, b.z, b.pos, b.batch,
                                               torsion=cls_name == "SphereNet", num_graphs=5)
     assert not ops.h16_overflow()

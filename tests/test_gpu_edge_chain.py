@@ -132,23 +132,22 @@ def test_edge_to_node_sums_are_deterministic_across_unit_boundaries():
 
 
 @pytest.mark.parametrize("nmol", [1, 5, 24, 128])
-def test_fused_part_a_is_bit_identical_in_the_model(nmol, monkeypatch):
-    """The model forward with part A of block l + 1 fused into part B of block l (DIG3D_FUSE_BA=1) and with separate
-    launches (0) gives the same energies bit for bit."""
+def test_fused_part_a_is_bit_identical_in_the_model(nmol):
+    """The model forward, with part A of block l + 1 fused into part B of block l, gives the same energies bit for bit as
+    the chain with separate launches."""
     from dig_b200 import ops
     from dig_b200.data import synthetic_batch
     from dig_b200.threedgraph.method import SphereNet
+    from helpers import sphere_forward_op_by_op
     dev = torch.device("cuda:0")
     model = SphereNet()
     model.load_state_dict(formula_state_dict(model.state_dict(), seed=4))
     model = model.to(dev).eval()
     b = synthetic_batch(nmol, "qm9", seed=0).to(dev)
-    outs = {}
     with torch.no_grad():
-        for fuse in ("0", "1"):
-            monkeypatch.setenv("DIG3D_FUSE_BA", fuse)
-            outs[fuse] = model(b)
+        fused = model(b)
+        apart = sphere_forward_op_by_op(model, b)
     torch.cuda.synchronize()
-    assert torch.isfinite(outs["1"]).all()
-    assert torch.equal(outs["0"], outs["1"])
+    assert torch.isfinite(fused).all()
+    assert torch.equal(apart, fused)
     assert ops.tc_timeouts() == 0 and not ops.h16_overflow()

@@ -134,14 +134,19 @@ def test_forward_is_deterministic():
 
 
 @pytest.mark.parametrize("cls_name", ["SphereNet", "DimeNetPP"])
-def test_lean_inference_path_is_bit_identical(cls_name, monkeypatch):
+def test_lean_inference_path_is_bit_identical(cls_name):
     """The inference forward runs from a cached plan (parameter-only state: weight-pointer structs, packed weights,
-    projection rows) with raw workspace addresses; DIG3D_LEAN=0 selects the general op-by-op path.  Same kernels, same
-    arguments: bit-identical energies -- and the plan follows the parameters (in-place update, .data write +
-    invalidate_packed(), load_state_dict), and survives copy.deepcopy of the model."""
+    projection rows) with raw workspace addresses and fused launches (init_e + part A of block 0, part B of block l +
+    part A of block l + 1).  It is bit-identical to the same chain issued op by op with separate launches, and within
+    1e-5 of the oracle, on 19, 24, 11 and 1 molecules of variable size (ragged last unit, odd unit count, a single unit)
+    -- and the plan follows the parameters (in-place update, .data write + invalidate_packed(), load_state_dict), and
+    survives copy.deepcopy of the model."""
     import copy
+    from dig_b200 import ops
     from dig_b200.data import synthetic_batch
     from dig_b200.threedgraph import method
+    from helpers import sphere_forward_op_by_op
+    from oracle import restated
     dev = torch.device("cuda:0")
     model = getattr(method, cls_name)()
     model.load_state_dict(formula_state_dict(model.state_dict(), seed=3))
@@ -150,17 +155,12 @@ def test_lean_inference_path_is_bit_identical(cls_name, monkeypatch):
 
     def both():
         with torch.no_grad():
-            monkeypatch.setenv("DIG3D_LEAN", "1")
-            monkeypatch.setenv("DIG3D_FUSE_BA", "1")
-            lean = model(b)                       # part A of block l + 1 fused into the chain of part B of block l
-            lean2 = model(b)                      # second call: the cached plan
-            monkeypatch.setenv("DIG3D_FUSE_BA", "0")
-            apart = model(b)
-            monkeypatch.setenv("DIG3D_LEAN", "0")
-            general = model(b)
+            planned = model(b)
+            planned2 = model(b)                   # second call: the cached plan
+            apart = sphere_forward_op_by_op(model, b)
         assert "_plan" in model.__dict__
-        assert torch.equal(lean, general) and torch.equal(lean, lean2) and torch.equal(lean, apart)
-        return lean
+        assert torch.equal(planned, apart) and torch.equal(planned, planned2)
+        return planned
 
     u0 = both()
     with torch.no_grad():
@@ -176,15 +176,29 @@ def test_lean_inference_path_is_bit_identical(cls_name, monkeypatch):
     clone = copy.deepcopy(model)                              # plan / packed caches are not copied (device pointers)
     assert "_plan" not in clone.__dict__
     with torch.no_grad():
-        monkeypatch.setenv("DIG3D_LEAN", "1")
         assert torch.equal(clone(b), u0)
 
+    sd = formula_state_dict(model.state_dict(), seed=4)
+    model.load_state_dict(sd)
+    sd = {k: v.to(dev) for k, v in sd.items()}
+    for nmol in (24, 11, 1):
+        b = synthetic_batch(nmol, "qm9", seed=7, variable=True).to(dev)
+        with torch.no_grad():
+            ref = restated.dimenet_family_forward(sd, b.z, b.pos, b.batch, torsion=cls_name == "SphereNet")
+            planned = model(b)
+            apart = sphere_forward_op_by_op(model, b)
+        torch.cuda.synchronize()
+        assert ops.tc_timeouts() == 0 and not ops.h16_overflow()
+        assert torch.equal(planned, apart), nmol
+        assert rel_err(planned.cpu().numpy(), ref.cpu().numpy()) < TOL, nmol
 
-def test_comenet_lean_inference_path_is_bit_identical(monkeypatch):
-    """ComENet's engine forward from the cached plan (one workspace, raw addresses) vs the op-by-op `_forward_h16`
-    (DIG3D_LEAN=0): same launches, bit-identical energies; the plan follows parameter updates."""
+
+def test_comenet_lean_inference_path_is_bit_identical():
+    """ComENet's engine forward from the cached plan (one workspace, raw addresses) vs the same launches issued op by op
+    through the tensor wrappers: bit-identical energies; the plan follows parameter updates."""
     from dig_b200.data import synthetic_batch
     from dig_b200.threedgraph.method import ComENet
+    from helpers import comenet_forward_op_by_op
     dev = torch.device("cuda:0")
     model = ComENet(cutoff=6.0)
     model.load_state_dict(formula_state_dict(model.state_dict(), seed=5))
@@ -193,13 +207,11 @@ def test_comenet_lean_inference_path_is_bit_identical(monkeypatch):
 
     def both():
         with torch.no_grad():
-            monkeypatch.setenv("DIG3D_LEAN", "1")
-            lean, lean2 = model(b), model(b)
-            monkeypatch.setenv("DIG3D_LEAN", "0")
-            general = model(b)
-        assert "_plan" in model.__dict__ and torch.isfinite(lean).all()
-        assert torch.equal(lean, general) and torch.equal(lean, lean2)
-        return lean
+            planned, planned2 = model(b), model(b)
+            general = comenet_forward_op_by_op(model, b)
+        assert "_plan" in model.__dict__ and torch.isfinite(planned).all()
+        assert torch.equal(planned, general) and torch.equal(planned, planned2)
+        return planned
 
     u0 = both()
     with torch.no_grad():
@@ -210,44 +222,46 @@ def test_comenet_lean_inference_path_is_bit_identical(monkeypatch):
     assert torch.equal(both(), u0)
 
 
-@pytest.mark.parametrize("cls_name", ["SphereNet", "DimeNetPP"])
-def test_wide_epilogue_chain_matches_the_eight_warp_chain(cls_name, monkeypatch):
-    """update_e part B (+ the next block's part A) with all sixteen epilogue warps on the ready tile (DIG3D_H16_WIDE=1,
-    default) against the eight-warps-per-tile kernel: same jobs and operands, only the edge -> node sums are grouped
-    differently -- energies agree to fp32 summation noise and both sit within 1e-5 of the oracle.  Ragged last tile, odd
-    tile count, a single tile; fused and separate part A."""
+@pytest.mark.parametrize("cls_name,kw,case", [
+    ("SphereNet", dict(num_layers=5), "qm9"), ("SphereNet", dict(num_layers=6), "qm9"),
+    ("DimeNetPP", dict(num_layers=5), "qm9"), ("DimeNetPP", dict(num_layers=6), "qm9"),
+    ("SphereNet", dict(out_channels=5), "qm9"), ("DimeNetPP", dict(out_channels=5), "qm9"),
+    ("SphereNet", {}, "single_atoms"), ("DimeNetPP", {}, "single_atoms")],
+    ids=["SphereNet-5_layers", "SphereNet-6_layers", "DimeNetPP-5_layers", "DimeNetPP-6_layers",
+         "SphereNet-5_outputs", "DimeNetPP-5_outputs", "SphereNet-no_edges", "DimeNetPP-no_edges"])
+def test_plan_covers_deep_wide_and_edgeless_inputs(cls_name, kw, case):
+    """More than four interaction blocks (basis projections in groups of four layers), out_channels beyond the 3xFP16
+    update_v engine (update_v on the exact-fp32 FFMA engine) and a batch without edges (update_v and the readout only)
+    all run from the plan: bit-identical to the op-by-op chain, within 1e-5 of the oracle."""
     from dig_b200 import ops
-    from dig_b200.data import synthetic_batch
+    from dig_b200.data import Batch, synthetic_batch
     from dig_b200.threedgraph import method
+    from helpers import sphere_forward_op_by_op
     from oracle import restated
     dev = torch.device("cuda:0")
-    tors = cls_name == "SphereNet"
-    model = getattr(method, cls_name)()
-    sd = formula_state_dict(model.state_dict(), seed=4)
+    model = getattr(method, cls_name)(**kw)
+    sd = formula_state_dict(model.state_dict(), seed=8)
     model.load_state_dict(sd)
     model = model.to(dev).eval()
     sd = {k: v.to(dev) for k, v in sd.items()}
-    try:
-        for nmol in (24, 11, 1):
-            b = synthetic_batch(nmol, "qm9", seed=7, variable=True).to(dev)
-            with torch.no_grad():
-                ref = restated.dimenet_family_forward(sd, b.z, b.pos, b.batch, torsion=tors)
-                outs = {}
-                for wide in ("0", "1"):
-                    for fuse in ("0", "1"):
-                        monkeypatch.setenv("DIG3D_H16_WIDE", wide)
-                        monkeypatch.setenv("DIG3D_FUSE_BA", fuse)
-                        outs[(wide, fuse)] = model(b)
-            torch.cuda.synchronize()
-            assert ops.tc_timeouts() == 0 and not ops.h16_overflow()
-            assert torch.equal(outs[("1", "0")], outs[("1", "1")]), nmol           # fusion is exact in both layouts
-            assert torch.equal(outs[("0", "0")], outs[("0", "1")]), nmol
-            assert rel_err(outs[("1", "1")].cpu().numpy(), outs[("0", "1")].cpu().numpy()) < 2e-6, nmol
-            for k, u in outs.items():
-                assert rel_err(u.cpu().numpy(), ref.cpu().numpy()) < TOL, (nmol, k)
-    finally:
-        monkeypatch.setenv("DIG3D_H16_WIDE", "1")
-        ops.h16_wide_from_env()
+    if case == "single_atoms":
+        b = Batch(z=torch.tensor([1, 6, 8], device=dev),
+                  pos=torch.tensor([[0., 0, 0], [0.5, 0.2, 0], [1.0, 0, 0.3]], device=dev),
+                  batch=torch.tensor([0, 1, 2], device=dev))
+    else:
+        b = synthetic_batch(9, "qm9", seed=2, variable=True).to(dev)
+    with torch.no_grad():
+        planned = model(b)
+        apart = sphere_forward_op_by_op(model, b)
+        ref = restated.dimenet_family_forward(sd, b.z, b.pos, b.batch, torsion=cls_name == "SphereNet",
+                                              num_layers=model.num_layers)
+    torch.cuda.synchronize()
+    assert "_plan" in model.__dict__
+    assert (model.__dict__["_plan"]["parr"] is None) == (kw.get("out_channels", 1) > 4)
+    assert planned.shape == (int(b.batch.max()) + 1, model.out_channels) and torch.isfinite(planned).all()
+    assert ops.tc_timeouts() == 0 and not ops.h16_overflow()
+    assert torch.equal(planned, apart)
+    assert rel_err(planned.cpu().numpy(), ref.cpu().numpy()) < TOL
 
 
 def test_segment_sum_against_index_add():
@@ -402,8 +416,8 @@ def test_edge_basis_split_by_order_is_bit_identical(basis_id, nr, nb, env_on_bes
 
 
 def test_comenet_engine_forward_and_its_edge_kernels():
-    """ComENet inference on the tensor engine (linear_h16 for every hidden x hidden linear, folded edge filter,
-    ComENet._forward_h16) vs round 1's exact-fp32 fused block kernel (DIG3D_COMENET_DENSE=simt) and vs the oracle, at the
+    """ComENet inference on the tensor engine (linear_h16 for every hidden x hidden linear, folded edge filter, the
+    planned forward) vs round 1's exact-fp32 fused block kernel (DIG3D_COMENET_DENSE=simt) and vs the oracle, at the
     BASELINE configs[3] size; and the two aggregation kernels against their definitions in fp64."""
     import os
     from dig_b200 import ops
