@@ -171,6 +171,17 @@ SIGNATURES = {
     "dig3d_linear_set_config": [c_int32],
     "dig3d_transpose": [P, c_int32, c_int32, P, P],
     "dig3d_schnet_edge_features": [P, c_int64, P, c_int32, c_double, c_double, P, P, P],
+    "dig3d_gsphere_edge_flags": [P, P, c_int64, c_int64, P, P],
+    "dig3d_gsphere_keep_rows": [P, P, P, P, P, c_int64, c_int32, P],
+    "dig3d_gsphere_attention": [P, P, c_int32, c_int32, c_int32, c_int64, c_int32, c_int32, P, P],
+    "dig3d_gsphere_tanh": [P, c_int64, P, P],
+    "dig3d_gsphere_flow_reverse": [P, P, c_int64, c_int32, c_int32, P, P],
+    "dig3d_gsphere_focus_select": [P, P, c_int64, c_int32, c_int32, c_double, c_int32, P, P, P, P, P, P],
+    "dig3d_gsphere_compact": [P, c_int64, c_int32, c_int32, c_int32, P, P, P, P, P, P, P],
+    "dig3d_gsphere_neighbors": [P, c_int32, c_int64, c_int32, P, P, P, P],
+    "dig3d_gsphere_place": [c_int64, c_int32, c_int32, P, P, P, P, P, P, P, P, P, P, P],
+    "dig3d_gsphere_gather_local": [P, c_int64, c_int32, c_int32, P, P, P, c_int32, P, P],
+    "dig3d_gsphere_type_scale": [P, c_int32, P, P, c_int64, c_int32, c_int32, P, P, P],
 }
 _RESTYPES = {"dig3d_last_error": c_char_p, "dig3d_h16_packed_bytes": c_int64}
 

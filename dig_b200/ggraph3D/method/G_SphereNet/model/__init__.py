@@ -1,0 +1,1 @@
+from .sphgen import SphGen, TorchDraws  # noqa: F401

@@ -1,0 +1,229 @@
+"""G-SphereNet's SphereNet copy (reference dig/ggraph3D/method/G_SphereNet/model/spherenet.py:218-299): node features
+[N, hidden] on the sm_90a kernels, inference only.
+
+It differs from dig.threedgraph's SphereNet in four places, all handled here:
+  * init_e embeds `num_node_types` node types and also returns the embedding (node_type_emb);
+  * the torsion uses one reference atom per triplet (kNN geometry, dig3d_triplet_geometry_knn);
+  * update_e ends with a mean re-scatter over cat(idx_ji, idx_kj) (:170-172): an edge in no triplet keeps its previous
+    e1 / e2 -- dig3d_gsphere_edge_flags + dig3d_gsphere_keep_rows;
+  * update_v has num_output_layers - 1 hidden linears, a biased output layer of width hidden, and ends with a mean
+    re-scatter over the in-edges (:205): 0 for a node without one; forward ends with node_type_emb +
+    mean over the out-edges of (v - node_type_emb) (:297), i.e. node_type_emb for a node without out-edges.
+Only the last update_v feeds the output (the others are overwritten and the u updates are commented out in the
+reference), so only that one runs.  Every dense layer runs on the exact-fp32 linear kernel (dig3d_linear).
+"""
+import torch
+from torch import nn
+
+from .....threedgraph.method import _common
+from .....threedgraph.method._common import ResidualLayer, glorot_orthogonal, swish
+from .....threedgraph.method.dimenet_family import dist_emb
+from ..... import ops
+
+
+class emb(nn.Module):
+    """Only dist_emb owns parameters (features.py)."""
+
+    def __init__(self, num_spherical, num_radial, cutoff, envelope_exponent):
+        super().__init__()
+        self.dist_emb = dist_emb(num_radial, cutoff, envelope_exponent)
+
+    def reset_parameters(self):
+        self.dist_emb.reset_parameters()
+
+
+class init(nn.Module):
+    def __init__(self, num_node_types, num_radial, hidden_channels, act=swish):
+        super().__init__()
+        self.emb = nn.Embedding(num_node_types, hidden_channels)
+        self.lin_rbf_0 = nn.Linear(num_radial, hidden_channels)
+        self.lin = nn.Linear(3 * hidden_channels, hidden_channels)
+        self.lin_rbf_1 = nn.Linear(num_radial, hidden_channels, bias=False)
+        self.reset_parameters()
+
+    def reset_parameters(self):
+        self.emb.weight.data.uniform_(-3 ** 0.5, 3 ** 0.5)
+        self.lin_rbf_0.reset_parameters()
+        self.lin.reset_parameters()
+        glorot_orthogonal(self.lin_rbf_1.weight, scale=2.0)
+
+
+class update_e(nn.Module):
+    def __init__(self, hidden_channels, int_emb_size, basis_emb_size, num_spherical, num_radial, num_before_skip,
+                 num_after_skip, act=swish):
+        super().__init__()
+        self.lin_rbf1 = nn.Linear(num_radial, basis_emb_size, bias=False)
+        self.lin_rbf2 = nn.Linear(basis_emb_size, hidden_channels, bias=False)
+        self.lin_sbf1 = nn.Linear(num_spherical * num_radial, basis_emb_size, bias=False)
+        self.lin_sbf2 = nn.Linear(basis_emb_size, int_emb_size, bias=False)
+        self.lin_t1 = nn.Linear(num_spherical * num_spherical * num_radial, basis_emb_size, bias=False)
+        self.lin_t2 = nn.Linear(basis_emb_size, int_emb_size, bias=False)
+        self.lin_rbf = nn.Linear(num_radial, hidden_channels, bias=False)
+        self.lin_kj = nn.Linear(hidden_channels, hidden_channels)
+        self.lin_ji = nn.Linear(hidden_channels, hidden_channels)
+        self.lin_down = nn.Linear(hidden_channels, int_emb_size, bias=False)
+        self.lin_up = nn.Linear(int_emb_size, hidden_channels, bias=False)
+        self.layers_before_skip = nn.ModuleList([ResidualLayer(hidden_channels) for _ in range(num_before_skip)])
+        self.lin = nn.Linear(hidden_channels, hidden_channels)
+        self.layers_after_skip = nn.ModuleList([ResidualLayer(hidden_channels) for _ in range(num_after_skip)])
+        self.reset_parameters()
+
+    def reset_parameters(self):
+        for n in ("lin_rbf1", "lin_rbf2", "lin_sbf1", "lin_sbf2", "lin_t1", "lin_t2", "lin_down", "lin_up", "lin_rbf"):
+            glorot_orthogonal(getattr(self, n).weight, scale=2.0)
+        for n in ("lin_kj", "lin_ji", "lin"):
+            glorot_orthogonal(getattr(self, n).weight, scale=2.0)
+            getattr(self, n).bias.data.fill_(0)
+        for layer in list(self.layers_before_skip) + list(self.layers_after_skip):
+            layer.reset_parameters()
+
+
+class update_v(nn.Module):
+    def __init__(self, hidden_channels, out_emb_channels, num_output_layers, act=swish):
+        super().__init__()
+        self.lin_up = nn.Linear(hidden_channels, out_emb_channels, bias=True)
+        self.lins = nn.ModuleList([nn.Linear(out_emb_channels, out_emb_channels)
+                                   for _ in range(num_output_layers - 1)])
+        self.lin = nn.Linear(out_emb_channels, hidden_channels)
+        self.reset_parameters()
+
+    def reset_parameters(self):
+        glorot_orthogonal(self.lin_up.weight, scale=2.0)
+        for lin in self.lins:
+            glorot_orthogonal(lin.weight, scale=2.0)
+            lin.bias.data.fill_(0)
+        glorot_orthogonal(self.lin.weight, scale=2.0)
+        self.lin.bias.data.fill_(0)
+
+
+class update_u(nn.Module):
+    """Parameter-free (spherenet.py:209-215); its use is commented out in the reference's forward."""
+
+
+def _lin(m, x, act=False):
+    b = m.bias.detach() if m.bias is not None else None
+    if act:
+        return ops.linear(x, m.weight.detach(), b, want_act=True)[1]
+    return ops.linear(x, m.weight.detach(), b)
+
+
+class SphereNet(nn.Module):
+    def __init__(self, cutoff, num_node_types, num_layers, hidden_channels, int_emb_size, basis_emb_size,
+                 out_emb_channels, num_spherical, num_radial, envelope_exponent=5, num_before_skip=1,
+                 num_after_skip=2, num_output_layers=3, act=swish):
+        super().__init__()
+        if int_emb_size != 64 or basis_emb_size != 8:
+            raise NotImplementedError("G-SphereNet feature network: the triplet kernels are compiled for "
+                                      f"int_emb_size=64, basis_emb_size=8 (got {int_emb_size}, {basis_emb_size})")
+        if ("dimenet", num_spherical, num_radial) not in ops.BASIS_IDS:
+            raise NotImplementedError(f"no generated basis for num_spherical={num_spherical}, num_radial={num_radial}")
+        if act is not swish and getattr(act, "__name__", "") != "swish":
+            raise NotImplementedError("only the default swish activation is built")
+        self.cutoff = cutoff
+        self.num_spherical, self.num_radial, self.envelope_exponent = num_spherical, num_radial, envelope_exponent
+        self._basis_id = ops.BASIS_IDS[("dimenet", num_spherical, num_radial)]
+        self.init_e = init(num_node_types, num_radial, hidden_channels, act)
+        self.init_v = update_v(hidden_channels, out_emb_channels, num_output_layers, act)
+        self.init_u = update_u()
+        self.emb = emb(num_spherical, num_radial, self.cutoff, envelope_exponent)
+        self.update_vs = nn.ModuleList([update_v(hidden_channels, out_emb_channels, num_output_layers, act)
+                                        for _ in range(num_layers)])
+        self.update_es = nn.ModuleList([update_e(hidden_channels, int_emb_size, basis_emb_size, num_spherical,
+                                                 num_radial, num_before_skip, num_after_skip, act)
+                                        for _ in range(num_layers)])
+        self.update_us = nn.ModuleList([update_u() for _ in range(num_layers)])
+        self.reset_parameters()
+
+    def reset_parameters(self):
+        self.init_e.reset_parameters()
+        self.init_v.reset_parameters()
+        self.emb.reset_parameters()
+        for m in self.update_es:
+            m.reset_parameters()
+        for m in self.update_vs:
+            m.reset_parameters()
+
+    # ------------------------------------------------------------------ pieces
+    def _graph(self, z, pos, batch, num_graphs):
+        _common.require_cuda(pos, "G-SphereNet SphereNet")
+        return ops.build_graph(pos, batch, self.cutoff, num_graphs=num_graphs, z=z,
+                               z_rows=self.init_e.emb.num_embeddings)
+
+    def _rbf(self, g, want_bessel):
+        return ops.edge_basis(g.dist, self.cutoff, self.envelope_exponent, self.emb.dist_emb.freq, self._basis_id,
+                              envelope_on_bessel=False, num_radial=self.num_radial,
+                              n_bessel=self.num_spherical * self.num_radial, want_bessel=want_bessel)
+
+    def _init_e(self, z, g, rbf0):                                           # spherenet.py:76-82
+        ie = self.init_e
+        r0 = _lin(ie.lin_rbf_0, rbf0, act=True)
+        x = ops.gather_rows(ie.emb.weight.detach(), z)
+        e1 = _lin(ie.lin, torch.cat([ops.gather_rows(x, g.dst), ops.gather_rows(x, g.src), r0], dim=-1), act=True)
+        return e1, ops.ewise(_lin(ie.lin_rbf_1, rbf0), e1, 0)
+
+    def _update_v(self, uv, e2, g):                                          # spherenet.py:198-206
+        v = _lin(uv.lin_up, ops.segment_sum(e2, g.row_ptr))
+        for lin in uv.lins:
+            v = _lin(lin, v, act=True)
+        return ops.gsphere_keep_rows(_lin(uv.lin, v), ptr=g.row_ptr)
+
+    # ------------------------------------------------------------------ forward
+    def dist_only_forward(self, z, pos, batch, num_graphs=None):
+        """spherenet.py:254-271: distances only, init_e then the last update_v."""
+        with torch.no_grad():
+            g = self._graph(z, pos, batch, num_graphs)
+            rbf0, _ = self._rbf(g, want_bessel=False)
+            _, e2 = self._init_e(z, g, rbf0)
+            return self._update_v(self.update_vs[-1], e2, g)
+
+    def forward(self, z, pos, batch, num_graphs=None):
+        """spherenet.py:273-299."""
+        with torch.no_grad():
+            g = self._graph(z, pos, batch, num_graphs)
+            n, e = g.n_nodes, g.n_edges
+            dev = pos.device
+            nn_ = torch.empty(2, max(n, 1), dtype=torch.int32, device=dev)
+            ops.call("dig3d_knn2", ops._p(pos.detach(), torch.float32, "pos"), ops._p(g.batch, torch.int64, "batch"),
+                     ops._p(g.graph_ptr), n, g.n_graphs, ops._p(nn_[0]), ops._p(nn_[1]), ops._stream())
+            t = g.n_triplets
+            g.angle = torch.empty(t, dtype=torch.float32, device=dev)
+            g.torsion = torch.empty(t, dtype=torch.float32, device=dev)
+            g.idx_kj64 = torch.empty(t, dtype=torch.int64, device=dev)
+            g.idx_ji64 = torch.empty(t, dtype=torch.int64, device=dev)
+            if e and t:
+                ops.call("dig3d_triplet_geometry_knn", ops._p(pos.detach(), torch.float32, "pos"), ops._p(g.src),
+                         ops._p(g.dst), ops._p(g.row_ptr), ops._p(g.trip_ptr), e, ops._p(nn_[0]), ops._p(nn_[1]),
+                         ops._p(g.angle), ops._p(g.torsion), ops._p(g.idx_kj64), ops._p(g.idx_ji64), ops._stream())
+            rbf0, bess = self._rbf(g, want_bessel=True)
+            L = len(self.update_es)
+            sbf_ps, t_ps = [], []
+            for first in range(0, L, 4):                   # lin_sbf1 / lin_t1 of four layers per fused projection
+                es = self.update_es[first:first + 4]
+                rows = []
+                for name in ("lin_sbf1", "lin_t1"):
+                    w = torch.cat([getattr(m, name).weight.detach() for m in es], 0)
+                    rows.append(torch.cat([w, w.new_zeros(32 - w.size(0), w.size(1))], 0) if w.size(0) < 32 else w)
+                s_p, t_p = ops.triplet_basis_project(g, bess, self._basis_id, rows[0].contiguous(),
+                                                     rows[1].contiguous())
+                sbf_ps += [s_p[k] for k in range(len(es))]
+                t_ps += [t_p[k] for k in range(len(es))]
+            flag = ops.gsphere_edge_flags(g)
+            e1, e2 = self._init_e(z, g, rbf0)
+            for l, ue in enumerate(self.update_es):                          # spherenet.py:141-174
+                x_ji = _lin(ue.lin_ji, e1, act=True)
+                x_kj = _lin(ue.lin_kj, e1, act=True)
+                x_kj = ops.ewise(x_kj, _lin(ue.lin_rbf2, _lin(ue.lin_rbf1, rbf0)), 0)
+                x_kj = _lin(ue.lin_down, x_kj, act=True)
+                m = ops.sphere_triplet_gather(x_kj, sbf_ps[l], t_ps[l], g, ue.lin_sbf2.weight.detach(),
+                                              ue.lin_t2.weight.detach())
+                h = ops.ewise(x_ji, _lin(ue.lin_up, m, act=True), 1)
+                for layer in ue.layers_before_skip:
+                    h = ops.ewise(h, _lin(layer.lin2, _lin(layer.lin1, h, act=True), act=True), 1)
+                h = ops.ewise(_lin(ue.lin, h, act=True), e1, 1)
+                for layer in ue.layers_after_skip:
+                    h = ops.ewise(h, _lin(layer.lin2, _lin(layer.lin1, h, act=True), act=True), 1)
+                e2_new = ops.ewise(_lin(ue.lin_rbf, rbf0), h, 0)
+                e1 = ops.gsphere_keep_rows(h, flag=flag, fallback=e1)
+                e2 = ops.gsphere_keep_rows(e2_new, flag=flag, fallback=e2)
+            v = self._update_v(self.update_vs[-1], e2, g)
+            return ops.gsphere_keep_rows(v, ptr=g.out_ptr, fallback=self.init_e.emb.weight.detach(), fallback_idx=z)

@@ -1382,3 +1382,123 @@ def pronet_edge_features(g, pos_ca, pos_n, pos_c, level, cutoff, num_pos_emb, wa
 def linear_set_config(cfg):
     """Tile configuration of the 128 -> 128 training linear (0 / 1 / 2, see include/dig3d.h); experiments only."""
     call("dig3d_linear_set_config", int(cfg))
+
+
+# ----------------------------------------------------------------------------- G-SphereNet generation (csrc/gsphere.cu)
+I64 = torch.int64
+
+
+def gsphere_edge_flags(g):
+    """int32 [E]: 1 for the edges listed in cat(idx_ji, idx_kj) (G-SphereNet spherenet.py:170); needs g.idx_kj64."""
+    e, t = g.n_edges, g.n_triplets
+    flag = torch.zeros(max(e, 1), dtype=torch.int32, device=g.dist.device)[:e]
+    if e:
+        call("dig3d_gsphere_edge_flags", _p(g.trip_ptr, torch.int32, "trip_ptr"),
+             _p(g.idx_kj64, I64, "idx_kj") if t else None, e, t, _p(flag), _stream())
+    return flag
+
+
+def gsphere_keep_rows(x, flag=None, ptr=None, fallback=None, fallback_idx=None):
+    """In place: rows r of x [R, W] with flag[r] != 0 (or a non-empty CSR segment ptr[r]..ptr[r+1]) keep their value
+    (as fallback + (x - fallback)), the others become fallback[fallback_idx[r] or r] or 0.  Returns x."""
+    rows = x.size(0)
+    width = x.numel() // max(rows, 1)
+    if rows and width:
+        call("dig3d_gsphere_keep_rows", _p(flag, torch.int32, "flag"), _p(ptr, torch.int32, "ptr"), _p(x, F32, "x"),
+             _p(fallback, F32, "fallback"), _p(fallback_idx, I64, "fallback_idx"), rows, width, _stream())
+    return x
+
+
+def gsphere_attention(q, kv, n_keys, n_heads, k_off, v_off):
+    """Multi-head attention pooling with one query per molecule over that molecule's n_keys consecutive key rows."""
+    out = torch.empty(q.size(0), 32 * n_heads, dtype=F32, device=q.device)
+    if q.size(1) != 32 * n_heads:
+        raise ValueError(f"gsphere_attention: query width {q.size(1)} != 32 * {n_heads} heads")
+    if kv.size(0) != q.size(0) * n_keys:
+        raise ValueError("gsphere_attention: key rows != queries * n_keys")
+    if q.size(0):
+        call("dig3d_gsphere_attention", _p(q, F32, "q"), _p(kv, F32, "kv"), kv.size(1), int(k_off), int(v_off),
+             q.size(0), int(n_keys), int(n_heads), _p(out), _stream())
+    return out
+
+
+def gsphere_tanh(x):
+    y = torch.empty_like(x)
+    if x.numel():
+        call("dig3d_gsphere_tanh", _p(x, F32, "x"), x.numel(), _p(y), _stream())
+    return y
+
+
+def gsphere_flow_reverse(st, rescale, latent):
+    """latent [G, D] in place through the ST_Net_Exp layers, last first; st [G, L, 2D], rescale [L]."""
+    rows, dim = latent.shape
+    n_layers = rescale.numel()
+    if tuple(st.shape) != (rows, n_layers, 2 * dim):
+        raise ValueError(f"gsphere_flow_reverse: st {tuple(st.shape)} vs latent {tuple(latent.shape)}")
+    if rows:
+        call("dig3d_gsphere_flow_reverse", _p(st, F32, "st"), _p(rescale, F32, "rescale"), rows, dim, n_layers,
+             _p(latent, F32, "latent"), _stream())
+    return latent
+
+
+def gsphere_focus_select(logit, z, n_mols, n_atoms, focus_th, emit):
+    """-> (score [G, n], can_focus [G, n] (first `continuing` rows valid), cont_src [G], emit_src [G], counts [2])."""
+    dev = logit.device
+    score = torch.empty(n_mols, n_atoms, dtype=F32, device=dev)
+    can = torch.empty(n_mols, n_atoms, dtype=F32, device=dev)
+    idx = torch.empty(2 * n_mols + 2, dtype=torch.int32, device=dev)
+    cont_src, emit_src, counts = idx[:n_mols], idx[n_mols:2 * n_mols], idx[2 * n_mols:]
+    call("dig3d_gsphere_focus_select", _p(logit, F32, "logit"), _p(z, I64, "z"), n_mols, n_atoms, z.size(1),
+         float(focus_th), int(bool(emit)), _p(score), _p(can), _p(cont_src), _p(emit_src), _p(counts), _stream())
+    return score, can, cont_src, emit_src, counts
+
+
+def gsphere_compact(src, n_atoms, ld_out, z, pos, focus):
+    """Rows src of the molecule state (z [G, ld], pos [G, ld, 3], focus [G, ld]) into new [R, ld_out] buffers."""
+    rows, dev = src.numel(), z.device
+    z2 = torch.empty(rows, ld_out, dtype=I64, device=dev)
+    pos2 = torch.empty(rows, ld_out, 3, dtype=F32, device=dev)
+    f2 = torch.empty(rows, ld_out, dtype=I64, device=dev)
+    if rows:
+        call("dig3d_gsphere_compact", _p(src, torch.int32, "src"), rows, n_atoms, z.size(1), ld_out, _p(z, I64, "z"),
+             _p(pos, F32, "pos"), _p(focus, I64, "focus"), _p(z2), _p(pos2), _p(f2), _stream())
+    return z2, pos2, f2
+
+
+def gsphere_neighbors(pos, n_atoms, focus_id, want_c2):
+    g = focus_id.numel()
+    c = torch.empty(2, g, dtype=I64, device=pos.device)
+    if g:
+        call("dig3d_gsphere_neighbors", _p(pos, F32, "pos"), pos.size(1), g, n_atoms, _p(focus_id, I64, "focus_id"),
+             _p(c[0]), _p(c[1]) if want_c2 else None, _stream())
+    return c[0], (c[1] if want_c2 else None)
+
+
+def gsphere_place(n_atoms, focus_id, c1, c2, dist, angle, torsion, type_id, z, pos, focus):
+    g = focus_id.numel()
+    if g:
+        call("dig3d_gsphere_place", g, n_atoms, z.size(1), _p(focus_id, I64, "focus_id"), _p(c1, I64, "c1"),
+             _p(c2, I64, "c2"), _p(dist, F32, "dist"), _p(angle, F32, "angle"), _p(torsion, F32, "torsion"),
+             _p(type_id, I64, "type_id"), _p(z, I64, "z"), _p(pos, F32, "pos"), _p(focus, I64, "focus"), _stream())
+
+
+def gsphere_gather_local(feat, n_mols, n_atoms, ids):
+    """cat_j feat[g * n_atoms + ids[j][g]] -> [G, len(ids) * W]."""
+    width = feat.size(1)
+    out = torch.empty(n_mols, len(ids) * width, dtype=F32, device=feat.device)
+    idp = [_p(t, I64, "ids") for t in ids] + [None] * (3 - len(ids))
+    if n_mols:
+        call("dig3d_gsphere_gather_local", _p(feat, F32, "feat"), n_mols, n_atoms, width, *idp, len(ids), _p(out),
+             _stream())
+    return out
+
+
+def gsphere_type_scale(latent, emb, feat, n_mols, n_atoms):
+    """(type [G] = argmax latent, feat [G*n, W] * emb[type] per molecule)."""
+    width = feat.size(1)
+    type_id = torch.empty(n_mols, dtype=I64, device=feat.device)
+    out = torch.empty_like(feat)
+    if n_mols:
+        call("dig3d_gsphere_type_scale", _p(latent, F32, "latent"), latent.size(1), _p(emb, F32, "emb"),
+             _p(feat, F32, "feat"), n_mols, n_atoms, width, _p(type_id), _p(out), _stream())
+    return type_id, out

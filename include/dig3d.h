@@ -637,6 +637,52 @@ int dig3d_transpose(const float* in, int32_t rows, int32_t cols, float* out, voi
 int dig3d_schnet_edge_features(const float* dist, int64_t n_edges, const float* offset, int32_t n_gauss, double coeff,
                                double cutoff, float* gauss, float* cut, void* stream);
 
+/* ------------------------------------------------------------------ G-SphereNet generation (csrc/gsphere.cu)
+ * reference dig/ggraph3D/method/G_SphereNet/model/{sphgen.py:82-204, spherenet.py, att.py, net_utils.py}.
+ * Generation state is padded per molecule: z[G, ld] int64, pos[G, ld, 3], focus[G, ld] int64; at a step every active
+ * molecule has n_atoms atoms, rows g*n_atoms .. of the flattened node arrays.
+ *
+ * SphereNet copy (spherenet.py:170-172,205,297): edge_flags marks the edges listed in cat(idx_ji, idx_kj) (flag zeroed
+ * by the caller); keep_rows keeps x[r] where flag[r] != 0 (or, flag NULL, where the CSR segment ptr[r]..ptr[r+1] is not
+ * empty) and writes fallback[fallback_idx ? fallback_idx[r] : r] (or 0 without fallback) elsewhere, in place. */
+int dig3d_gsphere_edge_flags(const int32_t* trip_ptr, const int64_t* idx_kj, int64_t n_edges, int64_t n_triplets,
+                             int32_t* flag, void* stream);
+int dig3d_gsphere_keep_rows(const int32_t* flag, const int32_t* ptr, float* x, const float* fallback,
+                            const int64_t* fallback_idx, int64_t rows, int32_t width, void* stream);
+/* MH_ATT with one query per molecule (att.py:18-35): q[n_queries, 32*n_heads] projected queries; keys / values of query g
+ * are rows g*n_keys .. of kv[*, ld_kv] at columns k_off / v_off; out = softmax-weighted value sum (d_k = 32). */
+int dig3d_gsphere_attention(const float* q, const float* kv, int32_t ld_kv, int32_t k_off, int32_t v_off,
+                            int64_t n_queries, int32_t n_keys, int32_t n_heads, float* out, void* stream);
+/* Flow reverse (net_utils.py:28-37,75-80): y = tanh(x); flow_reverse applies the n_layers ST_Net_Exp affine maps, last
+ * layer first, to latent[rows, dim] in place, st[g, l, :] = linear2 output (2*dim wide) of layer l, rescale[l] = its
+ * Rescale weight. */
+int dig3d_gsphere_tanh(const float* x, int64_t n, float* y, void* stream);
+int dig3d_gsphere_flow_reverse(const float* st, const float* rescale, int64_t rows, int32_t dim, int32_t n_layers,
+                               float* latent, void* stream);
+/* Focus decision and compaction (sphgen.py:116-142), one CTA: score = sigmoid(logit[G, n_atoms]); can_focus rows of the
+ * continuing molecules in order, cont_src / emit_src = their source rows, counts = (continuing, emitted). */
+int dig3d_gsphere_focus_select(const float* logit, const int64_t* z, int64_t n_mols, int32_t n_atoms, int32_t ld,
+                               double focus_th, int32_t emit, float* score, float* can_focus, int32_t* cont_src,
+                               int32_t* emit_src, int32_t* counts, void* stream);
+/* out row k = in row src[k] (first n_atoms columns of z / pos, n_atoms - 1 of focus). */
+int dig3d_gsphere_compact(const int32_t* src, int64_t rows, int32_t n_atoms, int32_t ld_in, int32_t ld_out,
+                          const int64_t* z, const float* pos, const int64_t* focus, int64_t* z_out, float* pos_out,
+                          int64_t* focus_out, void* stream);
+/* c1 = nearest atom to the focus, c2 (nullable) = nearest atom to c1 among the rest (sphgen.py:165-169,185-189). */
+int dig3d_gsphere_neighbors(const float* pos, int32_t ld, int64_t n_mols, int32_t n_atoms, const int64_t* focus_id,
+                            int64_t* c1, int64_t* c2, void* stream);
+/* The new atom: type, position (sphgen.py:162-197, dattoxyz geometric_computing.py:107-122) and focus, written at
+ * column n_atoms of z / pos and n_atoms - 1 of focus. */
+int dig3d_gsphere_place(int64_t n_mols, int32_t n_atoms, int32_t ld, const int64_t* focus_id, const int64_t* c1,
+                        const int64_t* c2, const float* dist, const float* angle, const float* torsion,
+                        const int64_t* type_id, int64_t* z, float* pos, int64_t* focus, void* stream);
+/* out[g] = cat_j feat[g*n_atoms + id_j[g]] for j < n_ids (<= 3): the local query features. */
+int dig3d_gsphere_gather_local(const float* feat, int64_t n_mols, int32_t n_atoms, int32_t width, const int64_t* id0,
+                               const int64_t* id1, const int64_t* id2, int32_t n_ids, float* out, void* stream);
+/* type[g] = argmax latent[g, :dim]; out = feat * emb[type[g]] over the molecule's atoms (sphgen.py:151-153). */
+int dig3d_gsphere_type_scale(const float* latent, int32_t dim, const float* emb, const float* feat, int64_t n_mols,
+                             int32_t n_atoms, int32_t width, int64_t* type_out, float* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
