@@ -69,36 +69,48 @@ def sphere_forward_op_by_op(model, data):
     return u
 
 
-def comenet_forward_op_by_op(model, data):
+def comenet_forward_op_by_op(model, data, record=None):
     """ComENet 3xFP16 inference issued op by op through the tensor wrappers: every hidden x hidden linear as
     `ops.linear_h16` (swish and residuals fused as in the planned forward), the EdgeGraphConv aggregations as
-    `ops.comenet_filter_sum`.  The planned model forward must equal it bit for bit."""
+    `ops.comenet_filter_sum`.  The planned model forward must equal it bit for bit.  `record` (a dict): filled with the
+    graph, the features and every intermediate, keyed "emb", "<block>.x1", "<block>.filt<c>", "<block>.agg<c>",
+    "<block>.root<c>", "<block>.conv<c>", "<block>.h<c>", "<block>.t", "<block>.cat", "<block>.lins<l>", "<block>.norm",
+    "<block>.shift", "<block>.std", "<block>.final", "head<l>", "out", "energy"."""
     from dig_b200 import ops
+    rec = record if record is not None else {}
     m = model
     z, pos = data.z.long(), data.pos
     g = ops.build_graph(pos, data.batch, m.cutoff, num_graphs=getattr(data, "num_graphs", None), want_edge_index=False,
                         z=z, z_rows=m.emb.emb.num_embeddings)
     f1, f2, _ = ops.comenet_geometry(g, pos, m.cutoff)
+    rec.update(graph=g, z=z, f1=f1, f2=f2)
     lin = ops.linear_h16
-    x = ops.comenet_embed(z, m.emb.emb.weight)                                  # swish(emb[z])
-    for blk in m.interaction_blocks:
-        x = lin(x, blk.lin.weight, blk.lin.bias, want_act=True, act_only=True)
+    x = rec["emb"] = ops.comenet_embed(z, m.emb.emb.weight)                    # swish(emb[z])
+    for b, blk in enumerate(m.interaction_blocks):
+        x = rec[f"{b}.x1"] = lin(x, blk.lin.weight, blk.lin.bias, want_act=True, act_only=True)
         hs = []
-        for conv, lf, l, feat in ((blk.conv1, blk.lin_feature1, blk.lin1, f1),
-                                  (blk.conv2, blk.lin_feature2, blk.lin2, f2)):
-            agg = ops.comenet_filter_sum(feat, m._filter_t(lf), x, g)
+        for c, (conv, lf, l, feat) in enumerate(((blk.conv1, blk.lin_feature1, blk.lin1, f1),
+                                                 (blk.conv2, blk.lin_feature2, blk.lin2, f2)), 1):
+            filt = rec[f"{b}.filt{c}"] = m._filter_t(lf)
+            agg = rec[f"{b}.agg{c}"] = ops.comenet_filter_sum(feat, filt, x, g)
             # GraphConv: lin_rel(agg) + lin_root(x) -- the second GEMM adds the first in its epilogue
-            h = lin(agg, conv.lin_rel.weight, conv.lin_rel.bias, residual=lin(x, conv.lin_root.weight, None))
+            root = rec[f"{b}.root{c}"] = lin(x, conv.lin_root.weight, None)
+            h = rec[f"{b}.conv{c}"] = lin(agg, conv.lin_rel.weight, conv.lin_rel.bias, residual=root)
             hs.append(lin(h, l.weight, l.bias, want_act=True, act_only=True))
+            rec[f"{b}.h{c}"] = hs[-1]
         wa, wb = m._cat_halves(blk)
         # lin_cat(cat[h1, h2]) + x = h1 Wa^T + b + (h2 Wb^T + x)
-        h = lin(hs[0], wa, blk.lin_cat.bias, residual=lin(hs[1], wb, None, residual=x))
-        for l in blk.lins:
-            h = lin(h, l.weight, l.bias, want_act=True, act_only=True, residual=h)          # swish(l(h)) + h
-        h, _, _ = ops.graphnorm(h, g.graph_ptr, blk.norm.weight.detach(), blk.norm.bias.detach(),
-                                blk.norm.mean_scale.detach(), blk.norm.eps)
-        x = lin(h, blk.final.weight, blk.final.bias)
-    for l in m.lins:
-        x = lin(x, l.weight, l.bias, want_act=True, act_only=True)
-    x = ops.linear(x, m.lin_out.weight.detach(), m.lin_out.bias.detach())
-    return ops.segment_sum(x, g.graph_ptr)
+        t = rec[f"{b}.t"] = lin(hs[1], wb, None, residual=x)
+        h = rec[f"{b}.cat"] = lin(hs[0], wa, blk.lin_cat.bias, residual=t)
+        for i, l in enumerate(blk.lins):
+            h = rec[f"{b}.lins{i}"] = lin(h, l.weight, l.bias, want_act=True, act_only=True, residual=h)   # swish(l(h)) + h
+        h, rec[f"{b}.shift"], rec[f"{b}.std"] = ops.graphnorm(h, g.graph_ptr, blk.norm.weight.detach(),
+                                                               blk.norm.bias.detach(), blk.norm.mean_scale.detach(),
+                                                               blk.norm.eps)
+        rec[f"{b}.norm"] = h
+        x = rec[f"{b}.final"] = lin(h, blk.final.weight, blk.final.bias)
+    for i, l in enumerate(m.lins):
+        x = rec[f"head{i}"] = lin(x, l.weight, l.bias, want_act=True, act_only=True)
+    x = rec["out"] = ops.linear(x, m.lin_out.weight.detach(), m.lin_out.bias.detach())
+    rec["energy"] = ops.segment_sum(x, g.graph_ptr)
+    return rec["energy"]

@@ -4,11 +4,15 @@ The 3xFP16 product is emulated exactly as the kernels split their operands (fp16
 the residual, the same for w * 64), with the three products summed in fp64.  The bound must accept it in every
 activation / weight regime the GPU tests use, and must reject (a) the same product with the A_lo * W_hi correction
 of one k16 step dropped and (b) an error confined to a row 100x below the batch maximum, which the old max-normalised
-metric (`helpers.rel_err < 1e-5`) lets through.  So the GPU test is sharp enough to see a missing correction."""
+metric (`helpers.rel_err < 1e-5`) lets through.  So the GPU test is sharp enough to see a missing correction.
+The same holds for the ComENet ops of tests/test_gpu_comenet_fp64.py: the split product at K = 256 / 384 (chunk sums
+carried across operand panels; rejects a dropped chunk), the folded edge-filter sum (rejects a dropped q term) and
+GraphNorm (cnt = 1, an empty slot, constant / large-offset channels, mean_scale 0 / 0.5 / 1; rejects a one-pass
+variance, a dropped eps and an ignored mean_scale), each emulated in fp32 in its kernel's operation order."""
 import pytest
 import torch
 
-from fp64_bound import Bounded, linear, split16
+from fp64_bound import Bounded, filter_sum, fold, graphnorm, linear, split16
 from helpers import rel_err
 
 ROWS, K, N = 512, 128, 128
@@ -77,3 +81,170 @@ def test_bound_rejects_a_row_local_error_that_rel_err_accepts():
     assert rel_err(y.numpy(), ref.v.numpy()) < 1e-5
     with pytest.raises(AssertionError, match="outside the bound"):
         ref.check(y)
+
+
+# ------------------------------------------------------------------------------------------------ K = 256 / 384 panels
+def _emulate_chunks(x, w, b, drop_chunk=None):
+    """The kernel's order at any K: each K = 64 chunk's three split products rounded to fp32 on their own (the
+    accumulator of a chunk starts from zero), the chunk sums added in fp32 in chunk order across the operand panels
+    (128 columns each), then the 1 / (H_SA H_SW) scale and the bias in one fma (emulated in fp64, rounded once)."""
+    xh, xl = (t.double() for t in split16(x, 8.0))
+    wh, wl = (t.double() for t in split16(w, 64.0))
+    acc = None
+    for c in range(x.size(1) // 64):
+        if c == drop_chunk:
+            continue
+        s = slice(64 * c, 64 * c + 64)
+        d = (xl[:, s] @ wh[:, s].T + xh[:, s] @ wl[:, s].T + xh[:, s] @ wh[:, s].T).float()
+        acc = d if acc is None else acc + d
+    return (acc.double() / 512.0 + b.double()).float()
+
+
+def _operands_k(k, n, act, seed):
+    g = torch.Generator().manual_seed(seed)
+    x = (torch.randn(ROWS, k, generator=g, dtype=torch.float64) * act / 3).clamp(-act, act).float()
+    x = x * 10.0 ** (torch.rand(ROWS, 1, generator=g, dtype=torch.float64) * 4 - 4).float()     # rows over 4 decades
+    a = (6.0 / (k + n)) ** 0.5
+    w = ((torch.rand(n, k, generator=g, dtype=torch.float64) * 2 - 1) * a).float()
+    b = (0.1 * (torch.rand(n, generator=g, dtype=torch.float64) * 2 - 1)).float()
+    return x, w, b
+
+
+@pytest.mark.parametrize("act", [1e-4, 1.0, 8100.0])
+@pytest.mark.parametrize("k", [256, 384])
+def test_bound_holds_across_operand_panels(k, act):
+    """tol_h16(K) for two / three panels: the chunk sums carried across panels are K/64 - 1 fp32 additions."""
+    x, w, b = _operands_k(k, 192, act, seed=k)
+    ratio = linear(Bounded.exact(x), w, b, "h16").check(_emulate_chunks(x, w, b), f"K={k} act={act}")
+    assert ratio < 0.5, ratio
+
+
+@pytest.mark.parametrize("k", [256, 384])
+def test_bound_rejects_a_dropped_chunk_of_the_second_panel(k):
+    x, w, b = _operands_k(k, 192, 1.0, seed=k + 1)
+    ref = linear(Bounded.exact(x), w, b, "h16")
+    ref.check(_emulate_chunks(x, w, b))
+    with pytest.raises(AssertionError, match="outside the bound"):
+        ref.check(_emulate_chunks(x, w, b, drop_chunk=2), f"K={k} chunk 2 (columns 128-191) dropped")
+
+
+# ------------------------------------------------------------------------------------------------ filter_sum
+def _filter_case(seed=3, n=40, q=12, width=32):
+    g = torch.Generator().manual_seed(seed)
+    deg = torch.randint(1, 9, (n,), generator=g)
+    row_ptr = torch.zeros(n + 1, dtype=torch.long)
+    row_ptr[1:] = torch.cumsum(deg, 0)
+    e = int(row_ptr[-1])
+    src = torch.randint(0, n, (e,), generator=g)
+    feat = torch.rand(e, q, generator=g).float()
+    weff_t = (torch.randn(q, width, generator=g) * 0.3).float()
+    x = (torch.randn(n, width, generator=g) * 10.0 ** (torch.rand(n, 1, generator=g) * 4 - 3)).float()
+    return feat, weff_t, x, src, row_ptr, n
+
+
+def _filter_emulate(feat, weff_t, x, src, row_ptr, n, drop_q=None):
+    """dig3d_comenet_filter_sum's order: w by Q fmas from zero, then one fma per in-edge (fma = exact fp64 product and
+    sum, rounded to fp32)."""
+    fma = lambda a, b, c: (a.double() * b.double() + c.double()).float()
+    out = torch.zeros(n, x.size(1))
+    for i in range(n):
+        acc = torch.zeros(x.size(1))
+        for e in range(int(row_ptr[i]), int(row_ptr[i + 1])):
+            w = torch.zeros(x.size(1))
+            for q in range(feat.size(1)):
+                if q != drop_q:
+                    w = fma(weff_t[q], feat[e, q].expand(x.size(1)), w)
+            acc = fma(w, x[src[e]], acc)
+        out[i] = acc
+    return out
+
+
+def test_filter_sum_bound_accepts_the_kernel_order_and_rejects_a_dropped_q_term():
+    feat, weff_t, x, src, row_ptr, n = _filter_case()
+    ref = filter_sum(feat, Bounded.exact(weff_t), Bounded.exact(x), src, row_ptr, n)
+    assert ref.check(_filter_emulate(feat, weff_t, x, src, row_ptr, n), "filter_sum") < 0.5
+    with pytest.raises(AssertionError, match="outside the bound"):
+        ref.check(_filter_emulate(feat, weff_t, x, src, row_ptr, n, drop_q=5), "filter_sum without q = 5")
+
+
+def test_fold_bound_is_relative_to_the_factor_magnitudes():
+    """W1^T W2^T in exact fp32 with a cancelling middle sum: the bound is built on |W1|^T |W2|^T."""
+    g = torch.Generator().manual_seed(4)
+    w1, w2 = torch.randn(64, 12, generator=g).float(), torch.randn(32, 64, generator=g).float()
+    w2[:, 32:] = -w2[:, :32] * (w1[:32, :].abs().mean() / w1[32:, :].abs().mean())   # partial cancellation
+    ref = fold(w1, w2)
+    y = (w1.T.double() @ w2.T.double())                           # fp64, then one fp32 rounding per K-term sum
+    assert ref.check(y.float(), "fold") < 0.5
+    assert torch.allclose(ref.m, w1.T.double().abs() @ w2.T.double().abs())
+
+
+# ------------------------------------------------------------------------------------------------ graphnorm
+GN_SIZES = [1, 0, 16, 2, 3, 40]                 # cnt = 1, an empty graph slot, small and large graphs
+GN_W = 8
+
+
+def _gn_case(ms_value, seed=5):
+    """Channel 0 constant, 1 a large offset (mean 1e3, spread 1e-2), 2 a small spread (1e-2 around 0), the rest randn
+    over four decades."""
+    g = torch.Generator().manual_seed(seed)
+    ptr = torch.zeros(len(GN_SIZES) + 1, dtype=torch.int32)
+    ptr[1:] = torch.cumsum(torch.tensor(GN_SIZES), 0)
+    n = int(ptr[-1])
+    h = torch.randn(n, GN_W, generator=g) * 10.0 ** (torch.rand(1, GN_W, generator=g) * 4 - 2)
+    h[:, 0] = 0.37
+    h[:, 1] = 1e3 + 1e-2 * torch.randn(n, generator=g)
+    h[:, 2] = 1e-2 * torch.randn(n, generator=g)
+    w = (1.0 + 0.1 * (torch.rand(GN_W, generator=g) * 2 - 1)).float()
+    b = (0.1 * (torch.rand(GN_W, generator=g) * 2 - 1)).float()
+    ms = torch.full((GN_W,), ms_value).float()
+    return h.float(), ptr, w, b, ms
+
+
+def _gn_emulate(h, ptr, w, b, ms, eps=1e-5, fault=None):
+    """graphnorm_fwd_kernel in fp32, node by node (vectorised over channels).  fault: 'one_pass' (E[h^2] - E[h]^2),
+    'no_eps', 'no_mean_scale'."""
+    eps = torch.tensor(eps, dtype=torch.float32)
+    y = torch.empty_like(h)
+    for gi in range(ptr.numel() - 1):
+        n0, n1 = int(ptr[gi]), int(ptr[gi + 1])
+        cnt = torch.tensor(float(max(n1 - n0, 1)))
+        s = torch.zeros(h.size(1))
+        for n in range(n0, n1):
+            s = s + h[n]
+        sh = s / cnt if fault == "no_mean_scale" else (s / cnt) * ms
+        sq = torch.zeros(h.size(1))
+        if fault == "one_pass":
+            for n in range(n0, n1):
+                sq = sq + h[n] * h[n]
+            var = sq / cnt - sh * sh
+        else:
+            for n in range(n0, n1):
+                o = h[n] - sh
+                sq = sq + o * o
+            var = sq / cnt
+        sd = torch.sqrt(var if fault == "no_eps" else var + eps)
+        for n in range(n0, n1):
+            y[n] = (w * (h[n] - sh)) / sd + b
+    return y
+
+
+@pytest.mark.parametrize("ms_value", [0.0, 0.5, 1.0])
+def test_graphnorm_bound_accepts_the_kernel_order(ms_value):
+    h, ptr, w, b, ms = _gn_case(ms_value)
+    y_ref, sh_ref, sd_ref = graphnorm(Bounded.exact(h), ptr, w, b, ms, 1e-5)
+    assert y_ref.check(_gn_emulate(h, ptr, w, b, ms), f"graphnorm ms={ms_value}") < 0.5
+    assert float(sd_ref.v[1].min()) == pytest.approx(1e-5 ** 0.5, rel=1e-6)     # the empty slot: sd = sqrt(eps)
+    assert float(sh_ref.v[1].abs().max()) == 0.0
+
+
+@pytest.mark.parametrize("fault", ["one_pass", "no_eps", "no_mean_scale"])
+def test_graphnorm_bound_rejects_a_wrong_kernel(fault):
+    """one_pass cancels on the large-offset channel (var 1e-4 under a mean of 1e3); no_eps moves sd by 5 % on the
+    1e-2-spread channel and divides by zero on the constant one; no_mean_scale shifts by the mean at mean_scale 0.5."""
+    h, ptr, w, b, ms = _gn_case(0.5 if fault == "no_mean_scale" else 1.0)
+    y_ref = graphnorm(Bounded.exact(h), ptr, w, b, ms, 1e-5)[0]
+    cols = {"one_pass": [1], "no_eps": [2], "no_mean_scale": list(range(GN_W))}[fault]
+    y = _gn_emulate(h, ptr, w, b, ms, fault=fault)
+    y_ref[:, cols].check(_gn_emulate(h, ptr, w, b, ms)[:, cols])
+    with pytest.raises(AssertionError, match="outside the bound|non-finite"):
+        y_ref[:, cols].check(y[:, cols], f"graphnorm with {fault}")
