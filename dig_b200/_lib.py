@@ -182,6 +182,7 @@ SIGNATURES = {
     "dig3d_gsphere_place": [c_int64, c_int32, c_int32, P, P, P, P, P, P, P, P, P, P, P],
     "dig3d_gsphere_gather_local": [P, c_int64, c_int32, c_int32, P, P, P, c_int32, P, P],
     "dig3d_gsphere_type_scale": [P, c_int32, P, P, c_int64, c_int32, c_int32, P, P, P],
+    "dig3d_mmd_terms": [P, c_int64, c_int64, c_double, c_int32, c_double, P, c_int64, P, P],
 }
 _RESTYPES = {"dig3d_last_error": c_char_p, "dig3d_h16_packed_bytes": c_int64}
 
@@ -215,7 +216,8 @@ def load():
 
 
 # Launch accounting (bench.py's `gpu_launches`) and optional per-kernel CUDA-event timing
-# (bench.py's roofline pass).  Every entry point except scan/ptr helpers launches exactly one kernel.
+# (bench.py's roofline pass).  Every entry point except scan/ptr helpers and dig3d_mmd_terms (three kernels) launches
+# exactly one kernel.
 launch_count = 0
 _timing = None            # None, or dict name -> list of (start_event, stop_event)
 

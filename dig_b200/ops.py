@@ -1386,6 +1386,7 @@ def linear_set_config(cfg):
 
 # ----------------------------------------------------------------------------- G-SphereNet generation (csrc/gsphere.cu)
 I64 = torch.int64
+F64 = torch.float64
 
 
 def gsphere_edge_flags(g):
@@ -1502,3 +1503,36 @@ def gsphere_type_scale(latent, emb, feat, n_mols, n_atoms):
         call("dig3d_gsphere_type_scale", _p(latent, F32, "latent"), latent.size(1), _p(emb, F32, "emb"),
              _p(feat, F32, "feat"), n_mols, n_atoms, width, _p(type_id), _p(out), _stream())
     return type_id, out
+
+
+# ---- bond-length MMD (csrc/mmd.cu) -------------------------------------------------------------------------------------
+_MMD_CTAS_PER_SM = 4          # the pair kernel's occupancy (256 threads, 62 registers): one wave of persistent CTAs
+
+
+def mmd_terms(source, target, kernel_mul=2.0, kernel_num=5, fix_sigma=None):
+    """(bandwidth, XX, YY, XY) of compute_mmd (eval_bond_mmd_utils.py:44-97) as a 4-element fp64 tensor on the device.
+
+    source / target: 1-D float32 or float64 tensors, concatenated and cast to fp64 here (the reference's torch.cat
+    promotes a float32 + float64 pair the same way; two float32 inputs are computed in fp64 too).  CPU tensors are copied
+    to the current CUDA device.  fix_sigma: None or 0 selects the data bandwidth.  One launch sequence on the current
+    stream, no host synchronisation."""
+    for name, t in (("source", source), ("target", target)):
+        if not isinstance(t, torch.Tensor):
+            raise TypeError(f"mmd_terms: {name} must be a torch.Tensor, got {type(t)}")
+        if t.dim() != 1 or t.dtype not in (torch.float32, torch.float64):
+            raise TypeError(f"mmd_terms: {name} must be a 1-D float32 / float64 tensor, got {t.dtype} {tuple(t.shape)}")
+    if not torch.cuda.is_available():
+        raise RuntimeError("mmd_terms needs a CUDA device (sm_90a); there is no CPU fallback")
+    devs = {t.device for t in (source, target) if t.is_cuda}
+    if len(devs) > 1:
+        raise ValueError(f"mmd_terms: source and target are on different devices {sorted(map(str, devs))}")
+    dev = devs.pop() if devs else torch.device("cuda", torch.cuda.current_device())
+    kernel_num = int(kernel_num)
+    with torch.cuda.device(dev):
+        v = torch.cat([source.to(dev, F64), target.to(dev, F64)]).contiguous()
+        ctas = _MMD_CTAS_PER_SM * torch.cuda.get_device_properties(dev).multi_processor_count
+        ws = torch.empty(3 * ctas, dtype=F64, device=dev)
+        out = torch.empty(4, dtype=F64, device=dev)
+        call("dig3d_mmd_terms", _p(v, F64, "v", align=8), source.numel(), target.numel(), float(kernel_mul), kernel_num,
+             float(fix_sigma) if fix_sigma else 0.0, _p(ws), ws.numel(), _p(out), _stream())
+    return out

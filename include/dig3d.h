@@ -683,6 +683,17 @@ int dig3d_gsphere_gather_local(const float* feat, int64_t n_mols, int32_t n_atom
 int dig3d_gsphere_type_scale(const float* latent, int32_t dim, const float* emb, const float* feat, int64_t n_mols,
                              int32_t n_atoms, int32_t width, int64_t* type_out, float* out, void* stream);
 
+/* ------------------------------------------------------------------ bond-length MMD (csrc/mmd.cu)
+ * compute_mmd, reference dig/ggraph3D/utils/eval_bond_mmd_utils.py:44-97, in fp64: v[n_source + n_target] = [source;
+ * target].  out[0] = bandwidth b (fix_sigma if non-zero, else sum_ij (v_i - v_j)^2 / (n^2 - n) from a two-pass centred
+ * sum), out[1..3] = XX / n_s^2, YY / n_t^2, XY / (n_s n_t), the sums over S x S, T x T, S x T (diagonals included) of
+ * sum_k exp(-d^2 / b_k), b_k = b / kernel_mul^(kernel_num / 2) * kernel_mul^k, 1 <= kernel_num <= 64.  Three launches;
+ * workspace[workspace_len] (>= 3 doubles) takes 3 partials per CTA of the persistent pair grid (workspace_len / 3 CTAs),
+ * reduced in a fixed order: the result is deterministic for a given workspace_len.  Empty or constant input gives NaN
+ * terms, as in the reference. */
+int dig3d_mmd_terms(const double* v, int64_t n_source, int64_t n_target, double kernel_mul, int32_t kernel_num,
+                    double fix_sigma, double* workspace, int64_t workspace_len, double* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
