@@ -352,7 +352,8 @@ class _EdgeBasis(torch.autograd.Function):
 class _BasisProject(torch.autograd.Function):
     """lin_sbf1(sbf) / lin_t1(tbf) of up to four layers with the fused basis-projection kernel (basis.cu).  Backward:
     weight gradients with the harmonics recomputed on chip (the [T, ns*ns*nr] basis is never materialised) and, on the
-    force path, d/d(dist_kj) and d/d(angle) of the sbf branch (the torsion branch has no geometry backward yet)."""
+    force path, d/d(dist_kj), d/d(angle) and, for the torsion models, d/d(torsion) of both branches
+    (ops.triplet_basis_project_bwd_geom)."""
 
     @staticmethod
     def forward(ctx, g, bess, dist, angle, tors_angle, geo_cfg, basis_id, ns, nr, n_layers, torsion, *weights):
