@@ -1536,3 +1536,44 @@ def mmd_terms(source, target, kernel_mul=2.0, kernel_num=5, fix_sigma=None):
         call("dig3d_mmd_terms", _p(v, F64, "v", align=8), source.numel(), target.numel(), float(kernel_mul), kernel_num,
              float(fix_sigma) if fix_sigma else 0.0, _p(ws), ws.numel(), _p(out), _stream())
     return out
+
+
+# ---- xyz2mol (csrc/xyz2mol.cu) -----------------------------------------------------------------------------------------
+XYZ2MOL_MAX_ATOMS = 64        # AC rows are uint64 masks in csrc/xyz2mol.cuh
+
+
+def xyz2mol(z, pos):
+    """Bond-order matrices and validity flags of G molecules with n atoms each (xyz2mol with use_graph=True, reference
+    eval_validity_utils.py:382-405), on the device.
+
+    z: [G, n] tensor of an integer dtype (atomic numbers; any value is accepted, elements outside H, C, N, O, F bond to
+    nothing and make a molecule invalid, as in the reference).  pos: [G, n, 3] float32 / float64 tensor, converted to
+    fp64 exactly.  CPU tensors are copied to the current CUDA device.  1 <= n <= 64 (ValueError otherwise).
+    Returns (bo [G, n, n] int8, valid [G] int8) on the device: one launch on the current stream, no host
+    synchronisation.  valid is 1 / 0; -1 marks an internal capacity overflow of the matching (see xyz2mol.cuh)."""
+    for name, t in (("z", z), ("pos", pos)):
+        if not isinstance(t, torch.Tensor):
+            raise TypeError(f"xyz2mol: {name} must be a torch.Tensor, got {type(t)}")
+    if z.dtype.is_floating_point or z.dtype.is_complex or z.dtype == torch.bool:
+        raise TypeError(f"xyz2mol: z must have an integer dtype, got {z.dtype}")
+    if pos.dtype not in (torch.float32, torch.float64):
+        raise TypeError(f"xyz2mol: pos must be float32 / float64, got {pos.dtype}")
+    if z.dim() != 2 or pos.dim() != 3 or pos.size(2) != 3 or tuple(pos.shape[:2]) != tuple(z.shape):
+        raise ValueError(f"xyz2mol: expected z [G, n] and pos [G, n, 3], got {tuple(z.shape)} and {tuple(pos.shape)}")
+    g, n = z.shape
+    if not 1 <= n <= XYZ2MOL_MAX_ATOMS:
+        raise ValueError(f"xyz2mol: molecules need 1 to {XYZ2MOL_MAX_ATOMS} atoms, got {n}")
+    if not torch.cuda.is_available():
+        raise RuntimeError("xyz2mol needs a CUDA device (sm_90a); there is no CPU fallback")
+    devs = {t.device for t in (z, pos) if t.is_cuda}
+    if len(devs) > 1:
+        raise ValueError(f"xyz2mol: z and pos are on different devices {sorted(map(str, devs))}")
+    dev = devs.pop() if devs else torch.device("cuda", torch.cuda.current_device())
+    with torch.cuda.device(dev):
+        zd = z.to(dev, I64).contiguous()
+        pd = pos.to(dev, F64).contiguous()
+        bo = torch.empty((g, n, n), dtype=torch.int8, device=dev)
+        valid = torch.empty(g, dtype=torch.int8, device=dev)
+        call("dig3d_xyz2mol", _p(zd, I64, "z", align=8), _p(pd, F64, "pos", align=8), g, n, _p(bo), _p(valid),
+             _stream())
+    return bo, valid

@@ -694,6 +694,15 @@ int dig3d_gsphere_type_scale(const float* latent, int32_t dim, const float* emb,
 int dig3d_mmd_terms(const double* v, int64_t n_source, int64_t n_target, double kernel_mul, int32_t kernel_num,
                     double fix_sigma, double* workspace, int64_t workspace_len, double* out, void* stream);
 
+/* ------------------------------------------------------------------ xyz2mol (csrc/xyz2mol.cu, csrc/xyz2mol.cuh)
+ * xyz2mol(use_graph=True), reference dig/ggraph3D/utils/eval_validity_utils.py:382-405, for n_mols molecules of n_atoms
+ * atoms each (1 <= n_atoms <= 64): z[n_mols * n_atoms] atomic numbers (any value; elements other than H, C, N, O, F
+ * bond to nothing and make the molecule invalid), pos[n_mols * n_atoms * 3] fp64 coordinates.  Writes the bond-order
+ * matrix bo[n_mols * n_atoms * n_atoms] (row-major per molecule) and valid[n_mols] (1 / 0; -1 would mark an internal
+ * capacity overflow of the matching, which the bounds in xyz2mol.cuh rule out).  One launch, one thread per molecule. */
+int dig3d_xyz2mol(const int64_t* z, const double* pos, int64_t n_mols, int32_t n_atoms, int8_t* bo, int8_t* valid,
+                  void* stream);
+
 #ifdef __cplusplus
 }
 #endif
