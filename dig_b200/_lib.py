@@ -184,6 +184,7 @@ SIGNATURES = {
     "dig3d_gsphere_type_scale": [P, c_int32, P, P, c_int64, c_int32, c_int32, P, P, P],
     "dig3d_mmd_terms": [P, c_int64, c_int64, c_double, c_int32, c_double, P, c_int64, P, P],
     "dig3d_xyz2mol": [P, P, c_int64, c_int32, P, P, P],
+    "dig3d_gen_traj": [P, P, P, P, c_int64, P, P, P, P, P, P, P, P, P, P, P, P, P],
 }
 _RESTYPES = {"dig3d_last_error": c_char_p, "dig3d_h16_packed_bytes": c_int64}
 

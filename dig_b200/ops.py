@@ -1577,3 +1577,73 @@ def xyz2mol(z, pos):
         call("dig3d_xyz2mol", _p(zd, I64, "z", align=8), _p(pd, F64, "pos", align=8), g, n, _p(bo), _p(valid),
              _stream())
     return bo, valid
+
+
+# ---- G-SphereNet trajectories (csrc/gen_traj.cu) -----------------------------------------------------------------------
+GEN_TRAJ_MAX_ATOMS = 32       # one warp per molecule, one lane per atom
+GEN_TRAJ_FIELDS = ("atom_type", "position", "batch", "cannot_focus", "focus", "c1_focus", "c2_c1_focus",
+                   "new_atom_type", "new_dist", "new_angle", "new_torsion")
+
+
+def gen_traj_ptr(n_atoms):
+    """[6, M + 1] int64 exclusive prefix sums of dig3d_gen_traj (atoms, n^2, rows, steps, angles, torsions) for the
+    atom counts n_atoms [M] (host int64 tensor)."""
+    n = n_atoms.to(I64)
+    counts = torch.stack([n, n * n, n * (n - 1) // 2, n - 1, (n - 2).clamp_min(0), (n - 3).clamp_min(0)])
+    ptr = torch.zeros((6, n.numel() + 1), dtype=I64)
+    torch.cumsum(counts, dim=1, out=ptr[:, 1:])
+    return ptr
+
+
+def gen_traj(atom_type, pos, con, n_atoms, device=None):
+    """Every field of QM93DGEN.get (reference ggraph3D_dataset.py:192-302) for M molecules, on the device.
+
+    atom_type [N] integer, pos [N, 3] float32 and con [sum n^2] integer (each molecule's n x n bond matrix, row-major,
+    back to back) are the molecules concatenated; n_atoms [M] their atom counts, 2 <= n <= 32 (ValueError otherwise).
+    Positions must be finite.  Host tensors are copied to `device` (default: the current CUDA device).
+    Returns (out, ptr, status): out maps each name of GEN_TRAJ_FIELDS to one device tensor holding all molecules' rows
+    (get()'s dtypes; c1_focus [., 2], c2_c1_focus [., 3], the others 1-D); ptr = gen_traj_ptr(n_atoms) on the host, whose
+    rows 2..5 index the row / step / angle / torsion fields; status [M] int32 on the device (1: the molecule's spanning
+    tree has no edge, all its atoms coincide).  One launch on the current stream, no host synchronisation."""
+    for name, t in (("atom_type", atom_type), ("pos", pos), ("con", con), ("n_atoms", n_atoms)):
+        if not isinstance(t, torch.Tensor):
+            raise TypeError(f"gen_traj: {name} must be a torch.Tensor, got {type(t)}")
+    for name, t in (("atom_type", atom_type), ("con", con), ("n_atoms", n_atoms)):
+        if t.dtype.is_floating_point or t.dtype.is_complex or t.dtype == torch.bool:
+            raise TypeError(f"gen_traj: {name} must have an integer dtype, got {t.dtype}")
+    if pos.dtype != torch.float32:
+        raise TypeError(f"gen_traj: pos must be float32, got {pos.dtype}")
+    n_cpu = n_atoms.detach().to("cpu", I64).reshape(-1)
+    if n_cpu.numel() and (int(n_cpu.min()) < 2 or int(n_cpu.max()) > GEN_TRAJ_MAX_ATOMS):
+        raise ValueError(f"gen_traj: molecules need 2 to {GEN_TRAJ_MAX_ATOMS} atoms, got "
+                         f"{int(n_cpu.min())} .. {int(n_cpu.max())}")
+    ptr = gen_traj_ptr(n_cpu)
+    tot = ptr[:, -1].tolist()
+    if (atom_type.dim() != 1 or atom_type.numel() != tot[0] or tuple(pos.shape) != (tot[0], 3)
+            or con.dim() != 1 or con.numel() != tot[1]):
+        raise ValueError(f"gen_traj: expected atom_type [{tot[0]}], pos [{tot[0]}, 3] and con [{tot[1]}], got "
+                         f"{tuple(atom_type.shape)}, {tuple(pos.shape)} and {tuple(con.shape)}")
+    if not bool(torch.isfinite(pos).all()):
+        raise ValueError("gen_traj: positions must be finite")
+    if not torch.cuda.is_available():
+        raise RuntimeError("gen_traj needs a CUDA device (sm_90a); there is no CPU fallback")
+    dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+    rows, steps, angles, torsions = tot[2:]
+    with torch.cuda.device(dev):
+        z = atom_type.to(dev, I64).contiguous()
+        p = pos.to(dev).contiguous()
+        c = con.to(dev, I64).contiguous()
+        ptr_d = ptr.to(dev)
+        # at least one element each, so that no pointer is NULL when a field is empty (e.g. only 2-atom molecules)
+        e = lambda r, *w, dtype=I64: torch.empty((max(r, 1),) + w, dtype=dtype, device=dev)[:r]
+        out = dict(atom_type=e(rows), position=e(rows, 3, dtype=torch.float32), batch=e(rows),
+                   cannot_focus=e(rows, dtype=torch.float32), focus=e(steps), c1_focus=e(angles, 2),
+                   c2_c1_focus=e(torsions, 3), new_atom_type=e(steps), new_dist=e(steps, dtype=F64),
+                   new_angle=e(angles, dtype=F64), new_torsion=e(torsions, dtype=F64))
+        status = e(n_cpu.numel(), dtype=torch.int32)
+        call("dig3d_gen_traj", _p(z, I64, "atom_type", align=8), _p(p, torch.float32, "pos"), _p(c, I64, "con", align=8),
+             _p(ptr_d), n_cpu.numel(), *(_p(out[k]) for k in ("atom_type", "position", "batch", "cannot_focus", "focus",
+                                                               "c1_focus", "c2_c1_focus", "new_atom_type", "new_dist",
+                                                               "new_angle", "new_torsion")),
+             _p(status), _stream())
+    return out, ptr, status

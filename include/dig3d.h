@@ -703,6 +703,20 @@ int dig3d_mmd_terms(const double* v, int64_t n_source, int64_t n_target, double 
 int dig3d_xyz2mol(const int64_t* z, const double* pos, int64_t n_mols, int32_t n_atoms, int8_t* bo, int8_t* valid,
                   void* stream);
 
+/* ------------------------------------------------------------------ G-SphereNet trajectories (csrc/gen_traj.cu)
+ * QM93DGEN.get, reference dig/ggraph3D/dataset/ggraph3D_dataset.py:192-302, for n_mols molecules of 2 to 32 atoms, one
+ * warp per molecule.  Inputs: atom_type [N] int64, pos [N, 3] fp32, con = the molecules' n x n bond matrices back to
+ * back (int64).  ptr [6, n_mols + 1] int64 holds exclusive prefix sums per molecule of, in this order: n (atoms), n^2
+ * (con), n(n-1)/2 (trajectory rows), n-1 (steps), max(n-2, 0) (angles), max(n-3, 0) (torsions).  Writes every field of
+ * get() at the molecule's offsets: out_type / out_pos [rows, 3] / out_batch / out_cannot_focus per trajectory row,
+ * out_focus / out_new_type / out_dist per step, out_c1 [angles, 2], out_angle per angle step, out_c2 [torsions, 3],
+ * out_torsion per torsion step; atom indices are offset as get() offsets them.  status[m] = 0, or 1 where the
+ * spanning tree has no edge (one atom, or all atoms at one position; that molecule's outputs are not written). */
+int dig3d_gen_traj(const int64_t* atom_type, const float* pos, const int64_t* con, const int64_t* ptr, int64_t n_mols,
+                   int64_t* out_type, float* out_pos, int64_t* out_batch, float* out_cannot_focus, int64_t* out_focus,
+                   int64_t* out_c1, int64_t* out_c2, int64_t* out_new_type, double* out_dist, double* out_angle,
+                   double* out_torsion, int32_t* status, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
