@@ -182,6 +182,13 @@ SIGNATURES = {
     "dig3d_gsphere_place": [c_int64, c_int32, c_int32, P, P, P, P, P, P, P, P, P, P, P],
     "dig3d_gsphere_gather_local": [P, c_int64, c_int32, c_int32, P, P, P, c_int32, P, P],
     "dig3d_gsphere_type_scale": [P, c_int32, P, P, c_int64, c_int32, c_int32, P, P, P],
+    "dig3d_gsphere_att_fwd": [P, P, P, P, P, c_int64, c_int32, P, P, P],
+    "dig3d_gsphere_att_bwd": [P, P, P, P, P, P, P, c_int64, c_int32, P, P, P, P],
+    "dig3d_gsphere_flow_fwd": [P, P, P, c_int32, c_int64, c_int32, c_int32, P, P, P],
+    "dig3d_gsphere_flow_bwd": [P, P, P, c_int32, P, P, c_int64, c_int32, c_int32, P, P, P, P],
+    "dig3d_gsphere_sigmoid": [P, c_int64, P, P],
+    "dig3d_gsphere_unary_bwd": [P, P, c_int64, c_int32, P, P],
+    "dig3d_gsphere_keep_rows_bwd": [P, P, P, c_int64, c_int32, P, P, P],
     "dig3d_mmd_terms": [P, c_int64, c_int64, c_double, c_int32, c_double, P, c_int64, P, P],
     "dig3d_xyz2mol": [P, P, c_int64, c_int32, P, P, P],
     "dig3d_gen_traj": [P, P, P, P, c_int64, P, P, P, P, P, P, P, P, P, P, P, P, P],

@@ -517,3 +517,101 @@ def geometry(pos, g, n_out):
 
 def schnet_edge_features(dist, offset, coeff, cutoff):
     return _SchnetEdgeFeatures.apply(dist, offset, coeff, cutoff)
+
+
+# ------------------------------------------------------------------------------------------- G-SphereNet (gsphere_train.cu)
+class _GsphereUnary(torch.autograd.Function):
+    """tanh (the flows' hidden layer) or sigmoid (the focus classifier); backward from the saved output."""
+
+    @staticmethod
+    def forward(ctx, x, mode):
+        x = _c(x)
+        y = ops.gsphere_tanh(x) if mode == ops.GSPHERE_TANH else ops.gsphere_sigmoid(x)
+        ctx.save_for_backward(y)
+        ctx.mode = mode
+        return y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dy):
+        (y,) = ctx.saved_tensors
+        return ops.gsphere_unary_bwd(y, _c(dy), ctx.mode), None
+
+
+def tanh(x):
+    return _GsphereUnary.apply(x, ops.GSPHERE_TANH)
+
+
+def sigmoid(x):
+    return _GsphereUnary.apply(x, ops.GSPHERE_SIGMOID)
+
+
+class _KeepRows(torch.autograd.Function):
+    """G-SphereNet's masked mean re-scatters (spherenet.py:171-172, 205, 297): y[r] = x[r] on kept rows (flag[r] != 0,
+    or a non-empty CSR segment ptr[r] .. ptr[r + 1]), fallback[r] (or 0 without one) elsewhere.  The forward is the
+    inference kernel on a copy of x; the backward splits the output gradient between x and the fallback by the mask."""
+
+    @staticmethod
+    def forward(ctx, x, fallback, flag, ptr):
+        y = _c(x).clone()
+        ops.gsphere_keep_rows(y, flag=flag, ptr=ptr, fallback=None if fallback is None else _c(fallback))
+        ctx.save_for_backward(flag, ptr)
+        ctx.has_fb = fallback is not None
+        return y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dy):
+        flag, ptr = ctx.saved_tensors
+        dx, dfb = ops.gsphere_keep_rows_bwd(_c(dy), flag, ptr, want_dx=ctx.needs_input_grad[0],
+                                            want_dfb=ctx.has_fb and ctx.needs_input_grad[1])
+        return dx, dfb, None, None
+
+
+def keep_rows(x, fallback=None, flag=None, ptr=None):
+    return _KeepRows.apply(x, fallback, flag, ptr)
+
+
+class _GsphereAttention(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, q, k, v, qgraph, graph_ptr, n_heads):
+        q, k, v = _c(q), _c(k), _c(v)
+        out, stat = ops.gsphere_att_fwd(q, qgraph, graph_ptr, k, v, n_heads)
+        ctx.save_for_backward(q, k, v, qgraph, graph_ptr, stat)
+        ctx.n_heads = n_heads
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dout):
+        q, k, v, qgraph, graph_ptr, stat = ctx.saved_tensors
+        dq, dk, dv = ops.gsphere_att_bwd(_c(dout), q, qgraph, graph_ptr, k, v, stat, ctx.n_heads)
+        return dq, dk, dv, None, None, None
+
+
+def gsphere_attention(q, k, v, qgraph, graph_ptr, n_heads):
+    """MH_ATT pooling (att.py:27-34) of projected queries q [Q, 32 n_heads] over their graphs' projected keys / values."""
+    return _GsphereAttention.apply(q, k, v, qgraph, graph_ptr, n_heads)
+
+
+class _GsphereFlow(torch.autograd.Function):
+    """flow_forward (net_utils.py:83-93) given the stacked ST_Net_Exp outputs st [L, rows, 2D] and Rescale weights [L];
+    x (the data being mapped to the latent) carries no gradient."""
+
+    @staticmethod
+    def forward(ctx, st, rescale, x):
+        st, rescale, x = _c(st), _c(rescale), _c(x.detach())
+        latent, log_jac = ops.gsphere_flow_fwd(st, rescale, x)
+        ctx.save_for_backward(st, rescale, x)
+        return latent, log_jac
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dlatent, dlog_jac):
+        st, rescale, x = ctx.saved_tensors
+        dst, dres = ops.gsphere_flow_bwd(st, rescale, x, _c(dlatent), _c(dlog_jac))
+        return dst, dres, None
+
+
+def gsphere_flow(st, rescale, x):
+    return _GsphereFlow.apply(st, rescale, x)

@@ -1,5 +1,6 @@
 """G_SphereNet method class (reference dig/ggraph3D/method/G_SphereNet/gspherenet.py): the same interface; generation
-runs on the sm_90a kernels (model/sphgen.py), training is not built yet."""
+runs on the sm_90a kernels (model/sphgen.py), and so does the training likelihood SphGen.forward; the training loop
+`train` is not wired in."""
 import numpy as np
 import torch
 
@@ -27,8 +28,9 @@ class G_SphereNet():
         self.model.load_state_dict(torch.load(path, map_location=dev))
 
     def train(self, loader, lr, wd, max_epochs, model_conf_dict, checkpoint_path, save_interval, save_dir):
-        raise NotImplementedError("G_SphereNet.train: training (SphGen's likelihood forward and backward) is not built "
-                                  "on the GPU kernels yet; see DESIGN.md section 6")
+        raise NotImplementedError("G_SphereNet.train: the training loop is not wired in; train with a loop over "
+                                  "SphGen.forward (loss, BCELoss, Adam) as shown in INTEGRATION.md; see DESIGN.md "
+                                  "section 6")
 
     def generate(self, model_conf_dict, checkpoint_path, n_mols=1000, chunk_size=100, num_min_node=7, num_max_node=25,
                  temperature=[1.0, 1.0, 1.0, 1.0], focus_th=0.5, draws=None):

@@ -1,13 +1,14 @@
 """Parameter holders of G-SphereNet's flow layers and focus classifier (reference
 dig/ggraph3D/method/G_SphereNet/model/net_utils.py).  Their arithmetic during generation is in sphgen.py's step, on the
-sm_90a kernels (flow reverse: dig3d_gsphere_flow_reverse)."""
+sm_90a kernels (flow reverse: dig3d_gsphere_flow_reverse), and during training in sphgen.py's forward
+(dig3d_gsphere_flow_fwd / _bwd)."""
 import torch
 import torch.nn as nn
 
 
 def _training_not_built(what):
-    raise NotImplementedError(f"{what}: only generation (SphGen.generate) runs on the GPU kernels; the likelihood "
-                              "forward and training are not built yet (DESIGN.md section 6)")
+    raise NotImplementedError(f"{what}: the flow and focus layers run inside SphGen.forward / SphGen.generate on the "
+                              "GPU kernels, not as separate modules (DESIGN.md section 6)")
 
 
 class Rescale(nn.Module):

@@ -1,5 +1,5 @@
 """G-SphereNet's SphereNet copy (reference dig/ggraph3D/method/G_SphereNet/model/spherenet.py:218-299): node features
-[N, hidden] on the sm_90a kernels, inference only.
+[N, hidden] on the sm_90a kernels: `forward` / `dist_only_forward` for generation, `forward_train` for the likelihood.
 
 It differs from dig.threedgraph's SphereNet in four places, all handled here:
   * init_e embeds `num_node_types` node types and also returns the embedding (node_type_emb);
@@ -18,6 +18,7 @@ from torch import nn
 from .....threedgraph.method import _common
 from .....threedgraph.method._common import ResidualLayer, glorot_orthogonal, swish
 from .....threedgraph.method.dimenet_family import dist_emb
+from ..... import autograd as ag
 from ..... import ops
 
 
@@ -167,6 +168,25 @@ class SphereNet(nn.Module):
             v = _lin(lin, v, act=True)
         return ops.gsphere_keep_rows(_lin(uv.lin, v), ptr=g.row_ptr)
 
+    @staticmethod
+    def _knn_geometry(g, pos):
+        """Angles, kNN torsions and int64 triplet indices of g (geometric_computing.py:54-104).  dig3d_knn2 writes -1
+        for the missing neighbours of graphs with fewer than three atoms; only the centre atom j of a triplet k -> j -> i
+        is looked up, and a triplet needs three atoms of one graph, so those entries are never read."""
+        n, e, t = g.n_nodes, g.n_edges, g.n_triplets
+        dev = pos.device
+        nn_ = torch.empty(2, max(n, 1), dtype=torch.int32, device=dev)
+        ops.call("dig3d_knn2", ops._p(pos.detach(), torch.float32, "pos"), ops._p(g.batch, torch.int64, "batch"),
+                 ops._p(g.graph_ptr), n, g.n_graphs, ops._p(nn_[0]), ops._p(nn_[1]), ops._stream())
+        g.angle = torch.empty(t, dtype=torch.float32, device=dev)
+        g.torsion = torch.empty(t, dtype=torch.float32, device=dev)
+        g.idx_kj64 = torch.empty(t, dtype=torch.int64, device=dev)
+        g.idx_ji64 = torch.empty(t, dtype=torch.int64, device=dev)
+        if e and t:
+            ops.call("dig3d_triplet_geometry_knn", ops._p(pos.detach(), torch.float32, "pos"), ops._p(g.src),
+                     ops._p(g.dst), ops._p(g.row_ptr), ops._p(g.trip_ptr), e, ops._p(nn_[0]), ops._p(nn_[1]),
+                     ops._p(g.angle), ops._p(g.torsion), ops._p(g.idx_kj64), ops._p(g.idx_ji64), ops._stream())
+
     # ------------------------------------------------------------------ forward
     def dist_only_forward(self, z, pos, batch, num_graphs=None):
         """spherenet.py:254-271: distances only, init_e then the last update_v."""
@@ -180,20 +200,7 @@ class SphereNet(nn.Module):
         """spherenet.py:273-299."""
         with torch.no_grad():
             g = self._graph(z, pos, batch, num_graphs)
-            n, e = g.n_nodes, g.n_edges
-            dev = pos.device
-            nn_ = torch.empty(2, max(n, 1), dtype=torch.int32, device=dev)
-            ops.call("dig3d_knn2", ops._p(pos.detach(), torch.float32, "pos"), ops._p(g.batch, torch.int64, "batch"),
-                     ops._p(g.graph_ptr), n, g.n_graphs, ops._p(nn_[0]), ops._p(nn_[1]), ops._stream())
-            t = g.n_triplets
-            g.angle = torch.empty(t, dtype=torch.float32, device=dev)
-            g.torsion = torch.empty(t, dtype=torch.float32, device=dev)
-            g.idx_kj64 = torch.empty(t, dtype=torch.int64, device=dev)
-            g.idx_ji64 = torch.empty(t, dtype=torch.int64, device=dev)
-            if e and t:
-                ops.call("dig3d_triplet_geometry_knn", ops._p(pos.detach(), torch.float32, "pos"), ops._p(g.src),
-                         ops._p(g.dst), ops._p(g.row_ptr), ops._p(g.trip_ptr), e, ops._p(nn_[0]), ops._p(nn_[1]),
-                         ops._p(g.angle), ops._p(g.torsion), ops._p(g.idx_kj64), ops._p(g.idx_ji64), ops._stream())
+            self._knn_geometry(g, pos)
             rbf0, bess = self._rbf(g, want_bessel=True)
             L = len(self.update_es)
             sbf_ps, t_ps = [], []
@@ -227,3 +234,54 @@ class SphereNet(nn.Module):
                 e2 = ops.gsphere_keep_rows(e2_new, flag=flag, fallback=e2)
             v = self._update_v(self.update_vs[-1], e2, g)
             return ops.gsphere_keep_rows(v, ptr=g.out_ptr, fallback=self.init_e.emb.weight.detach(), fallback_idx=z)
+
+    def forward_train(self, z, pos, batch, num_graphs=None, want_graph=False):
+        """spherenet.py:273-299 differentiable in the parameters, over the training primitives of dig_b200.autograd (the
+        SphGen.forward feature network).  Positions are data: the graph, the geometry and the angular bases are built
+        as in `forward`.  Only update_vs[-1] runs, so init_v,
+        update_vs[:-1] and dist_emb.freq get no gradient (None), as in the reference.  want_graph: also return the graph (its graph_ptr
+        delimits the step graphs for attention pooling)."""
+        pos = pos.detach()
+        ns, nr = self.num_spherical, self.num_radial
+        g = self._graph(z, pos, batch, num_graphs)
+        self._knn_geometry(g, pos)
+        # dist_emb.freq is not trained: the reference fills it with torch.arange(out=freq) (features.py:181), which
+        # clears its requires_grad, so its gradient is None there and Adam never moves it.
+        rbf0, bess = ag.edge_basis(self.emb.dist_emb.freq.detach(), g.dist, self.cutoff, self.envelope_exponent,
+                                   self._basis_id, False, nr, ns * nr)
+        geo_cfg = (self.cutoff, self.envelope_exponent, False, g.dist)
+        sbf_ps, t_ps = [], []
+        for first in range(0, len(self.update_es), 4):
+            es = self.update_es[first:first + 4]
+            s_l, t_l = ag.basis_project(g, bess, g.dist, g.angle, g.torsion, geo_cfg, self._basis_id, ns, nr,
+                                        [m.lin_sbf1.weight for m in es], [m.lin_t1.weight for m in es])
+            sbf_ps += s_l
+            t_ps += t_l
+        flag = ops.gsphere_edge_flags(g)
+        ie, lin = self.init_e, ag.lin
+        x = ag.gather_rows(ie.emb.weight, z)                                  # node_type_emb
+        r0 = ag.lin_swish(ie.lin_rbf_0, rbf0)
+        e1 = ag.lin_swish(ie.lin, torch.cat([ag.gather_rows(x, g.dst, g.row_ptr), ag.gather_rows(x, g.src), r0], dim=-1))
+        e2 = ag.mul(lin(ie.lin_rbf_1, rbf0), e1)
+        for l, ue in enumerate(self.update_es):                              # spherenet.py:141-174
+            x_ji = ag.lin_swish(ue.lin_ji, e1)
+            x_kj = ag.lin_swish(ue.lin_kj, e1)
+            x_kj = ag.mul(x_kj, lin(ue.lin_rbf2, lin(ue.lin_rbf1, rbf0)))
+            x_kj = ag.lin_swish(ue.lin_down, x_kj)
+            x_kj = ag.triplet_gather(x_kj, sbf_ps[l], t_ps[l], ue.lin_sbf2.weight, ue.lin_t2.weight, g)
+            h = ag.add(x_ji, ag.lin_swish(ue.lin_up, x_kj))
+            for layer in ue.layers_before_skip:
+                h = ag.add(h, ag.lin_swish(layer.lin2, ag.lin_swish(layer.lin1, h)))
+            h = ag.add(ag.lin_swish(ue.lin, h), e1)
+            for layer in ue.layers_after_skip:
+                h = ag.add(h, ag.lin_swish(layer.lin2, ag.lin_swish(layer.lin1, h)))
+            e2_new = ag.mul(lin(ue.lin_rbf, rbf0), h)
+            e1 = ag.keep_rows(h, e1, flag=flag)
+            e2 = ag.keep_rows(e2_new, e2, flag=flag)
+        uv = self.update_vs[-1]                                               # spherenet.py:198-206
+        v = lin(uv.lin_up, ag.segment_sum(e2, g.row_ptr, g.dst))
+        for m in uv.lins:
+            v = ag.lin_swish(m, v)
+        v = ag.keep_rows(lin(uv.lin, v), ptr=g.row_ptr)
+        v = ag.keep_rows(v, x, ptr=g.out_ptr)                                 # spherenet.py:297
+        return (v, g) if want_graph else v

@@ -1,5 +1,5 @@
-"""SphGen (reference dig/ggraph3D/method/G_SphereNet/model/sphgen.py): the reference's module tree as a parameter
-holder, and `generate` on the sm_90a kernels.
+"""SphGen (reference dig/ggraph3D/method/G_SphereNet/model/sphgen.py): the reference's module tree, `forward` (the
+training likelihood, differentiable through dig_b200.autograd) and `generate`, both on the sm_90a kernels.
 
 A generation step of the reference runs the feature network plus ~30 small ATen ops per molecule batch.  Here a step
 is: feature network (model/spherenet.py), the focus classifier (two linears + dig3d_gsphere_focus_select, which also
@@ -16,7 +16,9 @@ latent -- are made with torch's CUDA generator and the same distributions, throu
 """
 import torch
 import torch.nn as nn
+import torch.nn.functional as F
 
+from ..... import autograd as ag
 from ..... import ops
 from .att import MH_ATT
 from .net_utils import MLP, ST_Net_Exp
@@ -75,9 +77,73 @@ class SphGen(nn.Module):
         if use_gpu and torch.cuda.is_available():
             self.to("cuda")
 
-    def forward(self, data_batch):
-        raise NotImplementedError("SphGen.forward (the likelihood used for training) is not built on the GPU kernels "
-                                  "yet; only generate() is (DESIGN.md section 6)")
+    # ------------------------------------------------------------------ likelihood (training)
+    def forward(self, data_batch, deq_noise=None):
+        """sphgen.py:44-79: the likelihood terms of a collate_fn batch already on the model's CUDA device ->
+        ((node_latent, node_log_jacob), focus_score, (dist_latent, dist_log_jacob), (angle_latent, angle_log_jacob),
+        (torsion_latent, torsion_log_jacob)), differentiable in the parameters.  dtypes follow the reference: the
+        dist / angle / torsion latents are float64 (new_dist / new_angle / new_torsion are float64 and the affine map
+        promotes), everything else float32.  deq_noise: the U[0, 1) dequantisation noise [steps, num_node_types]
+        (default: drawn with torch's CUDA generator, as the reference's torch.rand).  A batch without torsion steps
+        gives empty [0, 1] torsion tensors (whose torch.mean is NaN, as in the reference)."""
+        if not self.use_gpu or self.feat_net.init_e.emb.weight.device.type != "cuda":
+            raise NotImplementedError("SphGen.forward runs on the sm_90a kernels: the model must be on a CUDA device "
+                                      "(use_gpu=True); there is no CPU path (DESIGN.md section 6)")
+        z, pos, batch = data_batch["atom_type"], data_batch["position"], data_batch["batch"]
+        new_atom_type, focus = data_batch["new_atom_type"], data_batch["focus"]
+        c1 = [data_batch["c1_focus"][:, k].contiguous() for k in range(2)]
+        c2 = [data_batch["c2_c1_focus"][:, k].contiguous() for k in range(3)]
+        n_steps = new_atom_type.size(0)
+        dev = self.feat_net.init_e.emb.weight.device
+        node_feat, g = self.feat_net.forward_train(z, pos, batch, num_graphs=n_steps, want_graph=True)
+        lin0, lin1 = self.focus_mlp.layers[0], self.focus_mlp.layers[2]
+        focus_score = ag.sigmoid(ag.lin(lin1, ag.relu(ag.lin(lin0, node_feat)))).view(-1)
+
+        x_z = F.one_hot(new_atom_type, num_classes=self.num_node_types).float()
+        if deq_noise is None:
+            deq_noise = torch.rand(x_z.size(), device=dev)
+        elif tuple(deq_noise.shape) != tuple(x_z.shape):
+            raise ValueError(f"deq_noise: expected shape {tuple(x_z.shape)}, got {tuple(deq_noise.shape)}")
+        x_z += self.deq_coeff * deq_noise
+
+        f0 = focus[:, 0].contiguous()
+        local = ag.gather_rows(node_feat, f0)
+        node_latent, node_log_jacob = self._flow_train(
+            self.node_flow_layers, x_z,
+            torch.cat((local, self._attend_train(self.node_att, local, node_feat, batch[f0], g)), dim=-1))
+
+        emb = self.feat_net.init_e.emb.weight
+        node_emb = ag.mul(node_feat, ag.gather_rows(ag.gather_rows(emb, new_atom_type), batch, g.graph_ptr))
+        local = ag.gather_rows(node_emb, f0)
+        dist = self._flow_train(self.dist_flow_layers, data_batch["new_dist"],
+                                torch.cat((local, self._attend_train(self.dist_att, local, node_emb, batch[f0], g)), -1))
+        local = torch.cat((ag.gather_rows(node_emb, c1[1]), ag.gather_rows(node_emb, c1[0])), dim=1)
+        angle = self._flow_train(
+            self.angle_flow_layers, data_batch["new_angle"],
+            torch.cat((local, self._attend_train(self.angle_att, local, node_emb, batch[c1[0]], g)), -1))
+        local = torch.cat([ag.gather_rows(node_emb, c2[k]) for k in (2, 1, 0)], dim=1)
+        torsion = self._flow_train(
+            self.torsion_flow_layers, data_batch["new_torsion"],
+            torch.cat((local, self._attend_train(self.torsion_att, local, node_emb, batch[c2[0]], g)), -1))
+        return (node_latent, node_log_jacob), focus_score, dist, angle, torsion
+
+    @staticmethod
+    def _attend_train(att, query, keys, query_graph, g):
+        """att.py:18-35 with one query per step graph: keys / values are the rows of the query's graph."""
+        q = ag.lin(att.q_proj, query)
+        k, v = ag.lin(att.k_proj, keys), ag.lin(att.v_proj, keys)
+        return ag.lin(att.out_proj, ag.gsphere_attention(q, k, v, query_graph, g.graph_ptr, att.n_att_heads))
+
+    @staticmethod
+    def _flow_train(layers, x, feat):
+        """flow_forward (net_utils.py:83-93): the six linear1 as one stacked GEMM, tanh, the six linear2 as one grouped
+        GEMM, then the affine maps and log-Jacobian in one kernel."""
+        n_l, rows = len(layers), feat.size(0)
+        w1 = torch.cat([m.linear1.weight for m in layers], 0)
+        b1 = torch.cat([m.linear1.bias for m in layers], 0)
+        h = ag.tanh(ag.linear(feat, w1, b1)).view(rows, n_l, w1.size(0) // n_l).transpose(0, 1).contiguous()
+        st = ag.grouped_lin([m.linear2 for m in layers], h)
+        return ag.gsphere_flow(st, torch.cat([m.rescale1.weight for m in layers], 0), x)
 
     # ------------------------------------------------------------------ generation
     def _plan(self):

@@ -1505,6 +1505,110 @@ def gsphere_type_scale(latent, emb, feat, n_mols, n_atoms):
     return type_id, out
 
 
+# ---- G-SphereNet training (csrc/gsphere_train.cu) ------------------------------------------------------------------
+def _att_check(q, qgraph, graph_ptr, k, v, n_heads):
+    w = 32 * n_heads
+    if q.dim() != 2 or q.size(1) != w or k.shape != v.shape or k.dim() != 2 or k.size(1) != w:
+        raise ValueError(f"gsphere attention: q {tuple(q.shape)}, k {tuple(k.shape)}, v {tuple(v.shape)} for "
+                         f"{n_heads} heads of 32")
+    if qgraph.shape != (q.size(0),):
+        raise ValueError("gsphere attention: one graph id per query expected")
+    if graph_ptr.dim() != 1 or graph_ptr.numel() < 1:
+        raise ValueError("gsphere attention: graph_ptr must be [n_graphs + 1]")
+
+
+def gsphere_att_fwd(q, qgraph, graph_ptr, k, v, n_heads):
+    """Attention pooling of query j over the rows graph_ptr[qgraph[j]] .. graph_ptr[qgraph[j] + 1] of k / v (att.py:18-35
+    with at most one query per graph) -> (out [Q, 32 n_heads], stat [Q, n_heads, 2] = (max, denominator))."""
+    _att_check(q, qgraph, graph_ptr, k, v, n_heads)
+    n_q = q.size(0)
+    out = torch.empty(n_q, 32 * n_heads, dtype=F32, device=q.device)
+    stat = torch.empty(n_q, n_heads, 2, dtype=F32, device=q.device)
+    if n_q:
+        call("dig3d_gsphere_att_fwd", _p(q, F32, "q"), _p(qgraph, I64, "qgraph"),
+             _p(graph_ptr, torch.int32, "graph_ptr"), _p(k, F32, "k"), _p(v, F32, "v"), n_q, n_heads, _p(out),
+             _p(stat), _stream())
+    return out, stat
+
+
+def gsphere_att_bwd(dout, q, qgraph, graph_ptr, k, v, stat, n_heads):
+    """(dq, dk, dv) of gsphere_att_fwd; key rows of graphs without a query get 0."""
+    _att_check(q, qgraph, graph_ptr, k, v, n_heads)
+    dq = torch.empty_like(q)
+    dkv = torch.zeros((2,) + tuple(k.shape), dtype=F32, device=k.device)      # one fill
+    if q.size(0):
+        call("dig3d_gsphere_att_bwd", _p(dout, F32, "dout"), _p(q, F32, "q"), _p(qgraph, I64, "qgraph"),
+             _p(graph_ptr, torch.int32, "graph_ptr"), _p(k, F32, "k"), _p(v, F32, "v"), _p(stat, F32, "stat"),
+             q.size(0), n_heads, _p(dq), _p(dkv[0]), _p(dkv[1]), _stream())
+    return dq, dkv[0], dkv[1]
+
+
+def _flow_check(st, rescale, x):
+    if x.dim() != 2 or x.dtype not in (F32, F64):
+        raise ValueError(f"gsphere flow: x must be a float32 or float64 [rows, dim] tensor, got {x.dtype} "
+                         f"{tuple(x.shape)}")
+    rows, dim = x.shape
+    if tuple(st.shape) != (rescale.numel(), rows, 2 * dim):
+        raise ValueError(f"gsphere flow: st {tuple(st.shape)} vs {rescale.numel()} layers and x {tuple(x.shape)}")
+    return rows, dim, rescale.numel(), int(x.dtype == F64)
+
+
+def gsphere_flow_fwd(st, rescale, x):
+    """flow_forward (net_utils.py:83-93): st [L, rows, 2D] of the L layers, rescale [L], x [rows, D] (float32 or float64)
+    -> (latent [rows, D] in x's dtype, log_jac [rows, D] float32)."""
+    rows, dim, n_layers, f64 = _flow_check(st, rescale, x)
+    out = torch.empty_like(x)
+    log_jac = torch.empty(rows, dim, dtype=F32, device=x.device)
+    if rows:
+        call("dig3d_gsphere_flow_fwd", _p(st, F32, "st"), _p(rescale, F32, "rescale"), _p(x, x.dtype, "x"), f64, rows,
+             dim, n_layers, _p(out), _p(log_jac), _stream())
+    return out, log_jac
+
+
+def gsphere_flow_bwd(st, rescale, x, dlatent, dlog_jac):
+    """(dst [L, rows, 2D], drescale [L]) of gsphere_flow_fwd."""
+    rows, dim, n_layers, f64 = _flow_check(st, rescale, x)
+    dst = torch.empty_like(st)
+    drescale = torch.empty(n_layers, dtype=F32, device=st.device)
+    part = torch.empty(max(n_layers * rows * dim, 1), dtype=F32, device=st.device)
+    call("dig3d_gsphere_flow_bwd", _p(st, F32, "st"), _p(rescale, F32, "rescale"), _p(x, x.dtype, "x"), f64,
+         _p(dlatent, x.dtype, "dlatent"), _p(dlog_jac, F32, "dlog_jac"), rows, dim, n_layers, _p(dst), _p(part),
+         _p(drescale), _stream())
+    return dst, drescale
+
+
+def gsphere_sigmoid(x):
+    y = torch.empty_like(x)
+    if x.numel():
+        call("dig3d_gsphere_sigmoid", _p(x, F32, "x"), x.numel(), _p(y), _stream())
+    return y
+
+
+GSPHERE_TANH, GSPHERE_SIGMOID = 0, 1
+
+
+def gsphere_unary_bwd(y, dy, mode):
+    """dx from the forward output y: dy (1 - y^2) for GSPHERE_TANH, dy y (1 - y) for GSPHERE_SIGMOID."""
+    if y.shape != dy.shape:
+        raise ValueError(f"gsphere_unary_bwd: shapes differ {tuple(y.shape)} vs {tuple(dy.shape)}")
+    dx = torch.empty_like(y)
+    if y.numel():
+        call("dig3d_gsphere_unary_bwd", _p(y, F32, "y"), _p(dy, F32, "dy"), y.numel(), mode, _p(dx), _stream())
+    return dx
+
+
+def gsphere_keep_rows_bwd(dy, flag=None, ptr=None, want_dx=True, want_dfb=True):
+    """(dx, dfb) of gsphere_keep_rows with a row-aligned fallback: kept rows pass dy to x, the others to the fallback."""
+    rows = dy.size(0)
+    width = dy.numel() // max(rows, 1)
+    dx = torch.empty_like(dy) if want_dx else None
+    dfb = torch.empty_like(dy) if want_dfb else None
+    if rows and width:
+        call("dig3d_gsphere_keep_rows_bwd", _p(flag, torch.int32, "flag"), _p(ptr, torch.int32, "ptr"),
+             _p(dy, F32, "dy"), rows, width, _p(dx), _p(dfb), _stream())
+    return dx, dfb
+
+
 # ---- bond-length MMD (csrc/mmd.cu) -------------------------------------------------------------------------------------
 _MMD_CTAS_PER_SM = 4          # the pair kernel's occupancy (256 threads, 62 registers): one wave of persistent CTAs
 

@@ -683,6 +683,36 @@ int dig3d_gsphere_gather_local(const float* feat, int64_t n_mols, int32_t n_atom
 int dig3d_gsphere_type_scale(const float* latent, int32_t dim, const float* emb, const float* feat, int64_t n_mols,
                              int32_t n_atoms, int32_t width, int64_t* type_out, float* out, void* stream);
 
+/* ------------------------------------------------------------------ G-SphereNet training (csrc/gsphere_train.cu)
+ * SphGen.forward (sphgen.py:44-79) and its backward; no atomics anywhere.
+ * att_fwd: MH_ATT over ragged step graphs (att.py:18-35): query j [32*n_heads] attends to the rows
+ * graph_ptr[qgraph[j]] .. graph_ptr[qgraph[j] + 1] of k / v; stat[j, h] = (segment maximum, denominator).
+ * att_bwd: dq, and dk / dv of the key rows of every queried graph (each graph has at most one query; the caller
+ * zeroes dk / dv for the others). */
+int dig3d_gsphere_att_fwd(const float* q, const int64_t* qgraph, const int32_t* graph_ptr, const float* k,
+                          const float* v, int64_t n_queries, int32_t n_heads, float* out, float* stat, void* stream);
+int dig3d_gsphere_att_bwd(const float* dout, const float* q, const int64_t* qgraph, const int32_t* graph_ptr,
+                          const float* k, const float* v, const float* stat, int64_t n_queries, int32_t n_heads,
+                          float* dq, float* dk, float* dv, void* stream);
+/* Flow forward (net_utils.py:83-93): st[l, rows, 2*dim] = linear2 output of layer l, rescale[l] its Rescale weight;
+ * x = (x + t) * exp(exp(w_l) tanh(s)) over the layers in order, in float64 when x_f64 (x0 / x_out are double) else
+ * float; log_jac[rows, dim] (float) = sum_l log(|s_l| + 1e-20).
+ * flow_bwd: dst [n_layers, rows, 2*dim] and drescale [n_layers] from d x_out and d log_jac; part is scratch of
+ * n_layers * rows * dim floats (per-element shares of d exp(w_l), reduced in a fixed order). */
+int dig3d_gsphere_flow_fwd(const float* st, const float* rescale, const void* x0, int32_t x_f64, int64_t rows,
+                           int32_t dim, int32_t n_layers, void* x_out, float* log_jac, void* stream);
+int dig3d_gsphere_flow_bwd(const float* st, const float* rescale, const void* x0, int32_t x_f64, const void* dx_out,
+                           const float* dlog_jac, int64_t rows, int32_t dim, int32_t n_layers, float* dst, float* part,
+                           float* drescale, void* stream);
+/* y = 1 / (1 + exp(-x)) (the focus classifier's Sigmoid); unary_bwd: dx = dy (1 - y^2) (mode 0, tanh) or
+ * dy y (1 - y) (mode 1, sigmoid) from the forward output y. */
+int dig3d_gsphere_sigmoid(const float* x, int64_t n, float* y, void* stream);
+int dig3d_gsphere_unary_bwd(const float* y, const float* dy, int64_t n, int32_t mode, float* dx, void* stream);
+/* Backward of gsphere_keep_rows: dx = dy on kept rows, 0 elsewhere; dfb = dy on the other rows, 0 on kept ones (either
+ * output nullable). */
+int dig3d_gsphere_keep_rows_bwd(const int32_t* flag, const int32_t* ptr, const float* dy, int64_t rows, int32_t width,
+                                float* dx, float* dfb, void* stream);
+
 /* ------------------------------------------------------------------ bond-length MMD (csrc/mmd.cu)
  * compute_mmd, reference dig/ggraph3D/utils/eval_bond_mmd_utils.py:44-97, in fp64: v[n_source + n_target] = [source;
  * target].  out[0] = bandwidth b (fix_sigma if non-zero, else sum_ij (v_i - v_j)^2 / (n^2 - n) from a two-pass centred
