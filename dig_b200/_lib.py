@@ -174,6 +174,7 @@ SIGNATURES = {
     "dig3d_gsphere_edge_flags": [P, P, c_int64, c_int64, P, P],
     "dig3d_gsphere_keep_rows": [P, P, P, P, P, c_int64, c_int32, P],
     "dig3d_gsphere_attention": [P, P, c_int32, c_int32, c_int32, c_int64, c_int32, c_int32, P, P],
+    "dig3d_gsphere_attention_dk": [P, P, c_int32, c_int32, c_int32, c_int64, c_int32, c_int32, c_int32, P, P],
     "dig3d_gsphere_tanh": [P, c_int64, P, P],
     "dig3d_gsphere_flow_reverse": [P, P, c_int64, c_int32, c_int32, P, P],
     "dig3d_gsphere_focus_select": [P, P, c_int64, c_int32, c_int32, c_double, c_int32, P, P, P, P, P, P],
@@ -184,6 +185,8 @@ SIGNATURES = {
     "dig3d_gsphere_type_scale": [P, c_int32, P, P, c_int64, c_int32, c_int32, P, P, P],
     "dig3d_gsphere_att_fwd": [P, P, P, P, P, c_int64, c_int32, P, P, P],
     "dig3d_gsphere_att_bwd": [P, P, P, P, P, P, P, c_int64, c_int32, P, P, P, P],
+    "dig3d_gsphere_att_fwd_dk": [P, P, P, P, P, c_int64, c_int32, c_int32, P, P, P],
+    "dig3d_gsphere_att_bwd_dk": [P, P, P, P, P, P, P, c_int64, c_int32, c_int32, P, P, P, P],
     "dig3d_gsphere_flow_fwd": [P, P, P, c_int32, c_int64, c_int32, c_int32, P, P, P],
     "dig3d_gsphere_flow_bwd": [P, P, P, c_int32, P, P, c_int64, c_int32, c_int32, P, P, P, P],
     "dig3d_gsphere_sigmoid": [P, c_int64, P, P],

@@ -574,24 +574,24 @@ def keep_rows(x, fallback=None, flag=None, ptr=None):
 
 class _GsphereAttention(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, q, k, v, qgraph, graph_ptr, n_heads):
+    def forward(ctx, q, k, v, qgraph, graph_ptr, n_heads, d_k):
         q, k, v = _c(q), _c(k), _c(v)
-        out, stat = ops.gsphere_att_fwd(q, qgraph, graph_ptr, k, v, n_heads)
+        out, stat = ops.gsphere_att_fwd(q, qgraph, graph_ptr, k, v, n_heads, d_k)
         ctx.save_for_backward(q, k, v, qgraph, graph_ptr, stat)
-        ctx.n_heads = n_heads
+        ctx.n_heads, ctx.d_k = n_heads, d_k
         return out
 
     @staticmethod
     @once_differentiable
     def backward(ctx, dout):
         q, k, v, qgraph, graph_ptr, stat = ctx.saved_tensors
-        dq, dk, dv = ops.gsphere_att_bwd(_c(dout), q, qgraph, graph_ptr, k, v, stat, ctx.n_heads)
-        return dq, dk, dv, None, None, None
+        dq, dk, dv = ops.gsphere_att_bwd(_c(dout), q, qgraph, graph_ptr, k, v, stat, ctx.n_heads, ctx.d_k)
+        return dq, dk, dv, None, None, None, None
 
 
-def gsphere_attention(q, k, v, qgraph, graph_ptr, n_heads):
-    """MH_ATT pooling (att.py:27-34) of projected queries q [Q, 32 n_heads] over their graphs' projected keys / values."""
-    return _GsphereAttention.apply(q, k, v, qgraph, graph_ptr, n_heads)
+def gsphere_attention(q, k, v, qgraph, graph_ptr, n_heads, d_k=32):
+    """MH_ATT pooling (att.py:27-34) of projected queries q [Q, d_k n_heads] over their graphs' projected keys / values."""
+    return _GsphereAttention.apply(q, k, v, qgraph, graph_ptr, n_heads, d_k)
 
 
 class _GsphereFlow(torch.autograd.Function):

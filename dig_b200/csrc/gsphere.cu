@@ -8,6 +8,7 @@
 #include <math.h>
 
 #include "common.cuh"
+#include "gsphere_att.cuh"
 
 using namespace dig3d;
 
@@ -79,6 +80,35 @@ __global__ void attention_kernel(const float* __restrict__ q, const float* __res
     acc = fmaf(base[(int64_t)k * ld_kv + v_off + c], __fdiv_rn(expf(s - m), denom), acc);
   }
   out[(int64_t)g * width + c] = acc;
+}
+
+// ---- attention pooling, any head width d_k (lane mapping: gsphere_att.cuh) --------------------------------------------
+// attention_kernel's op sequence with the scores summed over a head's slices; the weighted value sum runs per slice.
+__global__ void attention_dk_kernel(const float* __restrict__ q, const float* __restrict__ kv, int ld_kv, int k_off,
+                                    int v_off, int n_keys, int n_heads, int d_k, int seg, float scale,
+                                    float* __restrict__ out) {
+  const int64_t g = blockIdx.x;
+  const int warp = threadIdx.x >> 5, n_warps = blockDim.x >> 5, per_warp = 32 / seg;
+  const float* base = kv + g * n_keys * ld_kv;
+  for (int h0 = warp * per_warp; h0 < n_heads; h0 += n_warps * per_warp) {      // uniform across the warp
+    const HeadLanes l = head_lanes(h0, n_heads, d_k, seg);
+    const int64_t hc = (int64_t)l.h * d_k;
+    const float* qh = q + g * l.width + hc;
+    auto score = [&](int k) { return __fdiv_rn(l.dot(qh, base + (int64_t)k * ld_kv + k_off + hc), scale); };
+    float m = -INFINITY;
+    for (int k = 0; k < n_keys; ++k) m = fmaxf(m, score(k));
+    float sum = 0.f;
+    for (int k = 0; k < n_keys; ++k) sum += expf(score(k) - m);
+    const float denom = sum + 1e-16f;
+    for (int i = 0; i < l.slices; ++i) {
+      const bool own = l.owns(i);
+      const int64_t c = l.col(i);
+      float acc = 0.f;
+      for (int k = 0; k < n_keys; ++k)
+        acc = fmaf(own ? base[(int64_t)k * ld_kv + v_off + c] : 0.f, __fdiv_rn(expf(score(k) - m), denom), acc);
+      if (own) out[g * l.width + c] = acc;
+    }
+  }
 }
 
 // ---- flow reverse (net_utils.py:28-37,75-80) ------------------------------------------------------------------------
@@ -338,6 +368,20 @@ int dig3d_gsphere_attention(const float* q, const float* kv, int32_t ld_kv, int3
   if (n_queries == 0) return DIG3D_OK;
   attention_kernel<<<(unsigned)n_queries, 32 * n_heads, 0, (cudaStream_t)stream>>>(q, kv, ld_kv, k_off, v_off, n_keys,
                                                                                   n_heads, out);
+  DIG3D_LAUNCH_CHECK();
+  return DIG3D_OK;
+}
+
+int dig3d_gsphere_attention_dk(const float* q, const float* kv, int32_t ld_kv, int32_t k_off, int32_t v_off,
+                               int64_t n_queries, int32_t n_keys, int32_t n_heads, int32_t d_k, float* out,
+                               void* stream) {
+  DIG3D_REQUIRE(q && kv && out && n_keys > 0 && n_heads >= 1 && d_k >= 1 && n_queries >= 0 &&
+                    n_queries < (1LL << 31) && (int64_t)n_heads * d_k <= ld_kv,
+                "gsphere_attention_dk: bad arguments");
+  if (n_queries == 0) return DIG3D_OK;
+  const AttShape sh = att_shape(n_heads, d_k);
+  attention_dk_kernel<<<(unsigned)n_queries, sh.threads, 0, (cudaStream_t)stream>>>(
+      q, kv, ld_kv, k_off, v_off, n_keys, n_heads, d_k, sh.seg, sh.scale, out);
   DIG3D_LAUNCH_CHECK();
   return DIG3D_OK;
 }

@@ -8,6 +8,7 @@
 #include <math.h>
 
 #include "common.cuh"
+#include "gsphere_att.cuh"
 
 using namespace dig3d;
 
@@ -94,6 +95,87 @@ __global__ void att_bwd_kernel(const float* __restrict__ dout, const float* __re
     dv[r * width + c] = __fmul_rn(__fdiv_rn(e, denom), go);
   }
   dq[j * width + c] = gq;
+}
+
+// ---- the two kernels above at any head width d_k (lane mapping: gsphere_att.cuh) ------------------------------------
+// Same op sequences; a dot product over a head sums the lane's slices in order before the segment butterfly, and the
+// loops that accumulate or write per channel run once per slice.
+__global__ void att_fwd_dk_kernel(const float* __restrict__ q, const int64_t* __restrict__ qgraph,
+                                  const int32_t* __restrict__ graph_ptr, const float* __restrict__ k,
+                                  const float* __restrict__ v, int n_heads, int d_k, int seg, float scale,
+                                  float* __restrict__ out, float* __restrict__ stat) {
+  const int64_t j = blockIdx.x;
+  const int warp = threadIdx.x >> 5, n_warps = blockDim.x >> 5, per_warp = 32 / seg;
+  const int64_t b = qgraph[j];
+  const int64_t r0 = graph_ptr[b], r1 = graph_ptr[b + 1];
+  for (int h0 = warp * per_warp; h0 < n_heads; h0 += n_warps * per_warp) {      // uniform across the warp
+    const HeadLanes l = head_lanes(h0, n_heads, d_k, seg);
+    const int64_t hc = (int64_t)l.h * d_k;
+    const float* qh = q + j * l.width + hc;
+    auto score = [&](int64_t r) { return __fdiv_rn(l.dot(qh, k + r * l.width + hc), scale); };
+    float m = -INFINITY;
+    for (int64_t r = r0; r < r1; ++r) m = fmaxf(m, score(r));
+    float sum = 0.f;
+    for (int64_t r = r0; r < r1; ++r) sum = __fadd_rn(sum, expf(__fsub_rn(score(r), m)));
+    const float denom = __fadd_rn(sum, 1e-16f);
+    for (int i = 0; i < l.slices; ++i) {
+      const bool own = l.owns(i);
+      const int64_t c = l.col(i);
+      float acc = 0.f;
+      for (int64_t r = r0; r < r1; ++r) {
+        const float p = __fdiv_rn(expf(__fsub_rn(score(r), m)), denom);
+        acc = fmaf(own ? v[r * l.width + c] : 0.f, p, acc);
+      }
+      if (own) out[j * l.width + c] = acc;
+    }
+    if (l.head && l.s == 0) stat[(j * n_heads + l.h) * 2] = m, stat[(j * n_heads + l.h) * 2 + 1] = denom;
+  }
+}
+
+__global__ void att_bwd_dk_kernel(const float* __restrict__ dout, const float* __restrict__ q,
+                                  const int64_t* __restrict__ qgraph, const int32_t* __restrict__ graph_ptr,
+                                  const float* __restrict__ k, const float* __restrict__ v,
+                                  const float* __restrict__ stat, int n_heads, int d_k, int seg, float scale,
+                                  float* __restrict__ dq, float* __restrict__ dk, float* __restrict__ dv) {
+  const int64_t j = blockIdx.x;
+  const int warp = threadIdx.x >> 5, n_warps = blockDim.x >> 5, per_warp = 32 / seg;
+  const int64_t b = qgraph[j];
+  const int64_t r0 = graph_ptr[b], r1 = graph_ptr[b + 1];
+  for (int h0 = warp * per_warp; h0 < n_heads; h0 += n_warps * per_warp) {      // uniform across the warp
+    const HeadLanes l = head_lanes(h0, n_heads, d_k, seg);
+    const int64_t hc = (int64_t)l.h * d_k;
+    const float* qh = q + j * l.width + hc;
+    const float* goh = dout + j * l.width + hc;
+    const int64_t st = (j * n_heads + (l.head ? l.h : 0)) * 2;
+    const float m = stat[st], denom = stat[st + 1];
+    auto e_of = [&](int64_t r) {
+      return expf(__fsub_rn(__fdiv_rn(l.dot(qh, k + r * l.width + hc), scale), m));
+    };
+    auto dp_of = [&](int64_t r) { return l.dot(goh, v + r * l.width + hc); };
+    float a = 0.f;                                           // sum_r dp_r e_r
+    for (int64_t r = r0; r < r1; ++r) {
+      const float e = e_of(r);
+      a = fmaf(dp_of(r), e, a);
+    }
+    const float ds_sum = -__fdiv_rn(__fdiv_rn(a, denom), denom);
+    for (int i = 0; i < l.slices; ++i) {
+      const bool own = l.owns(i);
+      const int64_t c = l.col(i);
+      const float qv = own ? q[j * l.width + c] : 0.f, go = own ? dout[j * l.width + c] : 0.f;
+      float gq = 0.f;
+      for (int64_t r = r0; r < r1; ++r) {
+        const float e = e_of(r);
+        const float dp = dp_of(r);
+        const float dd = __fdiv_rn(__fmul_rn(e, __fadd_rn(__fdiv_rn(dp, denom), ds_sum)), scale);
+        gq = fmaf(dd, own ? k[r * l.width + c] : 0.f, gq);
+        if (own) {
+          dk[r * l.width + c] = __fmul_rn(dd, qv);
+          dv[r * l.width + c] = __fmul_rn(__fdiv_rn(e, denom), go);
+        }
+      }
+      if (own) dq[j * l.width + c] = gq;
+    }
+  }
 }
 
 // ---- affine flow, density direction (net_utils.py:83-93 over :28-37) ------------------------------------------------
@@ -241,6 +323,35 @@ int dig3d_gsphere_att_bwd(const float* dout, const float* q, const int64_t* qgra
   DIG3D_REQUIRE(dout && q && qgraph && graph_ptr && k && v && stat && dq && dk && dv, "gsphere_att_bwd: null pointer");
   att_bwd_kernel<<<(unsigned)n_queries, 32 * n_heads, 0, (cudaStream_t)stream>>>(dout, q, qgraph, graph_ptr, k, v, stat,
                                                                                 n_heads, dq, dk, dv);
+  DIG3D_LAUNCH_CHECK();
+  return DIG3D_OK;
+}
+
+int dig3d_gsphere_att_fwd_dk(const float* q, const int64_t* qgraph, const int32_t* graph_ptr, const float* k,
+                             const float* v, int64_t n_queries, int32_t n_heads, int32_t d_k, float* out, float* stat,
+                             void* stream) {
+  DIG3D_REQUIRE(n_heads >= 1 && d_k >= 1 && n_queries >= 0 && n_queries < (1LL << 31),
+                "gsphere_att_fwd_dk: bad arguments");
+  if (n_queries == 0) return DIG3D_OK;
+  DIG3D_REQUIRE(q && qgraph && graph_ptr && k && v && out && stat, "gsphere_att_fwd_dk: null pointer");
+  const AttShape sh = att_shape(n_heads, d_k);
+  att_fwd_dk_kernel<<<(unsigned)n_queries, sh.threads, 0, (cudaStream_t)stream>>>(q, qgraph, graph_ptr, k, v, n_heads,
+                                                                                 d_k, sh.seg, sh.scale, out, stat);
+  DIG3D_LAUNCH_CHECK();
+  return DIG3D_OK;
+}
+
+int dig3d_gsphere_att_bwd_dk(const float* dout, const float* q, const int64_t* qgraph, const int32_t* graph_ptr,
+                             const float* k, const float* v, const float* stat, int64_t n_queries, int32_t n_heads,
+                             int32_t d_k, float* dq, float* dk, float* dv, void* stream) {
+  DIG3D_REQUIRE(n_heads >= 1 && d_k >= 1 && n_queries >= 0 && n_queries < (1LL << 31),
+                "gsphere_att_bwd_dk: bad arguments");
+  if (n_queries == 0) return DIG3D_OK;
+  DIG3D_REQUIRE(dout && q && qgraph && graph_ptr && k && v && stat && dq && dk && dv,
+                "gsphere_att_bwd_dk: null pointer");
+  const AttShape sh = att_shape(n_heads, d_k);
+  att_bwd_dk_kernel<<<(unsigned)n_queries, sh.threads, 0, (cudaStream_t)stream>>>(
+      dout, q, qgraph, graph_ptr, k, v, stat, n_heads, d_k, sh.seg, sh.scale, dq, dk, dv);
   DIG3D_LAUNCH_CHECK();
   return DIG3D_OK;
 }

@@ -9,8 +9,10 @@ It differs from dig.threedgraph's SphereNet in four places, all handled here:
   * update_v has num_output_layers - 1 hidden linears, a biased output layer of width hidden, and ends with a mean
     re-scatter over the in-edges (:205): 0 for a node without one; forward ends with node_type_emb +
     mean over the out-edges of (v - node_type_emb) (:297), i.e. node_type_emb for a node without out-edges.
-Only the last update_v feeds the output (the others are overwritten and the u updates are commented out in the
-reference), so only that one runs.  Every dense layer runs on the exact-fp32 linear kernel (dig3d_linear).
+update_e's triplet branch runs on the fused basis projection and triplet gather at int_emb_size 64 / basis_emb_size 8,
+and op for op on materialised bases (ops.triplet_basis over the kNN torsions, ordinary linears, row gather, segment
+sum) at any other widths.  Only the last update_v feeds the output (the others are overwritten and the u updates are
+commented out in the reference), so only that one runs.  Every dense layer runs on the exact-fp32 linear kernel (dig3d_linear).
 """
 import torch
 from torch import nn
@@ -113,9 +115,6 @@ class SphereNet(nn.Module):
                  out_emb_channels, num_spherical, num_radial, envelope_exponent=5, num_before_skip=1,
                  num_after_skip=2, num_output_layers=3, act=swish):
         super().__init__()
-        if int_emb_size != 64 or basis_emb_size != 8:
-            raise NotImplementedError("G-SphereNet feature network: the triplet kernels are compiled for "
-                                      f"int_emb_size=64, basis_emb_size=8 (got {int_emb_size}, {basis_emb_size})")
         if ("dimenet", num_spherical, num_radial) not in ops.BASIS_IDS:
             raise NotImplementedError(f"no generated basis for num_spherical={num_spherical}, num_radial={num_radial}")
         if act is not swish and getattr(act, "__name__", "") != "swish":
@@ -123,6 +122,9 @@ class SphereNet(nn.Module):
         self.cutoff = cutoff
         self.num_spherical, self.num_radial, self.envelope_exponent = num_spherical, num_radial, envelope_exponent
         self._basis_id = ops.BASIS_IDS[("dimenet", num_spherical, num_radial)]
+        # The fused basis projection and triplet gather are compiled for int_emb_size 64 / basis_emb_size 8; other
+        # widths run update_e's triplet branch op for op on materialised bases (_triplet_basis, _triplet_message).
+        self._triplet_generic = int_emb_size != 64 or basis_emb_size != 8
         self.init_e = init(num_node_types, num_radial, hidden_channels, act)
         self.init_v = update_v(hidden_channels, out_emb_channels, num_output_layers, act)
         self.init_u = update_u()
@@ -187,6 +189,19 @@ class SphereNet(nn.Module):
                      ops._p(g.dst), ops._p(g.row_ptr), ops._p(g.trip_ptr), e, ops._p(nn_[0]), ops._p(nn_[1]),
                      ops._p(g.angle), ops._p(g.torsion), ops._p(g.idx_kj64), ops._p(g.idx_ji64), ops._stream())
 
+    def _triplet_basis(self, g, bess):
+        """Materialised sbf [T, ns*nr] / tbf [T, ns*ns*nr] over the kNN torsions (the generic triplet branch's inputs)."""
+        return ops.triplet_basis(bess, g.angle, g.torsion, g.idx_kj64.to(torch.int32), self._basis_id,
+                                 self.num_spherical, self.num_radial, True)
+
+    @staticmethod
+    def _triplet_message(ue, x_kj, sbf, tbf, g):
+        """spherenet.py:158-165 op for op: x_kj[idx_kj] * lin_sbf2(lin_sbf1(sbf)) * lin_t2(lin_t1(tbf)), summed per
+        idx_ji (the triplets are sorted by idx_ji: trip_ptr is its CSR)."""
+        m = ops.ewise(ops.gather_rows(x_kj, g.idx_kj64), _lin(ue.lin_sbf2, _lin(ue.lin_sbf1, sbf)), 0)
+        m = ops.ewise(m, _lin(ue.lin_t2, _lin(ue.lin_t1, tbf)), 0)
+        return ops.segment_sum(m, g.trip_ptr)
+
     # ------------------------------------------------------------------ forward
     def dist_only_forward(self, z, pos, batch, num_graphs=None):
         """spherenet.py:254-271: distances only, init_e then the last update_v."""
@@ -204,16 +219,19 @@ class SphereNet(nn.Module):
             rbf0, bess = self._rbf(g, want_bessel=True)
             L = len(self.update_es)
             sbf_ps, t_ps = [], []
-            for first in range(0, L, 4):                   # lin_sbf1 / lin_t1 of four layers per fused projection
-                es = self.update_es[first:first + 4]
-                rows = []
-                for name in ("lin_sbf1", "lin_t1"):
-                    w = torch.cat([getattr(m, name).weight.detach() for m in es], 0)
-                    rows.append(torch.cat([w, w.new_zeros(32 - w.size(0), w.size(1))], 0) if w.size(0) < 32 else w)
-                s_p, t_p = ops.triplet_basis_project(g, bess, self._basis_id, rows[0].contiguous(),
-                                                     rows[1].contiguous())
-                sbf_ps += [s_p[k] for k in range(len(es))]
-                t_ps += [t_p[k] for k in range(len(es))]
+            if self._triplet_generic:
+                sbf, tbf = self._triplet_basis(g, bess)
+            else:
+                for first in range(0, L, 4):               # lin_sbf1 / lin_t1 of four layers per fused projection
+                    es = self.update_es[first:first + 4]
+                    rows = []
+                    for name in ("lin_sbf1", "lin_t1"):
+                        w = torch.cat([getattr(m, name).weight.detach() for m in es], 0)
+                        rows.append(torch.cat([w, w.new_zeros(32 - w.size(0), w.size(1))], 0) if w.size(0) < 32 else w)
+                    s_p, t_p = ops.triplet_basis_project(g, bess, self._basis_id, rows[0].contiguous(),
+                                                         rows[1].contiguous())
+                    sbf_ps += [s_p[k] for k in range(len(es))]
+                    t_ps += [t_p[k] for k in range(len(es))]
             flag = ops.gsphere_edge_flags(g)
             e1, e2 = self._init_e(z, g, rbf0)
             for l, ue in enumerate(self.update_es):                          # spherenet.py:141-174
@@ -221,8 +239,11 @@ class SphereNet(nn.Module):
                 x_kj = _lin(ue.lin_kj, e1, act=True)
                 x_kj = ops.ewise(x_kj, _lin(ue.lin_rbf2, _lin(ue.lin_rbf1, rbf0)), 0)
                 x_kj = _lin(ue.lin_down, x_kj, act=True)
-                m = ops.sphere_triplet_gather(x_kj, sbf_ps[l], t_ps[l], g, ue.lin_sbf2.weight.detach(),
-                                              ue.lin_t2.weight.detach())
+                if self._triplet_generic:
+                    m = self._triplet_message(ue, x_kj, sbf, tbf, g)
+                else:
+                    m = ops.sphere_triplet_gather(x_kj, sbf_ps[l], t_ps[l], g, ue.lin_sbf2.weight.detach(),
+                                                  ue.lin_t2.weight.detach())
                 h = ops.ewise(x_ji, _lin(ue.lin_up, m, act=True), 1)
                 for layer in ue.layers_before_skip:
                     h = ops.ewise(h, _lin(layer.lin2, _lin(layer.lin1, h, act=True), act=True), 1)
@@ -251,12 +272,15 @@ class SphereNet(nn.Module):
                                    self._basis_id, False, nr, ns * nr)
         geo_cfg = (self.cutoff, self.envelope_exponent, False, g.dist)
         sbf_ps, t_ps = [], []
-        for first in range(0, len(self.update_es), 4):
-            es = self.update_es[first:first + 4]
-            s_l, t_l = ag.basis_project(g, bess, g.dist, g.angle, g.torsion, geo_cfg, self._basis_id, ns, nr,
-                                        [m.lin_sbf1.weight for m in es], [m.lin_t1.weight for m in es])
-            sbf_ps += s_l
-            t_ps += t_l
+        if self._triplet_generic:
+            sbf, tbf = self._triplet_basis(g, bess)       # constants: positions are data
+        else:
+            for first in range(0, len(self.update_es), 4):
+                es = self.update_es[first:first + 4]
+                s_l, t_l = ag.basis_project(g, bess, g.dist, g.angle, g.torsion, geo_cfg, self._basis_id, ns, nr,
+                                            [m.lin_sbf1.weight for m in es], [m.lin_t1.weight for m in es])
+                sbf_ps += s_l
+                t_ps += t_l
         flag = ops.gsphere_edge_flags(g)
         ie, lin = self.init_e, ag.lin
         x = ag.gather_rows(ie.emb.weight, z)                                  # node_type_emb
@@ -268,7 +292,12 @@ class SphereNet(nn.Module):
             x_kj = ag.lin_swish(ue.lin_kj, e1)
             x_kj = ag.mul(x_kj, lin(ue.lin_rbf2, lin(ue.lin_rbf1, rbf0)))
             x_kj = ag.lin_swish(ue.lin_down, x_kj)
-            x_kj = ag.triplet_gather(x_kj, sbf_ps[l], t_ps[l], ue.lin_sbf2.weight, ue.lin_t2.weight, g)
+            if self._triplet_generic:                                         # spherenet.py:158-165
+                m = ag.mul(ag.gather_rows(x_kj, g.idx_kj64), lin(ue.lin_sbf2, lin(ue.lin_sbf1, sbf)))
+                m = ag.mul(m, lin(ue.lin_t2, lin(ue.lin_t1, tbf)))
+                x_kj = ag.segment_sum(m, g.trip_ptr, g.idx_ji64)
+            else:
+                x_kj = ag.triplet_gather(x_kj, sbf_ps[l], t_ps[l], ue.lin_sbf2.weight, ue.lin_t2.weight, g)
             h = ag.add(x_ji, ag.lin_swish(ue.lin_up, x_kj))
             for layer in ue.layers_before_skip:
                 h = ag.add(h, ag.lin_swish(layer.lin2, ag.lin_swish(layer.lin1, h)))

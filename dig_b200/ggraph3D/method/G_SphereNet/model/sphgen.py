@@ -4,11 +4,15 @@ training likelihood, differentiable through dig_b200.autograd) and `generate`, b
 A generation step of the reference runs the feature network plus ~30 small ATen ops per molecule batch.  Here a step
 is: feature network (model/spherenet.py), the focus classifier (two linears + dig3d_gsphere_focus_select, which also
 decides which molecules are complete, dropped or continue and compacts them), and for node type / distance / angle /
-torsion: the local-feature gather, attention pooling (projection linears + dig3d_gsphere_attention) and the flow
+torsion: the local-feature gather, attention pooling (projection linears + dig3d_gsphere_attention, or
+dig3d_gsphere_attention_dk at head widths d_k = hidden_channels / n_att_heads other than 32) and the flow
 reverse (one GEMM over the six linear1, dig3d_gsphere_tanh, one block-diagonal GEMM over the six linear2,
 dig3d_gsphere_flow_reverse); then dig3d_gsphere_neighbors picks c1 / c2 and dig3d_gsphere_place writes the new atom.
 The molecule state (z, pos, focus) stays on the device; the one host read per step is the pair of counts
 (continuing, complete) -- the reference reads its molecule count every step as well.
+
+Any size the reference builds runs; refused are only hidden_channels not divisible by n_att_heads (the reference's
+MH_ATT cannot split it into heads), (num_spherical, num_radial) without a generated basis and a non-swish act.
 
 Randomness: the reference's two draws -- torch.multinomial over the focus candidates and Normal(0, T).sample for each
 latent -- are made with torch's CUDA generator and the same distributions, through one `draws` object
@@ -63,9 +67,9 @@ class SphGen(nn.Module):
                                                   for _ in range(num_flow_layers)])
         self.focus_mlp = MLP(hidden_channels)
         self.deq_coeff = deq_coeff
-        if hidden_channels != 32 * n_att_heads:
-            raise NotImplementedError(f"attention pooling is built for d_k = 32 (hidden_channels = 32 * n_att_heads); "
-                                      f"got hidden_channels={hidden_channels}, n_att_heads={n_att_heads}")
+        if hidden_channels % n_att_heads:
+            raise ValueError(f"hidden_channels={hidden_channels} is not a multiple of n_att_heads={n_att_heads} "
+                             f"(MH_ATT views its out_dim as n_att_heads heads of out_dim // n_att_heads)")
         self.node_att = MH_ATT(n_att_heads, q_dim=hidden_channels, k_dim=hidden_channels, v_dim=hidden_channels,
                                out_dim=hidden_channels)
         self.dist_att = MH_ATT(n_att_heads, q_dim=hidden_channels, k_dim=hidden_channels, v_dim=hidden_channels,
@@ -132,7 +136,7 @@ class SphGen(nn.Module):
         """att.py:18-35 with one query per step graph: keys / values are the rows of the query's graph."""
         q = ag.lin(att.q_proj, query)
         k, v = ag.lin(att.k_proj, keys), ag.lin(att.v_proj, keys)
-        return ag.lin(att.out_proj, ag.gsphere_attention(q, k, v, query_graph, g.graph_ptr, att.n_att_heads))
+        return ag.lin(att.out_proj, ag.gsphere_attention(q, k, v, query_graph, g.graph_ptr, att.n_att_heads, att.d_k))
 
     @staticmethod
     def _flow_train(layers, x, feat):
@@ -178,7 +182,7 @@ class SphGen(nn.Module):
 
     def _attend(self, att, query, kv, k_off, n_atoms):
         q = self._lin(att.q_proj, query)
-        pooled = ops.gsphere_attention(q, kv, n_atoms, att.n_att_heads, k_off, k_off + q.size(1))
+        pooled = ops.gsphere_attention(q, kv, n_atoms, att.n_att_heads, k_off, k_off + q.size(1), att.d_k)
         return self._lin(att.out_proj, pooled)
 
     @staticmethod

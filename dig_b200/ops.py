@@ -1410,16 +1410,22 @@ def gsphere_keep_rows(x, flag=None, ptr=None, fallback=None, fallback_idx=None):
     return x
 
 
-def gsphere_attention(q, kv, n_keys, n_heads, k_off, v_off):
-    """Multi-head attention pooling with one query per molecule over that molecule's n_keys consecutive key rows."""
-    out = torch.empty(q.size(0), 32 * n_heads, dtype=F32, device=q.device)
-    if q.size(1) != 32 * n_heads:
-        raise ValueError(f"gsphere_attention: query width {q.size(1)} != 32 * {n_heads} heads")
+def gsphere_attention(q, kv, n_keys, n_heads, k_off, v_off, d_k=32):
+    """Multi-head attention pooling with one query per molecule over that molecule's n_keys consecutive key rows; heads
+    of d_k channels (d_k = 32: dig3d_gsphere_attention, any other width: dig3d_gsphere_attention_dk)."""
+    w = d_k * n_heads
+    out = torch.empty(q.size(0), w, dtype=F32, device=q.device)
+    if q.size(1) != w:
+        raise ValueError(f"gsphere_attention: query width {q.size(1)} != {d_k} * {n_heads} heads")
     if kv.size(0) != q.size(0) * n_keys:
         raise ValueError("gsphere_attention: key rows != queries * n_keys")
     if q.size(0):
-        call("dig3d_gsphere_attention", _p(q, F32, "q"), _p(kv, F32, "kv"), kv.size(1), int(k_off), int(v_off),
-             q.size(0), int(n_keys), int(n_heads), _p(out), _stream())
+        args = (_p(q, F32, "q"), _p(kv, F32, "kv"), kv.size(1), int(k_off), int(v_off), q.size(0), int(n_keys),
+                int(n_heads))
+        if d_k == 32:
+            call("dig3d_gsphere_attention", *args, _p(out), _stream())
+        else:
+            call("dig3d_gsphere_attention_dk", *args, int(d_k), _p(out), _stream())
     return out
 
 
@@ -1506,40 +1512,48 @@ def gsphere_type_scale(latent, emb, feat, n_mols, n_atoms):
 
 
 # ---- G-SphereNet training (csrc/gsphere_train.cu) ------------------------------------------------------------------
-def _att_check(q, qgraph, graph_ptr, k, v, n_heads):
-    w = 32 * n_heads
+def _att_check(q, qgraph, graph_ptr, k, v, n_heads, d_k):
+    w = d_k * n_heads
     if q.dim() != 2 or q.size(1) != w or k.shape != v.shape or k.dim() != 2 or k.size(1) != w:
         raise ValueError(f"gsphere attention: q {tuple(q.shape)}, k {tuple(k.shape)}, v {tuple(v.shape)} for "
-                         f"{n_heads} heads of 32")
+                         f"{n_heads} heads of {d_k}")
     if qgraph.shape != (q.size(0),):
         raise ValueError("gsphere attention: one graph id per query expected")
     if graph_ptr.dim() != 1 or graph_ptr.numel() < 1:
         raise ValueError("gsphere attention: graph_ptr must be [n_graphs + 1]")
 
 
-def gsphere_att_fwd(q, qgraph, graph_ptr, k, v, n_heads):
+def gsphere_att_fwd(q, qgraph, graph_ptr, k, v, n_heads, d_k=32):
     """Attention pooling of query j over the rows graph_ptr[qgraph[j]] .. graph_ptr[qgraph[j] + 1] of k / v (att.py:18-35
-    with at most one query per graph) -> (out [Q, 32 n_heads], stat [Q, n_heads, 2] = (max, denominator))."""
-    _att_check(q, qgraph, graph_ptr, k, v, n_heads)
+    with at most one query per graph) -> (out [Q, d_k n_heads], stat [Q, n_heads, 2] = (max, denominator)).  d_k = 32
+    runs dig3d_gsphere_att_fwd, any other head width dig3d_gsphere_att_fwd_dk."""
+    _att_check(q, qgraph, graph_ptr, k, v, n_heads, d_k)
     n_q = q.size(0)
-    out = torch.empty(n_q, 32 * n_heads, dtype=F32, device=q.device)
+    out = torch.empty(n_q, d_k * n_heads, dtype=F32, device=q.device)
     stat = torch.empty(n_q, n_heads, 2, dtype=F32, device=q.device)
     if n_q:
-        call("dig3d_gsphere_att_fwd", _p(q, F32, "q"), _p(qgraph, I64, "qgraph"),
-             _p(graph_ptr, torch.int32, "graph_ptr"), _p(k, F32, "k"), _p(v, F32, "v"), n_q, n_heads, _p(out),
-             _p(stat), _stream())
+        args = (_p(q, F32, "q"), _p(qgraph, I64, "qgraph"), _p(graph_ptr, torch.int32, "graph_ptr"), _p(k, F32, "k"),
+                _p(v, F32, "v"), n_q, n_heads)
+        if d_k == 32:
+            call("dig3d_gsphere_att_fwd", *args, _p(out), _p(stat), _stream())
+        else:
+            call("dig3d_gsphere_att_fwd_dk", *args, int(d_k), _p(out), _p(stat), _stream())
     return out, stat
 
 
-def gsphere_att_bwd(dout, q, qgraph, graph_ptr, k, v, stat, n_heads):
+def gsphere_att_bwd(dout, q, qgraph, graph_ptr, k, v, stat, n_heads, d_k=32):
     """(dq, dk, dv) of gsphere_att_fwd; key rows of graphs without a query get 0."""
-    _att_check(q, qgraph, graph_ptr, k, v, n_heads)
+    _att_check(q, qgraph, graph_ptr, k, v, n_heads, d_k)
     dq = torch.empty_like(q)
     dkv = torch.zeros((2,) + tuple(k.shape), dtype=F32, device=k.device)      # one fill
     if q.size(0):
-        call("dig3d_gsphere_att_bwd", _p(dout, F32, "dout"), _p(q, F32, "q"), _p(qgraph, I64, "qgraph"),
-             _p(graph_ptr, torch.int32, "graph_ptr"), _p(k, F32, "k"), _p(v, F32, "v"), _p(stat, F32, "stat"),
-             q.size(0), n_heads, _p(dq), _p(dkv[0]), _p(dkv[1]), _stream())
+        args = (_p(dout, F32, "dout"), _p(q, F32, "q"), _p(qgraph, I64, "qgraph"),
+                _p(graph_ptr, torch.int32, "graph_ptr"), _p(k, F32, "k"), _p(v, F32, "v"), _p(stat, F32, "stat"),
+                q.size(0), n_heads)
+        if d_k == 32:
+            call("dig3d_gsphere_att_bwd", *args, _p(dq), _p(dkv[0]), _p(dkv[1]), _stream())
+        else:
+            call("dig3d_gsphere_att_bwd_dk", *args, int(d_k), _p(dq), _p(dkv[0]), _p(dkv[1]), _stream())
     return dq, dkv[0], dkv[1]
 
 

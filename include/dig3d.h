@@ -653,6 +653,11 @@ int dig3d_gsphere_keep_rows(const int32_t* flag, const int32_t* ptr, float* x, c
  * are rows g*n_keys .. of kv[*, ld_kv] at columns k_off / v_off; out = softmax-weighted value sum (d_k = 32). */
 int dig3d_gsphere_attention(const float* q, const float* kv, int32_t ld_kv, int32_t k_off, int32_t v_off,
                             int64_t n_queries, int32_t n_keys, int32_t n_heads, float* out, void* stream);
+/* The same at any head width d_k >= 1: q[n_queries, n_heads*d_k], scores divided by sqrt(d_k) computed in fp64 and
+ * rounded to fp32 (att.py); equal to dig3d_gsphere_attention at d_k = 32. */
+int dig3d_gsphere_attention_dk(const float* q, const float* kv, int32_t ld_kv, int32_t k_off, int32_t v_off,
+                               int64_t n_queries, int32_t n_keys, int32_t n_heads, int32_t d_k, float* out,
+                               void* stream);
 /* Flow reverse (net_utils.py:28-37,75-80): y = tanh(x); flow_reverse applies the n_layers ST_Net_Exp affine maps, last
  * layer first, to latent[rows, dim] in place, st[g, l, :] = linear2 output (2*dim wide) of layer l, rescale[l] = its
  * Rescale weight. */
@@ -694,6 +699,14 @@ int dig3d_gsphere_att_fwd(const float* q, const int64_t* qgraph, const int32_t* 
 int dig3d_gsphere_att_bwd(const float* dout, const float* q, const int64_t* qgraph, const int32_t* graph_ptr,
                           const float* k, const float* v, const float* stat, int64_t n_queries, int32_t n_heads,
                           float* dq, float* dk, float* dv, void* stream);
+/* att_fwd / att_bwd at any head width d_k >= 1 (rows n_heads*d_k wide, scale sqrt(d_k) in fp64 rounded to fp32);
+ * equal to the two above at d_k = 32. */
+int dig3d_gsphere_att_fwd_dk(const float* q, const int64_t* qgraph, const int32_t* graph_ptr, const float* k,
+                             const float* v, int64_t n_queries, int32_t n_heads, int32_t d_k, float* out, float* stat,
+                             void* stream);
+int dig3d_gsphere_att_bwd_dk(const float* dout, const float* q, const int64_t* qgraph, const int32_t* graph_ptr,
+                             const float* k, const float* v, const float* stat, int64_t n_queries, int32_t n_heads,
+                             int32_t d_k, float* dq, float* dk, float* dv, void* stream);
 /* Flow forward (net_utils.py:83-93): st[l, rows, 2*dim] = linear2 output of layer l, rescale[l] its Rescale weight;
  * x = (x + t) * exp(exp(w_l) tanh(s)) over the layers in order, in float64 when x_f64 (x0 / x_out are double) else
  * float; log_jac[rows, dim] (float) = sum_l log(|s_l| + 1e-20).
