@@ -99,16 +99,26 @@ __device__ __forceinline__ float rcp_ftz(float x) {
   asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
+// The FAST forms spell every rounding out (__fmul_rn / __fadd_rn cannot be contracted into an FFMA), so that how the
+// epilogues are scheduled cannot change a result bit.  One exception: hswish's final product stays a plain multiply,
+// which its callers either store or scale by H_SA (an exact power of two, which ptxas folds into the same FMUL as .M8).
 template <bool FAST>
 __device__ __forceinline__ float hswish(float x) {
-  return FAST ? x * rcp_ftz(1.0f + ex2_ftz(x * -1.4426950408889634f)) : __fdiv_rn(x, 1.0f + expf(-x));
+  return FAST ? x * rcp_ftz(__fadd_rn(1.0f, ex2_ftz(__fmul_rn(x, -1.4426950408889634f))))
+              : __fdiv_rn(x, 1.0f + expf(-x));
 }
 // H_SA * swish(t8 / H_SA): the chain keeps its activations pre-scaled by the operand scale, so the split needs no
 // multiply and the scale costs nothing (it is folded into the accumulator scale and the bias).
 template <bool FAST>
 __device__ __forceinline__ float hswish8(float t8) {
-  return FAST ? t8 * rcp_ftz(1.0f + ex2_ftz(t8 * (-1.4426950408889634f / H_SA)))
+  return FAST ? __fmul_rn(t8, rcp_ftz(__fadd_rn(1.0f, ex2_ftz(__fmul_rn(t8, -1.4426950408889634f / H_SA)))))
               : __fdiv_rn(t8, 1.0f + expf(-t8 * (1.0f / H_SA)));
+}
+// hswish8(t8) + r, with the final product and the add as ONE rounding in the FAST form (t8 * rcp + r, one FFMA)
+template <bool FAST>
+__device__ __forceinline__ float hswish8_plus(float t8, float r) {
+  return FAST ? fmaf(t8, rcp_ftz(__fadd_rn(1.0f, ex2_ftz(__fmul_rn(t8, -1.4426950408889634f / H_SA)))), r)
+              : hswish8<false>(t8) + r;
 }
 
 // ---- control warpgroup: streams every K = 32 slab of every job (layer x tile) through the ring and issues the
@@ -410,6 +420,7 @@ constexpr int R_UNIT = 64;              // edges per consumer unit: the M of one
 constexpr int R_STAGES = 8;             // two K = 128, N = 128 layers: one consumer may hold a layer the other has left
 constexpr int R_LDS = 136;              // row stride (floats) of a consumer tile: 8-byte fragment accesses are conflict free
 constexpr int R_WG = 128;
+constexpr int R_EPI_J = 8;              // column pairs per group of the e2 epilogues: tile stores wait for the group's loads
 constexpr int R_THREADS = 3 * R_WG;     // producer warpgroup + two consumer warpgroups
 // setmaxnreg: the kernel is compiled for 168 registers (384 threads); the producer drops to 40 and the consumers grow to
 // 232 (128 x 40 + 256 x 232 <= 64 K): a consumer holds the A operand (64), the chunk-0 and chunk-1 accumulators (2 x 64).
@@ -558,13 +569,29 @@ __device__ __forceinline__ void r_complete_onto(RSmem& s, float (&acc)[64], cons
       acc[i + 1] = __fadd_rn(__fadd_rn(t.y, acc[i + 1]), d[i + 1]);
     }
 }
-// the thread's fragment elements -> the consumer tile
-__device__ __forceinline__ void r_park(const float (&acc)[64], float* tile, int fr, int fc) {
+// the thread's fragment elements of column pairs j0 .. j0 + NJ - 1 (default: all) -> the consumer tile.  The epilogues
+// write the tile only after the shared-memory reads of a whole group of elements: the compiler cannot tell a tile
+// store from a later bias / gate-weight / tile load (one dynamic shared-memory base, different registers), so a store
+// ahead of a load keeps the next element's loads behind it and leaves one element's latency chain (loads, two MUFU
+// ops, the FP32 ops) exposed at a time.
+template <int NJ = 16>
+__device__ __forceinline__ void r_park(const float (&acc)[64], float* tile, int fr, int fc, int j0 = 0) {
 #pragma unroll
-  for (int j = 0; j < 16; ++j)
+  for (int j = j0; j < j0 + NJ; ++j)
 #pragma unroll
     for (int h = 0; h < 2; ++h)
       *reinterpret_cast<float2*>(tile + (fr + 8 * h) * R_LDS + 8 * j + fc) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+}
+// rbf0 rows fr, fr + 8 of the unit
+__device__ __forceinline__ void r_rbf_rows(const float* rbf, int fr, float (&rb)[2][6]) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int n = 0; n < 6; ++n) rb[h][n] = rbf[(fr + 8 * h) * 6 + n];
+}
+// the e2 gate lin_rbf(rbf0[row]) at one column (w0, w1: its lin_rbf row; shared by the thread's two rows)
+__device__ __forceinline__ float r_gate6(const float4& w0, const float2& w1, const float (&rb)[6]) {
+  return fmaf(w1.y, rb[5], fmaf(w1.x, rb[4], fmaf(w0.w, rb[3], fmaf(w0.z, rb[2], fmaf(w0.y, rb[1], __fmul_rn(w0.x, rb[0]))))));
 }
 // a consumer without a unit in this round still passes every slab of it (the ring counts both consumers per stage)
 __device__ __forceinline__ void r_skip(RSmem& s, int& it, int n) {
@@ -731,7 +758,7 @@ sphere_update_e_h16_kernel(const float* __restrict__ m, const float* __restrict_
               float t = 0.f;
 #pragma unroll
               for (int n = 0; n < 6; ++n) t = fmaf(w0[(col + u) * 6 + n], rbf[row * 6 + n], t);
-              x[u] = row < rows ? H_SA * hswish<FAST>(t + s.bias[1][col + u]) : 0.f;
+              x[u] = row < rows ? H_SA * hswish<FAST>(__fadd_rn(t, s.bias[1][col + u])) : 0.f;   // one FMUL.M8 (see hswish)
             }
             r_split(x[0], x[1], a.hi[k][r], a.lo[k][r]);
           }
@@ -759,8 +786,8 @@ sphere_update_e_h16_kernel(const float* __restrict__ m, const float* __restrict_
           for (int h = 0; h < 2; ++h) {
             const int row = fr + 8 * h, col = 8 * j + fc, i = 4 * j + 2 * h;
             const float2 t = *reinterpret_cast<const float2*>(tile + row * R_LDS + col);
-            acc[i] = fmaf(acc[i], H_INV, t.x) * (H_SA * H_SW);
-            acc[i + 1] = fmaf(acc[i + 1], H_INV, t.y) * (H_SA * H_SW);
+            acc[i] = __fmul_rn(fmaf(acc[i], H_INV, t.x), H_SA * H_SW);
+            acc[i + 1] = __fmul_rn(fmaf(acc[i + 1], H_INV, t.y), H_SA * H_SW);
           }
       } else {   // K = 384 as three K = 128 panels, A rebuilt between them; six chunks summed in order
         embedding_a(zi);                                             // panel 0: x_i
@@ -779,28 +806,27 @@ sphere_update_e_h16_kernel(const float* __restrict__ m, const float* __restrict_
         r_complete_onto(s, acc, d, tile, fr, fc, it);
       }
       // e1 = act(. + b) and the e2 tile; edge -> node sums                                     spherenet.py:211
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int row = fr + 8 * h;
-        float rb[6];
-#pragma unroll
-        for (int n = 0; n < 6; ++n) rb[n] = rbf[row * 6 + n];
+      {
+        float rb[2][6], e2[64];
+        r_rbf_rows(rbf, fr, rb);
 #pragma unroll
         for (int j = 0; j < 16; ++j) {
-          const int col = 8 * j + fc, i = 4 * j + 2 * h;
-          float e2[2];
 #pragma unroll
           for (int u = 0; u < 2; ++u) {
-            const float o = hswish<FAST>(fmaf(acc[i + u], H_INV, s.bias[0][col + u]));
-            bad |= !h_finite(o);
-            const float4 w0 = *reinterpret_cast<const float4*>(s.wr + (col + u) * 8);
-            const float2 w1 = *reinterpret_cast<const float2*>(s.wr + (col + u) * 8 + 4);
-            const float gsum = fmaf(w1.y, rb[5], fmaf(w1.x, rb[4], fmaf(w0.w, rb[3], fmaf(w0.z, rb[2],
-                               fmaf(w0.y, rb[1], w0.x * rb[0])))));
-            e2[u] = gsum * o;
-            acc[i + u] = o;
+            const int col = 8 * j + fc + u;
+            const float b = s.bias[0][col];
+            const float4 w0 = *reinterpret_cast<const float4*>(s.wr + col * 8);
+            const float2 w1 = *reinterpret_cast<const float2*>(s.wr + col * 8 + 4);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int i = 4 * j + 2 * h + u;
+              const float o = hswish<FAST>(fmaf(acc[i], H_INV, b));
+              bad |= !h_finite(o);
+              e2[i] = __fmul_rn(r_gate6(w0, w1, rb[h]), o);
+              acc[i] = o;
+            }
           }
-          *reinterpret_cast<float2*>(tile + row * R_LDS + col) = make_float2(e2[0], e2[1]);
+          if (j % R_EPI_J == R_EPI_J - 1) r_park<R_EPI_J>(e2, tile, fr, fc, j + 1 - R_EPI_J);
         }
       }
       r_bar(cw);
@@ -843,23 +869,23 @@ sphere_update_e_h16_kernel(const float* __restrict__ m, const float* __restrict_
         const float tile_scale = (q == 0 || q == 3) ? H_SA : 1.0f;   // x_ji / e1_in arrive unscaled (x H_SA is exact)
         if (q == 0 || q == 3) cp_async_wait_all();
 #pragma unroll
-        for (int j = 0; j < 16; ++j)
+        for (int j = 0; j < 16; ++j) {
+          const float2 b = *reinterpret_cast<const float2*>(&s.bias[q][8 * j + fc]);   // shared by both rows
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
-            const int row = fr + 8 * h, col = 8 * j + fc, i = 4 * j + 2 * h;
-            const float2 b = *reinterpret_cast<const float2*>(&s.bias[q][col]);
+            const int i = 4 * j + 2 * h;
             float v0 = hswish8<FAST>(fmaf(acc[i], H_SA * H_INV, b.x));
             float v1 = hswish8<FAST>(fmaf(acc[i + 1], H_SA * H_INV, b.y));
-            float2* tp2 = reinterpret_cast<float2*>(tile + row * R_LDS + col);
             if (add_tile) {
-              const float2 r = *tp2;
-              v0 += r.x * tile_scale;
-              v1 += r.y * tile_scale;
+              const float2 r = *reinterpret_cast<const float2*>(tile + (fr + 8 * h) * R_LDS + 8 * j + fc);
+              v0 = fmaf(r.x, tile_scale, v0);
+              v1 = fmaf(r.y, tile_scale, v1);
             }
-            if (to_tile) *tp2 = make_float2(v0, v1);
             acc[i] = v0;
             acc[i + 1] = v1;
           }
+        }
+        if (to_tile) r_park(acc, tile, fr, fc);
         r_acc_to_a(acc, a);
         if (q == 0) r_bar(cw);                                            // rbf / dst of the unit: visible to all
         if (q == 2) r_fetch_rows(tile, e1_in + (size_t)e0 * 128, rows, fr, fc);   // read above; q = 3 adds e1_in
@@ -872,34 +898,30 @@ sphere_update_e_h16_kernel(const float* __restrict__ m, const float* __restrict_
       r_complete<2, 128>(s, acc, d, it);
       tp(tr, 2);
       {
-        float rb[2][6];
+        float rb[2][6], e2[64];
+        r_rbf_rows(rbf, fr, rb);
 #pragma unroll
-        for (int h = 0; h < 2; ++h)
+        for (int j = 0; j < 16; ++j) {
+          float2 r[2];
 #pragma unroll
-          for (int n = 0; n < 6; ++n) rb[h][n] = rbf[(fr + 8 * h) * 6 + n];
+          for (int h = 0; h < 2; ++h) r[h] = *reinterpret_cast<const float2*>(tile + (fr + 8 * h) * R_LDS + 8 * j + fc);
 #pragma unroll
-        for (int j = 0; j < 16; ++j)
+          for (int u = 0; u < 2; ++u) {
+            const int col = 8 * j + fc + u;
+            const float b = s.bias[7][col];
+            const float4 w0 = *reinterpret_cast<const float4*>(s.wr + col * 8);
+            const float2 w1 = *reinterpret_cast<const float2*>(s.wr + col * 8 + 4);
 #pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const int row = fr + 8 * h, col = 8 * j + fc, i = 4 * j + 2 * h;
-            const float2 b = *reinterpret_cast<const float2*>(&s.bias[7][col]);
-            float2* tp2 = reinterpret_cast<float2*>(tile + row * R_LDS + col);
-            const float2 r = *tp2;
-            float e2[2];
-#pragma unroll
-            for (int u = 0; u < 2; ++u) {
-              const float v = hswish8<FAST>(fmaf(acc[i + u], H_SA * H_INV, u ? b.y : b.x)) + (u ? r.y : r.x);
-              const float o = v * (1.0f / H_SA);
+            for (int h = 0; h < 2; ++h) {
+              const int i = 4 * j + 2 * h + u;
+              const float o = __fmul_rn(hswish8_plus<FAST>(fmaf(acc[i], H_SA * H_INV, b), u ? r[h].y : r[h].x), 1.0f / H_SA);
               bad |= !h_finite(o);
-              const float4 w0 = *reinterpret_cast<const float4*>(s.wr + (col + u) * 8);
-              const float2 w1 = *reinterpret_cast<const float2*>(s.wr + (col + u) * 8 + 4);
-              const float gsum = fmaf(w1.y, rb[h][5], fmaf(w1.x, rb[h][4], fmaf(w0.w, rb[h][3], fmaf(w0.z, rb[h][2],
-                                 fmaf(w0.y, rb[h][1], w0.x * rb[h][0])))));
-              e2[u] = gsum * o;
-              acc[i + u] = o;
+              e2[i] = __fmul_rn(r_gate6(w0, w1, rb[h]), o);
+              acc[i] = o;
             }
-            *tp2 = make_float2(e2[0], e2[1]);
           }
+          if (j % R_EPI_J == R_EPI_J - 1) r_park<R_EPI_J>(e2, tile, fr, fc, j + 1 - R_EPI_J);
+        }
       }
       tp(tr, 3);
       ++lq;
@@ -927,18 +949,22 @@ sphere_update_e_h16_kernel(const float* __restrict__ m, const float* __restrict_
       tp(tr, 1);
       r_complete<2, 128>(s, acc, d, it);
       tp(tr, 2);
+      {
+        float2 b[16];   // read ahead of the x_ji stores, which the compiler cannot tell from shared-memory writes
 #pragma unroll
-      for (int j = 0; j < 16; ++j)
+        for (int j = 0; j < 16; ++j) b[j] = *reinterpret_cast<const float2*>(&s.bias_a[0][8 * j + fc]);
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int row = fr + 8 * h, col = 8 * j + fc, i = 4 * j + 2 * h;
-          const float2 b = *reinterpret_cast<const float2*>(&s.bias_a[0][col]);
-          if (row < rows) {
-            const float2 o = make_float2(hswish<FAST>(fmaf(acc[i], H_INV, b.x)), hswish<FAST>(fmaf(acc[i + 1], H_INV, b.y)));
-            bad |= !(h_finite(o.x) && h_finite(o.y));   // e1 (part A's split operand) out of range: the flag of RE_A
-            *reinterpret_cast<float2*>(P.x_ji + (size_t)(e0 + row) * 128 + col) = o;
+        for (int j = 0; j < 16; ++j)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int row = fr + 8 * h, col = 8 * j + fc, i = 4 * j + 2 * h;
+            if (row < rows) {
+              const float2 o = make_float2(hswish<FAST>(fmaf(acc[i], H_INV, b[j].x)), hswish<FAST>(fmaf(acc[i + 1], H_INV, b[j].y)));
+              bad |= !(h_finite(o.x) && h_finite(o.y));   // e1 (part A's split operand) out of range: the flag of RE_A
+              *reinterpret_cast<float2*>(P.x_ji + (size_t)(e0 + row) * 128 + col) = o;
+            }
           }
-        }
+      }
       if (MODE == RE_A) { cp_async_wait_all(); r_bar(cw); }   // rbf of the unit: visible to all
       tp(tr, 3);
       ++lq;
@@ -962,17 +988,20 @@ sphere_update_e_h16_kernel(const float* __restrict__ m, const float* __restrict_
 #pragma unroll
         for (int j = 0; j < 16; ++j)
 #pragma unroll
-          for (int h = 0; h < 2; ++h)
+          for (int u = 0; u < 2; ++u) {
+            const int col = 8 * j + fc + u;   // lin_rbf2 row and bias of the column: shared by the thread's two rows
+            const float4 w0 = *reinterpret_cast<const float4*>(s.wr2 + col * 8);
+            const float4 w1 = *reinterpret_cast<const float4*>(s.wr2 + col * 8 + 4);
+            const float b = s.bias_a[1][col];
 #pragma unroll
-            for (int u = 0; u < 2; ++u) {
-              const int col = 8 * j + fc + u, i = 4 * j + 2 * h + u;
-              const float4 w0 = *reinterpret_cast<const float4*>(s.wr2 + col * 8);
-              const float4 w1 = *reinterpret_cast<const float4*>(s.wr2 + col * 8 + 4);
+            for (int h = 0; h < 2; ++h) {
+              const int i = 4 * j + 2 * h + u;
               const float* g = r8[h];
               const float gate = fmaf(w1.w, g[7], fmaf(w1.z, g[6], fmaf(w1.y, g[5], fmaf(w1.x, g[4],
-                                 fmaf(w0.w, g[3], fmaf(w0.z, g[2], fmaf(w0.y, g[1], w0.x * g[0])))))));
-              acc[i] = hswish8<FAST>(fmaf(acc[i], H_SA * H_INV, s.bias_a[1][col])) * gate;
+                                 fmaf(w0.w, g[3], fmaf(w0.z, g[2], fmaf(w0.y, g[1], __fmul_rn(w0.x, g[0]))))))));
+              acc[i] = __fmul_rn(hswish8<FAST>(fmaf(acc[i], H_SA * H_INV, b)), gate);
             }
+          }
       }
       r_acc_to_a(acc, a);
       tp(tr, 3);
