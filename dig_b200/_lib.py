@@ -154,6 +154,7 @@ SIGNATURES = {
     "dig3d_edge_basis_bwd": [P, c_int64, c_double, c_int32, P, c_int32, c_int32, P, P, P, P],
     "dig3d_triplet_basis_project_bwd_geom": [P, P, P, P, P, P, P, P, P, P, c_int64, c_int64, c_int32, P, P, P, P,
                                              c_double, P, P, P, P],
+    "dig3d_triplet_basis_bwd": [P, P, P, P, P, P, P, P, P, P, c_int64, c_int64, c_int32, P, P, c_double, P, P, P, P],
     "dig3d_triplet_torsion_bwd": [P, P, P, P, P, P, c_int64, P, P],
     "dig3d_schnet_edge_features_bwd": [P, c_int64, P, c_int32, c_double, c_double, P, P, P, P],
     "dig3d_rowdot": [P, P, c_int64, c_int32, P, P],

@@ -397,6 +397,46 @@ class _BasisProject(torch.autograd.Function):
         return (None, None, ddist, dangle, dtors) + (None,) * 6 + tuple(out)
 
 
+class _TripletBasis(torch.autograd.Function):
+    """The materialised angular bases sbf [T, ns*nr] / tbf [T, ns*ns*nr] (ops.triplet_basis) of the generic triplet
+    branch, differentiable in the geometry: backward = d(bess)/dx of the edges (ops.edge_basis_bwd) and the reverse-mode
+    basis kernel (ops.triplet_basis_bwd) -> d dist (the k->j edge's share), d angle, d torsion."""
+
+    @staticmethod
+    def forward(ctx, bess, dist, angle, torsion, g, geo_cfg, basis_id, ns, nr, want_tbf):
+        sbf, tbf = ops.triplet_basis(bess, angle.detach(), None if torsion is None else torsion.detach(), g.idx_kj,
+                                     basis_id, ns, nr, want_tbf)
+        ctx.g, ctx.cfg, ctx.geo_cfg = g, (basis_id, ns, nr, want_tbf), geo_cfg
+        ctx.save_for_backward(bess, dist, angle, torsion)
+        ctx.set_materialize_grads(False)
+        if tbf is None:
+            return sbf
+        return sbf, tbf
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, d_sbf, d_tbf=None):
+        bess, dist, angle, torsion = ctx.saved_tensors
+        basis_id, ns, nr, want_tbf = ctx.cfg
+        if not any(ctx.needs_input_grad[1:4]) or (d_sbf is None and d_tbf is None):
+            return (None,) * 10
+        cutoff, exponent, env_on_bessel = ctx.geo_cfg
+        _, bess_dx = ops.edge_basis_bwd(dist.detach(), cutoff, exponent, None, basis_id, env_on_bessel, None, ns * nr,
+                                        want_ddist=False, want_bess_dx=True)
+        ddist, dangle, dtors = ops.triplet_basis_bwd(
+            ctx.g, bess, bess_dx, angle.detach(), None if torsion is None else torsion.detach(), basis_id,
+            None if d_sbf is None else _c(d_sbf), None if d_tbf is None else _c(d_tbf), cutoff, torsion is not None)
+        return (None, ddist if ctx.needs_input_grad[1] else None, dangle if ctx.needs_input_grad[2] else None,
+                dtors if ctx.needs_input_grad[3] else None) + (None,) * 6
+
+
+def triplet_basis(bess, dist, angle, torsion, g, geo_cfg, basis_id, ns, nr, want_tbf):
+    """-> (sbf, tbf | None) of ops.triplet_basis, differentiable in dist / angle / torsion (torsion None for DimeNet++).
+    geo_cfg = (cutoff, envelope_exponent, envelope_on_bessel); g carries idx_kj and the out-edge lists."""
+    out = _TripletBasis.apply(bess, dist, angle, torsion, g, geo_cfg, basis_id, ns, nr, want_tbf)
+    return (out[0], out[1]) if want_tbf else (out, None)
+
+
 class _TripletGather(torch.autograd.Function):
     """m[e] = sum_{t in trip(e)} x_down[kj(t)] * lin_sbf2(sbf_p[t]) * lin_t2(t_p[t])   (spherenet.py:163-171), one fused
     kernel forward and one backward (csrc/train_sphere.cu)."""

@@ -61,6 +61,11 @@ def add_dual(a, ad, b, bd):
     return y, ag.add(ad, bd)
 
 
+def gather_rows_dual(x, xd, idx):
+    """y = x[idx]; its tangent is the gathered tangent."""
+    return ag.gather_rows(x, idx), (None if xd is None else ag.gather_rows(xd, idx))
+
+
 def segment_sum_dual(x, xd, ptr, idx):
     return ag.segment_sum(x, ptr, idx), (None if xd is None else ag.segment_sum(xd, ptr, idx))
 

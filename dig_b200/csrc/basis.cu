@@ -892,6 +892,115 @@ __global__ void triplet_basis_tangent_kernel(const float* __restrict__ bess, con
   }
 }
 
+// Reverse mode of triplet_basis_kernel (the transpose of triplet_basis_tangent_kernel), for the generic triplet branch
+// (materialised bases, any int_emb_size / basis_emb_size) on the force path:
+//   dangle[t]   = sum_{l,n}  d_sbf[t][l,n]  Y_l0'(th) bess[kj][l,n] + sum_{ab,r} d_tbf[t][ab,r] dY_ab/dth bess[kj][b,r]
+//   dtorsion[t] = sum_{ab,r} d_tbf[t][ab,r] dY_ab/dph bess[kj][b,r]
+//   ddist[kj]   = (1/cutoff) sum_{t: idx_kj[t] = kj} ( sum_{l,n} d_sbf[t][l,n] Y_l0 bess_dx[kj][l,n]
+//                                                     + sum_{ab,r} d_tbf[t][ab,r] Y_ab bess_dx[kj][b,r] )
+// with bess_dx = d(bess)/dx, x = dist / cutoff (edge_basis_bwd_kernel).  The harmonics and their derivatives are the
+// generated closed forms the forward and tangent kernels call, so the three cannot drift apart.
+// One warp per (k->j) edge; lane = one triplet that uses the edge as its k->j edge, found through the out-edge lists of
+// j (edges j->i, 32 per pass): the triplet of (k->j, j->i) sits at trip_ptr[ji] + rank(k) - (rank(i) < rank(k)), the
+// order triplet_geometry writes (rank = position among j's in-edges; pos_in[ji] = rank(i), deg(j) when i is none).
+// Every triplet is the k->j triplet of exactly one edge, so dangle / dtorsion are written once each, and ddist[kj] is a
+// sum the warp owns: per-lane partials in pass order, then a fixed butterfly.  No float atomics and no kj-sorted copy
+// of the triplets: the result is the same bit for bit from run to run.  Edges that are no triplet's k->j edge get 0.
+constexpr int TBB_WARPS = 4;
+
+template <class BS>
+__global__ void __launch_bounds__(TBB_WARPS * 32)
+triplet_basis_bwd_kernel(const float* __restrict__ bess, const float* __restrict__ bess_dx,
+                         const float* __restrict__ angle, const float* __restrict__ torsion,
+                         const int32_t* __restrict__ dst, const int32_t* __restrict__ row_ptr,
+                         const int32_t* __restrict__ trip_ptr, const int32_t* __restrict__ out_ptr,
+                         const int32_t* __restrict__ out_list, const int32_t* __restrict__ pos_in, int n_edges,
+                         const float* __restrict__ d_sbf, const float* __restrict__ d_tbf, float inv_cutoff,
+                         float* __restrict__ ddist, float* __restrict__ dangle, float* __restrict__ dtorsion) {
+  constexpr int NS = BS::NS, NR = BS::NR, NB = BS::NB, NY = BS::NY;
+  __shared__ float sb[TBB_WARPS][NB], sbd[TBB_WARPS][NB];
+  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int kj = blockIdx.x * TBB_WARPS + w;
+  if (kj >= n_edges) return;                                   // uniform per warp
+  for (int c = lane; c < NB; c += 32) {
+    sb[w][c] = bess[(size_t)kj * NB + c];
+    sbd[w][c] = bess_dx[(size_t)kj * NB + c];
+  }
+  __syncwarp();
+  const int j = dst[kj], rank_k = kj - row_ptr[j];
+  const int o_lo = out_ptr[j], o_hi = out_ptr[j + 1];
+  float acc_x = 0.f;
+  for (int o0 = o_lo; o0 < o_hi; o0 += 32) {
+    const int o = o0 + lane;
+    if (o >= o_hi) continue;
+    const int ji = out_list[o], rank_i = pos_in[ji];
+    if (rank_i == rank_k) continue;                            // i == k: no triplet
+    const int t = trip_ptr[ji] + rank_k - (rank_i < rank_k ? 1 : 0);
+    const float th = angle[t];
+    float dth = 0.f, dph = 0.f, dx = 0.f;
+    if (d_sbf) {
+      const float* ds = d_sbf + (size_t)t * NB;
+      float y0[NS], y0d[NS];
+      BS::yl0(th, y0);
+      BS::yl0_dtheta(th, y0d);
+#pragma unroll
+      for (int l = 0; l < NS; ++l) {
+        float h = 0.f, hd = 0.f;
+#pragma unroll
+        for (int n = 0; n < NR; ++n) {
+          const float gr = ds[l * NR + n];
+          h = fmaf(gr, sb[w][l * NR + n], h);
+          hd = fmaf(gr, sbd[w][l * NR + n], hd);
+        }
+        dth = fmaf(y0d[l], h, dth);
+        dx = fmaf(y0[l], hd, dx);
+      }
+    }
+    if (d_tbf) {
+      const float ph = torsion[t];
+      const float* dt = d_tbf + (size_t)t * (NY * NR);
+      float H[NY], Hd[NY];
+#pragma unroll
+      for (int ab = 0; ab < NY; ++ab) {
+        const int b = ab % NS;
+        float h = 0.f, hd = 0.f;
+#pragma unroll
+        for (int r = 0; r < NR; ++r) {
+          const float gr = dt[ab * NR + r];
+          h = fmaf(gr, sb[w][b * NR + r], h);
+          hd = fmaf(gr, sbd[w][b * NR + r], hd);
+        }
+        H[ab] = h;
+        Hd[ab] = hd;
+      }
+      {
+        float y[NY];
+        BS::ylm(th, ph, y);
+#pragma unroll
+        for (int ab = 0; ab < NY; ++ab) dx = fmaf(y[ab], Hd[ab], dx);
+      }
+      {
+        float y[NY];
+        BS::ylm_dtheta(th, ph, y);
+#pragma unroll
+        for (int ab = 0; ab < NY; ++ab) dth = fmaf(y[ab], H[ab], dth);
+      }
+      {
+        float y[NY];
+        BS::ylm_dphi(th, ph, y);
+#pragma unroll
+        for (int ab = 0; ab < NY; ++ab) dph = fmaf(y[ab], H[ab], dph);
+      }
+    }
+    dangle[t] = dth;
+    if (dtorsion) dtorsion[t] = dph;
+    acc_x += dx;
+  }
+#pragma unroll
+  for (int off = 16; off; off >>= 1) acc_x += __shfl_xor_sync(0xffffffffu, acc_x, off);
+  if (lane == 0) ddist[kj] = acc_x * inv_cutoff;
+}
+
 // Backward of the fused projection w.r.t. the geometry (forces):
 //   sbf_p[q][t] = sum_l  Y_l0(angle_t)            Rs[q][l],   Rs[q][l]  = sum_r bess[kj][l,r]  w_sbf1[q][l,r]
 //   t_p[q][t]   = sum_ab Y_ab(angle_t, torsion_t) R[q][ab],   R[q][ab]  = sum_r bess[kj][b,r]  w_t1[q][ab,r]
@@ -1204,6 +1313,30 @@ int dig3d_triplet_basis_tangent(const float* bess, const float* bess_dot, const 
     case 0: triplet_basis_tangent_kernel<B76><<<grid, 128, 0, st>>>(bess, bess_dot, angle, angle_dot, torsion, torsion_dot, idx_kj, (int)n_triplets, sbf_dot, tbf_dot); break;
     case 1: triplet_basis_tangent_kernel<B36><<<grid, 128, 0, st>>>(bess, bess_dot, angle, angle_dot, torsion, torsion_dot, idx_kj, (int)n_triplets, sbf_dot, tbf_dot); break;
     default: set_error("triplet_basis_tangent: unsupported basis_id %d", basis_id); return DIG3D_EUNSUPPORTED;
+  }
+  DIG3D_LAUNCH_CHECK();
+  return DIG3D_OK;
+}
+
+int dig3d_triplet_basis_bwd(const float* bess, const float* bess_dx, const float* angle, const float* torsion,
+                            const int32_t* dst, const int32_t* row_ptr, const int32_t* trip_ptr, const int32_t* out_ptr,
+                            const int32_t* out_list, const int32_t* pos_in, int64_t n_edges, int64_t n_triplets,
+                            int32_t basis_id, const float* d_sbf, const float* d_tbf, double cutoff, float* ddist,
+                            float* dangle, float* dtorsion, void* stream) {
+  DIG3D_REQUIRE(cutoff > 0.0, "triplet_basis_bwd: cutoff must be positive");
+  if (n_edges == 0) return DIG3D_OK;
+  // without triplets every per-triplet buffer is empty (possibly NULL): only ddist (all zeros) is written
+  DIG3D_REQUIRE(bess && bess_dx && dst && row_ptr && trip_ptr && out_ptr && out_list && pos_in && ddist &&
+                    (n_triplets == 0 || (angle && dangle)), "triplet_basis_bwd: null pointer");
+  DIG3D_REQUIRE(n_triplets == 0 || !(d_tbf || dtorsion) || torsion, "triplet_basis_bwd: d_tbf / dtorsion need torsion");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int grid = ceil_div(n_edges, TBB_WARPS);
+  const float inv = 1.0f / (float)cutoff;
+  if (n_triplets == 0) { d_sbf = nullptr; d_tbf = nullptr; dtorsion = nullptr; }
+  switch (basis_id) {
+    case 0: triplet_basis_bwd_kernel<B76><<<grid, TBB_WARPS * 32, 0, st>>>(bess, bess_dx, angle, torsion, dst, row_ptr, trip_ptr, out_ptr, out_list, pos_in, (int)n_edges, d_sbf, d_tbf, inv, ddist, dangle, dtorsion); break;
+    case 1: triplet_basis_bwd_kernel<B36><<<grid, TBB_WARPS * 32, 0, st>>>(bess, bess_dx, angle, torsion, dst, row_ptr, trip_ptr, out_ptr, out_list, pos_in, (int)n_edges, d_sbf, d_tbf, inv, ddist, dangle, dtorsion); break;
+    default: set_error("triplet_basis_bwd: unsupported basis_id %d", basis_id); return DIG3D_EUNSUPPORTED;
   }
   DIG3D_LAUNCH_CHECK();
   return DIG3D_OK;

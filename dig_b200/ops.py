@@ -1087,6 +1087,26 @@ def triplet_basis_project_bwd_geom(g, bess, bess_dx, basis_id, d_sbf_p, d_t_p, w
     return ddist, dangle, dtors
 
 
+def triplet_basis_bwd(g, bess, bess_dx, angle, torsion, basis_id, d_sbf, d_tbf, cutoff, want_dtorsion):
+    """Reverse mode of `triplet_basis`: d_sbf [T, ns*nr] / d_tbf [T, ns*ns*nr] (either None = zero) ->
+    (ddist [E], the k->j edge's share through bess; dangle [T]; dtorsion [T] | None).  bess_dx: `edge_basis_bwd`'s
+    d(bess)/dx.  Needs the graph's out-edge lists (`build_graph` makes them)."""
+    dev = bess.device
+    e, t = g.n_edges, angle.numel()
+    if g.out_ptr is None or g.out_list is None or g.pos_in is None:
+        raise ValueError("triplet_basis_bwd: the graph carries no out-edge lists (build it with ops.build_graph)")
+    ddist = torch.empty(e, device=dev, dtype=F32)
+    dangle = torch.empty(t, device=dev, dtype=F32)
+    dtors = torch.empty(t, device=dev, dtype=F32) if want_dtorsion else None
+    if e == 0:
+        return ddist, dangle, dtors
+    call("dig3d_triplet_basis_bwd", _p(bess, F32, "bess"), _p(bess_dx, F32, "bess_dx"), _p(angle, F32, "angle"),
+         _p(torsion, F32, "torsion") if (want_dtorsion or d_tbf is not None) else None, _p(g.dst), _p(g.row_ptr),
+         _p(g.trip_ptr), _p(g.out_ptr), _p(g.out_list), _p(g.pos_in), e, t, int(basis_id), _p(d_sbf, F32, "d_sbf"),
+         _p(d_tbf, F32, "d_tbf"), float(cutoff), _p(ddist), _p(dangle), _p(dtors), _stream())
+    return ddist, dangle, dtors
+
+
 def schnet_edge_features_bwd(dist, offset, coeff, cutoff, dgauss, dcut):
     ddist = torch.empty_like(dist)
     if dist.numel() == 0:

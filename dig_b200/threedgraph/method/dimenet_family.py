@@ -468,7 +468,9 @@ class _DimeNetFamily(nn.Module):
         primitives of dig_b200.autograd; taken whenever autograd is recording (run.train).  Geometry and the
         spherical basis carry no parameters except dist_emb.freq, so they run on the same kernels as inference."""
         ns, nr = self.num_spherical, self.num_radial
-        ops.triplet_geometry(g, pos, use_torsion=self._torsion, want_idx=False)
+        # the generic triplet branch on the force path reads idx_kj (its bases are materialised per triplet)
+        ops.triplet_geometry(g, pos, use_torsion=self._torsion,
+                             want_idx=bool(self._triplet_generic and pos.requires_grad))
         tors_angle = None
         if pos.requires_grad:      # forces: dist / angle / torsion carry the position gradient (csrc/train_geom.cu)
             if self._torsion:
@@ -485,13 +487,14 @@ class _DimeNetFamily(nn.Module):
         sbf = tbf = None
         if self._triplet_generic:
             # triplet-branch widths the fused projection / gather kernels are not compiled for: the angular bases are
-            # materialised once (constants: no parameters) and the branch runs op for op as spherenet.py:163-171
+            # materialised once (no parameters) and the branch runs op for op as spherenet.py:163-171.  On the force
+            # path they are functions of dist / angle / torsion (ag.triplet_basis: reverse mode in csrc/basis.cu).
             if pos.requires_grad:
-                raise NotImplementedError(
-                    f"{type(self).__name__}: forces with non-default int_emb_size / basis_emb_size_angle / _torsion are not "
-                    "built (the materialised-basis path carries no geometry gradient)")
-            ops.triplet_geometry(g, pos, use_torsion=self._torsion, want_idx=True)
-            sbf, tbf = ops.triplet_basis(bess, g.angle, g.torsion, g.idx_kj, self._basis_id, ns, nr, self._torsion)
+                sbf, tbf = ag.triplet_basis(bess, dist, angle, tors_angle, g, geo_cfg[:3], self._basis_id, ns, nr,
+                                            self._torsion)
+            else:
+                ops.triplet_geometry(g, pos, use_torsion=self._torsion, want_idx=True)
+                sbf, tbf = ops.triplet_basis(bess, g.angle, g.torsion, g.idx_kj, self._basis_id, ns, nr, self._torsion)
         else:
             for first in range(0, L, 4):
                 es = self.update_es[first:first + 4]
@@ -566,13 +569,16 @@ class _DimeNetFamily(nn.Module):
         geo_cfg = (self.cutoff, self.envelope_exponent, not tors, dist)
         L = self.num_layers
         sbf_ps, t_ps = [], []
-        for first in range(0, L, 4):
-            es = self.update_es[first:first + 4]
-            s_l, t_l = ag.basis_project(g, bess, dist, angle, tors_angle, geo_cfg, self._basis_id, ns, nr,
-                                        [m.lin_sbf1.weight for m in es],
-                                        [m.lin_t1.weight for m in es] if tors else None)
-            sbf_ps += s_l
-            t_ps += t_l if t_l is not None else [None] * len(s_l)
+        if self._triplet_generic:          # materialised bases (constants here, with the tangents above)
+            sbf, tbf = ops.triplet_basis(bess, angle, tors_angle, g.idx_kj, self._basis_id, ns, nr, tors)
+        else:
+            for first in range(0, L, 4):
+                es = self.update_es[first:first + 4]
+                s_l, t_l = ag.basis_project(g, bess, dist, angle, tors_angle, geo_cfg, self._basis_id, ns, nr,
+                                            [m.lin_sbf1.weight for m in es],
+                                            [m.lin_t1.weight for m in es] if tors else None)
+                sbf_ps += s_l
+                t_ps += t_l if t_l is not None else [None] * len(s_l)
         lin, lsd, muld, addd = ag.lin, jv.lin_swish_dual, jv.mul_dual, jv.add_dual
         # init_e (spherenet.py:79-91): the embedding rows carry no tangent
         ie = self.init_e
@@ -595,10 +601,17 @@ class _DimeNetFamily(nn.Module):
             rb, rb_d = jv.lin_dual(ue.lin_rbf2, *jv.lin_dual(ue.lin_rbf1, rbf0, rbf0_d))
             x_kj, x_kj_d = muld(x_kj, x_kj_d, rb, rb_d)
             x_kj, x_kj_d = lsd(ue.lin_down, x_kj, x_kj_d)
-            s_d = ag.linear(sbf_d, ue.lin_sbf1.weight, None)                            # tangent of lin_sbf1(sbf)
-            t_d = ag.linear(tbf_d, ue.lin_t1.weight, None) if tors else None
-            x_kj, x_kj_d = jv.triplet_gather_dual(x_kj, x_kj_d, sbf_ps[l], s_d, t_ps[l], t_d, ue.lin_sbf2.weight,
-                                                  ue.lin_t2.weight if tors else None, g)
+            if self._triplet_generic:                                                   # spherenet.py:163-171
+                s, s_d = jv.lin_dual(ue.lin_sbf2, *jv.lin_dual(ue.lin_sbf1, sbf, sbf_d))
+                prod, prod_d = muld(*jv.gather_rows_dual(x_kj, x_kj_d, g.idx_kj), s, s_d)
+                if tors:
+                    prod, prod_d = muld(prod, prod_d, *jv.lin_dual(ue.lin_t2, *jv.lin_dual(ue.lin_t1, tbf, tbf_d)))
+                x_kj, x_kj_d = jv.segment_sum_dual(prod, prod_d, g.trip_ptr, g.idx_ji)
+            else:
+                s_d = ag.linear(sbf_d, ue.lin_sbf1.weight, None)                        # tangent of lin_sbf1(sbf)
+                t_d = ag.linear(tbf_d, ue.lin_t1.weight, None) if tors else None
+                x_kj, x_kj_d = jv.triplet_gather_dual(x_kj, x_kj_d, sbf_ps[l], s_d, t_ps[l], t_d, ue.lin_sbf2.weight,
+                                                      ue.lin_t2.weight if tors else None, g)
             x_kj, x_kj_d = lsd(ue.lin_up, x_kj, x_kj_d)
             h, h_d = addd(x_ji, x_ji_d, x_kj, x_kj_d)
             for layer in ue.layers_before_skip:
@@ -625,7 +638,8 @@ class SphereNet(_DimeNetFamily):
 
     Same constructor arguments and defaults.  `use_extra_node_feature=True` / `use_node_features=False` run on the
     generic primitives (the fused init_e kernels are compiled for the default 3H-wide input), and so do
-    `int_emb_size` / `basis_emb_size_*` other than the defaults (materialised bases, ordinary linears; no forces there).
+    `int_emb_size` / `basis_emb_size_angle` / `basis_emb_size_torsion` other than the defaults (materialised bases,
+    ordinary linears), energies, forces and training on forces included.
     Restrictions (raise at construction): non-swish `act`, (num_spherical, num_radial) pairs without a generated basis.  `energy_and_force=True`: forward is differentiable w.r.t. pos, and in training mode twice (force training,
     dig_b200/autograd_jvp.py)."""
     _torsion = True
@@ -644,7 +658,10 @@ class SphereNet(_DimeNetFamily):
 
 
 class DimeNetPP(_DimeNetFamily):
-    r"""Drop-in for dig.threedgraph.method.DimeNetPP (reference dimenetpp.py:207-293)."""
+    r"""Drop-in for dig.threedgraph.method.DimeNetPP (reference dimenetpp.py:207-293).
+
+    `int_emb_size` / `basis_emb_size` other than 64 / 8 run the triplet branch on the generic primitives (materialised
+    bases, ordinary linears), energies, forces and training on forces included."""
     _torsion = False
 
     def __init__(self, energy_and_force=False, cutoff=5.0, num_layers=4, hidden_channels=128, out_channels=1,

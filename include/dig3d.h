@@ -563,6 +563,10 @@ int dig3d_graphnorm_bwd(const float* h, const float* dy, const int32_t* graph_pt
  * triplet_basis_project_bwd_geom: dangle[T], ddist_kj[E] (and dtorsion[T] when the torsion arguments are given; every
  *   row written) of dig3d_triplet_basis_project given d_sbf_p / d_t_p (host arrays of 4 device pointers, NULL entries
  *   allowed) and the forward's w_sbf1 / w_t1 rows.
+ * triplet_basis_bwd: reverse mode of dig3d_triplet_basis (materialised sbf [T, ns*nr] / tbf [T, ns*ns*nr]) given
+ *   d_sbf / d_tbf (either NULL = zero): dangle[T], dtorsion[T] (NULL: skip) and ddist[E], the k->j edge's share through
+ *   bess, with bess_dx from dig3d_edge_basis_bwd.  Every row of every output written (0 for an edge that is no
+ *   triplet's k->j edge); one warp per k->j edge over the out-edge lists of dig3d_edge_fill_out, deterministic.
  * schnet_edge_features_bwd: ddist[E] from dgauss[E,G] / dcut[E] (either may be NULL).  rowdot: out[r] = a[r,:].b[r,:]. */
 int dig3d_edge_dist_bwd(const float* pos, const int32_t* src, const int32_t* dst, const float* dist, const float* ddist,
                         int64_t n_edges, float* dpos, void* stream);
@@ -578,6 +582,11 @@ int dig3d_triplet_basis_project_bwd_geom(const float* bess, const float* bess_dx
                                          const float* const* d_sbf_p, const float* const* d_t_p, const float* w_sbf1,
                                          const float* w_t1, double cutoff, float* ddist, float* dangle, float* dtorsion,
                                          void* stream);
+int dig3d_triplet_basis_bwd(const float* bess, const float* bess_dx, const float* angle, const float* torsion,
+                            const int32_t* dst, const int32_t* row_ptr, const int32_t* trip_ptr, const int32_t* out_ptr,
+                            const int32_t* out_list, const int32_t* pos_in, int64_t n_edges, int64_t n_triplets,
+                            int32_t basis_id, const float* d_sbf, const float* d_tbf, double cutoff, float* ddist,
+                            float* dangle, float* dtorsion, void* stream);
 int dig3d_triplet_torsion_bwd(const float* pos, const int32_t* src, const int32_t* dst, const int32_t* row_ptr,
                               const int32_t* trip_ptr, const float* dtorsion, int64_t n_edges, float* dpos, void* stream);
 /* ---- forward-mode (tangent) kernels of the force-TRAINING path (reference run.py:110-123; dig_b200/autograd_jvp.py) ----
