@@ -15,7 +15,7 @@
 
 namespace dig3d {
 
-constexpr int GEO_MAXDEG = 64;  // in-degree supported per node (cap <= 64)
+constexpr int GEO_MAXDEG = 64;  // the capped builder's cap, and the in-degree the warp-per-edge geometry kernel handles
 
 static thread_local char g_err[512] = "";
 void set_error(const char* fmt, ...) {
@@ -300,30 +300,105 @@ __global__ void csr_from_sorted_kernel(const int32_t* __restrict__ dst, int n_ed
   row_ptr[n] = lo;
 }
 
-__global__ void edge_triplet_count_kernel(const float* __restrict__ pos, const int32_t* __restrict__ src,
-                                          const int32_t* __restrict__ dst, const int32_t* __restrict__ row_ptr,
-                                          int n_edges, int max_deg, int32_t* __restrict__ cnt,
-                                          float* __restrict__ dist, int32_t* __restrict__ flag) {
-  const int e = blockIdx.x * blockDim.x + threadIdx.x;
-  if (e >= n_edges) return;
-  const int j = src[e], i = dst[e];
-  const int b = row_ptr[j], d = row_ptr[j + 1] - b;
-  if (d > max_deg) atomicOr(flag, 2);   // the geometry kernel parks one plane per in-neighbour in shared memory
-  cnt[e] = d - (find_sorted(src + b, d, i) >= 0 ? 1 : 0);
-  dist[e] = norm3_aten(sub3(load3(pos, i), load3(pos, j)));
+// cnt[e] = triplets of edge e = (j -> i), dist[e]; flag[1] += edges whose source has more than max_deg in-edges (the
+// heavy edges, only they pay an atomic), *t64 += the triplet total in 64 bits (one atomic per CTA): the int32 scan of
+// cnt wraps at 2^31.
+constexpr int COUNT_THREADS = 256;
+
+__global__ void __launch_bounds__(COUNT_THREADS)
+edge_triplet_count_kernel(const float* __restrict__ pos, const int32_t* __restrict__ src,
+                          const int32_t* __restrict__ dst, const int32_t* __restrict__ row_ptr, int n_edges,
+                          int max_deg, int32_t* __restrict__ cnt, float* __restrict__ dist,
+                          int32_t* __restrict__ flag, unsigned long long* __restrict__ t64) {
+  __shared__ unsigned long long warp_sum[COUNT_THREADS / 32];
+  const int e = blockIdx.x * blockDim.x + threadIdx.x, lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  unsigned long long c64 = 0;
+  if (e < n_edges) {
+    const int j = src[e], i = dst[e];
+    const int b = row_ptr[j], d = row_ptr[j + 1] - b;
+    if (d > max_deg) atomicAdd(flag + 1, 1);
+    const int c = d - (find_sorted(src + b, d, i) >= 0 ? 1 : 0);
+    cnt[e] = c;
+    c64 = (unsigned long long)c;
+    dist[e] = norm3_aten(sub3(load3(pos, i), load3(pos, j)));
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) c64 += __shfl_xor_sync(0xffffffffu, c64, o);
+  if (lane == 0) warp_sum[w] = c64;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    unsigned long long tot = 0;
+#pragma unroll
+    for (int k = 0; k < COUNT_THREADS / 32; ++k) tot += warp_sum[k];
+    if (tot) atomicAdd(t64, tot);
+  }
 }
 
 // ------------------------------------------------------------------ triplet geometry
-// One warp per edge e = (j -> i).  Lane s owns in-edge s of j (k = src[row_ptr[j]+s]); up to
-// WMAX in-edges per pass.  plane_s = cross(pos_ji, pos_k - pos_j) is both the angle's cross
-// product and the torsion's plane1/plane2, so each lane computes its plane once, parks it in
-// shared memory and every lane then scans all candidates k_n.
+// plane_s = cross(pos_ji, pos_k - pos_j) is both the angle's cross product and the torsion's plane1 / plane2, so it is
+// computed once per in-edge s of j.  The per-triplet arithmetic lives in the two device functions below, which both
+// geometry kernels call: whatever the in-degree, a triplet gets the same op sequence.
+
+// One torsion candidate k_n of the triplet with plane p1: atan2(((p1 x p2) . ji) / |ji|, p1 . p2), <= 0 -> +2pi
+//                                                              geometric_computing.py:53-75
+__device__ __forceinline__ float torsion_candidate(const f3 p1, const f3 p2, const f3 pos_ji, const float dist_ji) {
+  const float ta = sum3_aten(mul3(p1, p2));
+  const float tb = __fdiv_rn(sum3_aten(mul3(cross_aten(p1, p2), pos_ji)), dist_ji);
+  float tor = atan2f(tb, ta);
+  if (tor <= 0.0f) tor = __fadd_rn(tor, 6.2831855f);
+  return tor;
+}
+
+// best folded with fminf over the candidates planes[c], c in [0, n), c != skip (the slot of i).  fminf is exact and
+// order-independent, so a min folded tile by tile equals the min over all candidates at once.
+__device__ __forceinline__ float torsion_min_fold(float best, const f3 p1, const float (*planes)[3], int n, int skip,
+                                                  const f3 pos_ji, const float dist_ji) {
+  for (int c = 0; c < n; ++c) {
+    if (c == skip) continue;
+    const f3 p2 = {planes[c][0], planes[c][1], planes[c][2]};
+    best = fminf(best, torsion_candidate(p1, p2, pos_ji, dist_ji));
+  }
+  return best;
+}
+
+// Outputs of triplet t = (k -> j -> i) with k the in-edge kj of j and plane p1: the angle, the indices and the torsion
+// (use_torsion 1: `tor_min`, the min over all candidates folded by the caller; 2: G-SphereNet's single reference atom).
+__device__ __forceinline__ void triplet_emit(const float* __restrict__ pos, const f3 pj, const f3 pos_ji,
+                                             const float dist_ji, int k, const f3 p1, int t, int kj, int e, int j,
+                                             int i, int use_torsion, float tor_min, float* __restrict__ angle,
+                                             float* __restrict__ torsion, int32_t* __restrict__ idx_kj,
+                                             int32_t* __restrict__ idx_ji, int64_t* __restrict__ idx_kj64,
+                                             int64_t* __restrict__ idx_ji64, const int32_t* __restrict__ nn1,
+                                             const int32_t* __restrict__ nn2) {
+  // angle = atan2(|ji x jk|, ji . jk)       geometric_computing.py:44-48
+  const f3 pos_jk = sub3(load3(pos, k), pj);
+  const float a = sum3_aten(mul3(pos_ji, pos_jk));
+  const float b = norm3_aten(p1);
+  angle[t] = atan2f(b, a);
+  if (idx_kj) idx_kj[t] = kj;
+  if (idx_ji) idx_ji[t] = e;
+  if (idx_kj64) idx_kj64[t] = kj;
+  if (idx_ji64) idx_ji64[t] = e;
+  if (use_torsion == 2) {
+    // G-SphereNet's variant (ggraph3D/.../geometric_computing.py:87-103): ONE reference atom, the nearest
+    // neighbour of j in its graph, or the second nearest when the nearest is i
+    const int k_n = (nn1[j] == i) ? nn2[j] : nn1[j];
+    const f3 p2 = cross_aten(pos_ji, sub3(load3(pos, k_n), pj));
+    torsion[t] = torsion_candidate(p1, p2, pos_ji, dist_ji);
+  } else if (use_torsion) {
+    torsion[t] = tor_min;
+  }
+}
+
+// One warp per edge e = (j -> i) whose source j has at most max_deg <= GEO_MAXDEG in-edges (heavier edges are left to
+// triplet_geometry_heavy_kernel).  Lane s owns in-edge s of j (k = src[row_ptr[j]+s]), parks its plane in shared
+// memory and every lane then scans all candidates k_n.
 constexpr int GEO_WARPS = 8;
 
 __global__ void __launch_bounds__(GEO_WARPS * 32)
 triplet_geometry_kernel(const float* __restrict__ pos, const int32_t* __restrict__ src,
                         const int32_t* __restrict__ dst, const int32_t* __restrict__ row_ptr,
-                        const int32_t* __restrict__ trip_ptr, int n_edges, int use_torsion,
+                        const int32_t* __restrict__ trip_ptr, int n_edges, int max_deg, int use_torsion,
                         float* __restrict__ angle, float* __restrict__ torsion, int32_t* __restrict__ idx_kj,
                         int32_t* __restrict__ idx_ji, int64_t* __restrict__ idx_kj64,
                         int64_t* __restrict__ idx_ji64, const int32_t* __restrict__ nn1 = nullptr,
@@ -335,6 +410,7 @@ triplet_geometry_kernel(const float* __restrict__ pos, const int32_t* __restrict
   if (e >= n_edges) return;
   const int j = src[e], i = dst[e];
   const int base = row_ptr[j], d = row_ptr[j + 1] - base;
+  if (d > max_deg) return;
   const f3 pj = load3(pos, j);
   const f3 pos_ji = sub3(load3(pos, i), pj);
   const float dist_ji = norm3_aten(pos_ji);
@@ -353,44 +429,83 @@ triplet_geometry_kernel(const float* __restrict__ pos, const int32_t* __restrict
   const int t0 = trip_ptr[e];
   for (int s = lane; s < d; s += 32) {
     if (s == p_i) continue;
-    const int k = ks[w][s];
     const f3 p1 = {planes[w][s][0], planes[w][s][1], planes[w][s][2]};
-    const int t = t0 + s - (s > p_i ? 1 : 0);
-    // angle = atan2(|ji x jk|, ji . jk)       geometric_computing.py:44-48
-    const f3 pos_jk = sub3(load3(pos, k), pj);
-    const float a = sum3_aten(mul3(pos_ji, pos_jk));
-    const float b = norm3_aten(p1);
-    angle[t] = atan2f(b, a);
-    if (idx_kj) idx_kj[t] = base + s;
-    if (idx_ji) idx_ji[t] = e;
-    if (idx_kj64) idx_kj64[t] = base + s;
-    if (idx_ji64) idx_ji64[t] = e;
-    if (use_torsion == 2) {
-      // G-SphereNet's variant (ggraph3D/.../geometric_computing.py:87-103): ONE reference atom, the nearest
-      // neighbour of j in its graph, or the second nearest when the nearest is i
-      const int k_n = (nn1[j] == i) ? nn2[j] : nn1[j];
-      const f3 p2 = cross_aten(pos_ji, sub3(load3(pos, k_n), pj));
-      const float ta = sum3_aten(mul3(p1, p2));
-      const float tb = __fdiv_rn(sum3_aten(mul3(cross_aten(p1, p2), pos_ji)), dist_ji);
-      float tor = atan2f(tb, ta);
-      if (tor <= 0.0f) tor = __fadd_rn(tor, 6.2831855f);
-      torsion[t] = tor;
-    } else if (use_torsion) {
-      // min over k_n != i (k_n == k kept) of atan2(((p1 x p2).ji)/|ji|, p1.p2), <=0 -> +2pi
-      //                                         geometric_computing.py:53-75
-      float best = __int_as_float(0x7f800000);
-      for (int c = 0; c < d; ++c) {
-        if (c == p_i) continue;
-        const f3 p2 = {planes[w][c][0], planes[w][c][1], planes[w][c][2]};
-        const float ta = sum3_aten(mul3(p1, p2));
-        const float tb = __fdiv_rn(sum3_aten(mul3(cross_aten(p1, p2), pos_ji)), dist_ji);
-        float tor = atan2f(tb, ta);
-        if (tor <= 0.0f) tor = __fadd_rn(tor, 6.2831855f);
-        best = fminf(best, tor);
-      }
-      torsion[t] = best;
-    }
+    float best = __int_as_float(0x7f800000);
+    if (use_torsion == 1) best = torsion_min_fold(best, p1, planes[w], d, p_i, pos_ji, dist_ji);
+    triplet_emit(pos, pj, pos_ji, dist_ji, ks[w][s], p1, t0 + s - (s > p_i ? 1 : 0), base + s, e, j, i, use_torsion,
+                 best, angle, torsion, idx_kj, idx_ji, idx_kj64, idx_ji64, nn1, nn2);
   }
+}
+
+// One CTA per heavy edge e = (j -> i) (heavy[h], or h itself when heavy is null), any in-degree d of j.  Thread x owns
+// the triplet slots s = x, x + HEAVY_THREADS, ...; for the full-candidate torsion the CTA walks j's in-edges in tiles
+// of HEAVY_THREADS planes parked in shared memory and every thread folds its min across the tiles.  Shared memory stays
+// at one tile whatever d is; the planes of a tile are recomputed once per slot pass (d / HEAVY_THREADS passes), which
+// is small next to the d^2 torsion candidates per edge.
+constexpr int HEAVY_THREADS = 128;
+
+__global__ void __launch_bounds__(HEAVY_THREADS)
+triplet_geometry_heavy_kernel(const float* __restrict__ pos, const int32_t* __restrict__ src,
+                              const int32_t* __restrict__ dst, const int32_t* __restrict__ row_ptr,
+                              const int32_t* __restrict__ trip_ptr, const int32_t* __restrict__ heavy,
+                              int use_torsion, float* __restrict__ angle, float* __restrict__ torsion,
+                              int64_t* __restrict__ idx_kj64, int64_t* __restrict__ idx_ji64,
+                              const int32_t* __restrict__ nn1, const int32_t* __restrict__ nn2) {
+  __shared__ float planes[HEAVY_THREADS][3];
+  const int x = threadIdx.x;
+  const int e = heavy ? heavy[blockIdx.x] : (int)blockIdx.x;
+  const int j = src[e], i = dst[e];
+  const int base = row_ptr[j], d = row_ptr[j + 1] - base;
+  const f3 pj = load3(pos, j);
+  const f3 pos_ji = sub3(load3(pos, i), pj);
+  const float dist_ji = norm3_aten(pos_ji);
+  int p_i = find_sorted(src + base, d, i);                 // j's in-neighbours ascend: the edges are sorted
+  if (p_i < 0) p_i = d;
+  const int t0 = trip_ptr[e];
+  for (int s0 = 0; s0 < d; s0 += HEAVY_THREADS) {           // uniform across the CTA: every thread reaches the barriers
+    const int s = s0 + x;
+    int k = 0;
+    f3 p1 = {0.f, 0.f, 0.f};
+    if (s < d) {
+      k = src[base + s];
+      p1 = cross_aten(pos_ji, sub3(load3(pos, k), pj));
+    }
+    float best = __int_as_float(0x7f800000);
+    if (use_torsion == 1) {
+      for (int c0 = 0; c0 < d; c0 += HEAVY_THREADS) {
+        __syncthreads();                                    // the previous tile has been read
+        const int c = c0 + x;
+        if (c < d) {
+          const f3 pl = cross_aten(pos_ji, sub3(load3(pos, src[base + c]), pj));
+          planes[x][0] = pl.x; planes[x][1] = pl.y; planes[x][2] = pl.z;
+        }
+        __syncthreads();
+        if (s < d && s != p_i)
+          best = torsion_min_fold(best, p1, planes, min(HEAVY_THREADS, d - c0), p_i - c0, pos_ji, dist_ji);
+      }
+    }
+    if (s < d && s != p_i)
+      triplet_emit(pos, pj, pos_ji, dist_ji, k, p1, t0 + s - (s > p_i ? 1 : 0), base + s, e, j, i, use_torsion, best,
+                   angle, torsion, nullptr, nullptr, idx_kj64, idx_ji64, nn1, nn2);
+  }
+}
+
+// heavy[1 + h] = the edges whose source has more than max_deg in-edges (any order), heavy[0] = their number
+// (zeroed by the dispatcher).  One atomic per warp that has a heavy edge.
+__global__ void heavy_edges_kernel(const int32_t* __restrict__ src, const int32_t* __restrict__ row_ptr, int n_edges,
+                                   int max_deg, int32_t* __restrict__ heavy) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x, lane = threadIdx.x & 31;
+  bool h = false;
+  if (e < n_edges) {
+    const int j = src[e];
+    h = row_ptr[j + 1] - row_ptr[j] > max_deg;
+  }
+  const unsigned m = __ballot_sync(0xffffffffu, h);
+  if (!m) return;
+  int base = 0;
+  if (lane == 0) base = atomicAdd(heavy, __popc(m));
+  base = __shfl_sync(0xffffffffu, base, 0);
+  if (h) heavy[1 + base + __popc(m & ((1u << lane) - 1))] = e;
 }
 
 // ------------------------------------------------------------------ segment sum (sorted index as CSR)
@@ -549,8 +664,44 @@ int dig3d_triplet_geometry(const float* pos, const int32_t* src, const int32_t* 
   DIG3D_REQUIRE(!use_torsion || torsion, "triplet_geometry: torsion requested without output buffer");
   if (n_edges == 0) return DIG3D_OK;
   triplet_geometry_kernel<<<ceil_div(n_edges, GEO_WARPS), GEO_WARPS * 32, 0, (cudaStream_t)stream>>>(
-      pos, src, dst, row_ptr, trip_ptr, (int)n_edges, use_torsion, angle, torsion, idx_kj, idx_ji, idx_kj64,
-      idx_ji64);
+      pos, src, dst, row_ptr, trip_ptr, (int)n_edges, GEO_MAXDEG, use_torsion, angle, torsion, idx_kj, idx_ji,
+      idx_kj64, idx_ji64);
+  DIG3D_LAUNCH_CHECK();
+  return DIG3D_OK;
+}
+
+int dig3d_triplet_geometry_any_degree(const float* pos, const int32_t* src, const int32_t* dst,
+                                      const int32_t* row_ptr, const int32_t* trip_ptr, int64_t n_edges,
+                                      int64_t n_heavy, int32_t use_torsion, const int32_t* nn1, const int32_t* nn2,
+                                      int32_t* heavy_ws, float* angle, float* torsion, int64_t* idx_kj64,
+                                      int64_t* idx_ji64, void* stream) {
+  DIG3D_REQUIRE(pos && src && dst && row_ptr && trip_ptr && angle && idx_kj64 && idx_ji64,
+                "triplet_geometry_any_degree: null pointer");
+  DIG3D_REQUIRE(use_torsion >= 0 && use_torsion <= 2, "triplet_geometry_any_degree: use_torsion=%d", use_torsion);
+  DIG3D_REQUIRE(!use_torsion || torsion, "triplet_geometry_any_degree: torsion requested without output buffer");
+  DIG3D_REQUIRE(use_torsion != 2 || (nn1 && nn2), "triplet_geometry_any_degree: the kNN torsion needs nn1 and nn2");
+  DIG3D_REQUIRE(n_heavy >= 0 && n_heavy <= n_edges && n_edges < (1ll << 31),
+                "triplet_geometry_any_degree: %lld heavy edges of %lld", (long long)n_heavy, (long long)n_edges);
+  DIG3D_REQUIRE(n_heavy == 0 || n_heavy == n_edges || heavy_ws,
+                "triplet_geometry_any_degree: the heavy-edge list needs a workspace");
+  if (n_edges == 0) return DIG3D_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (n_heavy < n_edges) {
+    triplet_geometry_kernel<<<ceil_div(n_edges, GEO_WARPS), GEO_WARPS * 32, 0, st>>>(
+        pos, src, dst, row_ptr, trip_ptr, (int)n_edges, GEO_MAXDEG, use_torsion, angle, torsion, nullptr, nullptr,
+        idx_kj64, idx_ji64, nn1, nn2);
+    DIG3D_LAUNCH_CHECK();
+  }
+  if (n_heavy == 0) return DIG3D_OK;
+  const int32_t* heavy = nullptr;                           // n_heavy == n_edges: every edge, no list needed
+  if (n_heavy < n_edges) {
+    cudaMemsetAsync(heavy_ws, 0, sizeof(int32_t), st);
+    heavy_edges_kernel<<<ceil_div(n_edges, 256), 256, 0, st>>>(src, row_ptr, (int)n_edges, GEO_MAXDEG, heavy_ws);
+    DIG3D_LAUNCH_CHECK();
+    heavy = heavy_ws + 1;
+  }
+  triplet_geometry_heavy_kernel<<<(unsigned)n_heavy, HEAVY_THREADS, 0, st>>>(
+      pos, src, dst, row_ptr, trip_ptr, heavy, use_torsion, angle, torsion, idx_kj64, idx_ji64, nn1, nn2);
   DIG3D_LAUNCH_CHECK();
   return DIG3D_OK;
 }
@@ -572,19 +723,20 @@ int dig3d_triplet_geometry_knn(const float* pos, const int32_t* src, const int32
                 "triplet_geometry_knn: null pointer");
   if (n_edges == 0) return DIG3D_OK;
   triplet_geometry_kernel<<<ceil_div(n_edges, GEO_WARPS), GEO_WARPS * 32, 0, (cudaStream_t)stream>>>(
-      pos, src, dst, row_ptr, trip_ptr, (int)n_edges, 2, angle, torsion, nullptr, nullptr, idx_kj64, idx_ji64, nn1,
-      nn2);
+      pos, src, dst, row_ptr, trip_ptr, (int)n_edges, GEO_MAXDEG, 2, angle, torsion, nullptr, nullptr, idx_kj64,
+      idx_ji64, nn1, nn2);
   DIG3D_LAUNCH_CHECK();
   return DIG3D_OK;
 }
 
 int dig3d_edges_to_csr(const float* pos, const int64_t* edge_index, int64_t n_edges, int64_t n_nodes, int32_t* src,
                        int32_t* dst, int32_t* row_ptr, int32_t* cnt_ws, int32_t* trip_ptr, float* dist,
-                       int32_t* flags /*[4]: [0] unsorted/out-of-range, [2] E, [3] T*/, void* stream) {
+                       int32_t* flags /*[6]: see include/dig3d.h*/, void* stream) {
   DIG3D_REQUIRE(pos && edge_index && src && dst && row_ptr && cnt_ws && trip_ptr && dist && flags,
                 "edges_to_csr: null pointer");
+  DIG3D_REQUIRE(((uintptr_t)flags & 7) == 0, "edges_to_csr: flags must be 8-byte aligned");
   cudaStream_t st = (cudaStream_t)stream;
-  cudaMemsetAsync(flags, 0, 4 * sizeof(int32_t), st);
+  cudaMemsetAsync(flags, 0, 6 * sizeof(int32_t), st);
   if (n_edges) {
     edges_prepare_kernel<<<ceil_div(n_edges, 256), 256, 0, st>>>(edge_index, n_edges, (int)n_nodes, src, dst, flags);
     DIG3D_LAUNCH_CHECK();
@@ -592,8 +744,9 @@ int dig3d_edges_to_csr(const float* pos, const int64_t* edge_index, int64_t n_ed
   csr_from_sorted_kernel<<<ceil_div(n_nodes + 1, 256), 256, 0, st>>>(dst, (int)n_edges, (int)n_nodes, row_ptr);
   DIG3D_LAUNCH_CHECK();
   if (n_edges) {
-    edge_triplet_count_kernel<<<ceil_div(n_edges, 256), 256, 0, st>>>(pos, src, dst, row_ptr, (int)n_edges,
-                                                                    GEO_MAXDEG, cnt_ws, dist, flags);
+    edge_triplet_count_kernel<<<ceil_div(n_edges, COUNT_THREADS), COUNT_THREADS, 0, st>>>(
+        pos, src, dst, row_ptr, (int)n_edges, GEO_MAXDEG, cnt_ws, dist, flags,
+        reinterpret_cast<unsigned long long*>(flags + 4));
     DIG3D_LAUNCH_CHECK();
   }
   scan_counts_kernel<<<1, 1024, 0, st>>>(cnt_ws, cnt_ws, nullptr, (int)n_edges, trip_ptr, cnt_ws + n_edges + 1, nullptr,

@@ -130,6 +130,96 @@ def build_graph(pos, batch, cutoff, num_graphs=None, max_num_neighbors=32, want_
     return g
 
 
+def radius_graph_dense(pos, batch, cutoff, num_graphs=None, max_num_neighbors=32, want_edge_index=True, z=None,
+                       z_rows=0):
+    """radius_graph(pos, r=cutoff, batch, max_num_neighbors) for ANY max_num_neighbors >= 0 (csrc/graph_dense.cu):
+    the edges of `build_graph` -- same hits, same (target, source) order -- without its [N, max_num_neighbors + 1]
+    neighbour table and its cap of 63.  Returns a Graph3D with src, dst, row_ptr, graph_ptr, batch, n_nodes, n_edges,
+    n_graphs and, if asked, edge_index; no triplet offsets, distances or out-edge lists.
+
+    One host synchronisation (the edge total, with the index validation of `build_graph`).  Raises ValueError for
+    invalid batch ids / atomic numbers and for 2^31 edges or more, before any edge is written."""
+    if pos.dim() != 2 or pos.size(1) != 3:
+        raise ValueError(f"pos must be [N, 3], got {tuple(pos.shape)}")
+    m = int(max_num_neighbors)
+    if m < 0:
+        raise ValueError(f"max_num_neighbors must be >= 0, got {m}")
+    n = pos.size(0)
+    if batch is None:
+        batch = torch.zeros(n, dtype=torch.long, device=pos.device)
+    if batch.shape != (n,):
+        raise ValueError("batch must be [N]")
+    if z is not None and z.shape != (n,):
+        raise ValueError("z must be [N]")
+    pos = pos.detach()
+    dev = pos.device
+    st = _stream()
+    if num_graphs is None:
+        num_graphs = int(batch[-1].item()) + 1 if n else 0
+    g = Graph3D()
+    g.n_nodes, g.n_graphs, g.batch = n, int(num_graphs), batch
+    info = torch.zeros(2, dtype=torch.int64, device=dev)
+    if n:
+        g.graph_ptr = torch.empty(g.n_graphs + 1, dtype=torch.int32, device=dev)
+        call("dig3d_graph_ptr", _p(batch, torch.int64, "batch"), n, g.n_graphs, _p(g.graph_ptr), st)
+        call("dig3d_validate_nodes", _p(batch), _p(z, torch.int64, "z"), n, g.n_graphs, int(z_rows),
+             ctypes.c_void_p(info.data_ptr() + 8), st)
+    else:                                                  # no nodes: every graph is empty
+        g.graph_ptr = torch.zeros(g.n_graphs + 1, dtype=torch.int32, device=dev)
+    counts = torch.empty(max(n, 1), dtype=torch.int32, device=dev)
+    g.row_ptr = torch.empty(n + 1, dtype=torch.int32, device=dev)
+    info_host = (ctypes.c_int64 * 2)()
+    try:
+        call("dig3d_radius_graph_dense_count", _p(pos, torch.float32, "pos"), _p(batch), _p(g.graph_ptr), n,
+             g.n_graphs, float(cutoff), m, _p(counts), _p(g.row_ptr), _p(info), ctypes.byref(info_host), st)
+        rejected = None
+    except _lib.Dig3dError as exc:
+        if exc.rc != -1:                                   # DIG3D_EINVAL: the input was rejected
+            raise
+        rejected = exc
+    flags = int(info_host[1])
+    if flags:
+        what = [msg for bit, msg in ((1, f"batch ids outside [0, {g.n_graphs})"), (2, "batch is not sorted ascending"),
+                                     (4, f"atomic numbers outside the {z_rows}-row embedding table")) if flags & bit]
+        raise ValueError("invalid node indices: " + "; ".join(what))
+    if rejected is not None:
+        raise ValueError(str(rejected)) from None
+    e = g.n_edges = int(info_host[0])
+    g.src = torch.empty(max(e, 1), dtype=torch.int32, device=dev)[:e]
+    g.dst = torch.empty(max(e, 1), dtype=torch.int32, device=dev)[:e]
+    g.edge_index = torch.empty(2, e, dtype=torch.int64, device=dev) if want_edge_index else None
+    call("dig3d_radius_graph_dense_fill", _p(pos), _p(batch), _p(g.graph_ptr), n, g.n_graphs, float(cutoff), m,
+         _p(g.row_ptr), e, _p(g.edge_index) if want_edge_index else None, _p(g.src), _p(g.dst), st)
+    return g
+
+
+def check_int32_total(total, what):
+    """Kernels index edges and triplets with int32: a total of 2^31 or more is refused before it is allocated."""
+    if int(total) >= 1 << 31:
+        raise ValueError(f"{int(total)} {what}: the kernels index them with int32, the limit is 2^31 - 1")
+
+
+def triplet_geometry_any_degree(g, pos, use_torsion, n_heavy, nn=None):
+    """xyz_to_dat's angle / torsion / idx_kj64 / idx_ji64 at any in-degree (dig3d_triplet_geometry_any_degree).
+    use_torsion: 0, 1 (min over all candidates) or 2 (G-SphereNet's single reference atom; nn = [2, N] nearest
+    neighbours from dig3d_knn2).  n_heavy: the edges whose source has in-degree > 64 (flags[1] of
+    dig3d_edges_to_csr); n_heavy == n_edges runs every edge on the heavy-edge kernel."""
+    dev = pos.device
+    t = g.n_triplets
+    g.angle = torch.empty(t, dtype=torch.float32, device=dev)
+    g.torsion = torch.empty(t, dtype=torch.float32, device=dev) if use_torsion else None
+    g.idx_kj64 = torch.empty(t, dtype=torch.int64, device=dev)
+    g.idx_ji64 = torch.empty(t, dtype=torch.int64, device=dev)
+    e = g.n_edges
+    if e and t:
+        ws = torch.empty(n_heavy + 1, dtype=torch.int32, device=dev) if 0 < n_heavy < e else None
+        call("dig3d_triplet_geometry_any_degree", _p(pos.detach(), torch.float32, "pos"), _p(g.src), _p(g.dst),
+             _p(g.row_ptr), _p(g.trip_ptr), e, int(n_heavy), int(use_torsion),
+             _p(nn[0]) if nn is not None else None, _p(nn[1]) if nn is not None else None, _p(ws), _p(g.angle),
+             _p(g.torsion) if use_torsion else None, _p(g.idx_kj64), _p(g.idx_ji64), _stream())
+    return g
+
+
 def _out_lists(g):
     """(out_ptr, out_list, pos_in) device addresses of a graph's out-edge lists, or three NULLs."""
     if getattr(g, "out_ptr", None) is None or g.out_list is None or g.pos_in is None:

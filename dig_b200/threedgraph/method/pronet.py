@@ -102,7 +102,8 @@ class InteractionBlock(nn.Module):
 
 class ProNet(nn.Module):
     r"""Drop-in for dig.threedgraph.method.ProNet (reference pronet.py:256-342; same arguments and defaults).
-    num_radial / num_spherical are fixed to the generated basis (6, 2); dropout must be 0 and the two noise flags False."""
+    num_radial / num_spherical are fixed to the generated basis (6, 2); dropout must be 0 and the two noise flags False.
+    Any max_num_neighbors >= 1: from 64 on, the radius graph is built without the capped builder's neighbour table."""
 
     def __init__(self, level='aminoacid', num_blocks=4, hidden_channels=128, out_channels=1, mid_emb=64, num_radial=6,
                  num_spherical=2, cutoff=10.0, max_num_neighbors=32, int_emb_layers=3, out_layers=2, num_pos_emb=16,
@@ -116,8 +117,10 @@ class ProNet(nn.Module):
         if dropout or data_augment_eachlayer or euler_noise:
             raise NotImplementedError("dropout / data_augment_eachlayer / euler_noise (training-time randomness) are "
                                       "not implemented by the kernels")
-        if num_pos_emb % 2 or not (1 <= max_num_neighbors <= 63):
-            raise NotImplementedError("num_pos_emb must be even and max_num_neighbors in [1, 63]")
+        if num_pos_emb % 2:
+            raise NotImplementedError("num_pos_emb must be even")
+        if max_num_neighbors < 1:
+            raise NotImplementedError(f"max_num_neighbors must be >= 1, got {max_num_neighbors}")
         self.cutoff, self.max_num_neighbors, self.num_pos_emb = cutoff, max_num_neighbors, num_pos_emb
         self.data_augment_eachlayer, self.euler_noise, self.level = data_augment_eachlayer, euler_noise, level
         self.act = swish
@@ -138,9 +141,10 @@ class ProNet(nn.Module):
         z = torch.squeeze(batch_data.x.long())
         pos, batch = batch_data.coords_ca, batch_data.batch
         require_cuda(pos, "ProNet.forward")
-        g = ops.build_graph(pos, batch, self.cutoff, num_graphs=getattr(batch_data, "num_graphs", None),
-                            max_num_neighbors=self.max_num_neighbors, want_edge_index=False,
-                            z=z.reshape(-1), z_rows=num_aa_type)
+        # up to 63 neighbours: the capped builder; beyond, the builder without a neighbour table (same edges)
+        build = ops.build_graph if self.max_num_neighbors <= 63 else ops.radius_graph_dense
+        g = build(pos, batch, self.cutoff, num_graphs=getattr(batch_data, "num_graphs", None),
+                  max_num_neighbors=self.max_num_neighbors, want_edge_index=False, z=z.reshape(-1), z_rows=num_aa_type)
         lvl = 0 if self.level == 'aminoacid' else 1
         f0, f1, pe, _, _ = ops.pronet_edge_features(
             g, pos, batch_data.coords_n if lvl else None, batch_data.coords_c if lvl else None, lvl, self.cutoff,

@@ -12,11 +12,20 @@ from ...ops import _p, _stream, call
 
 
 def radius_graph(x, r, batch=None, loop=False, max_num_neighbors=32, flow='source_to_target', num_workers=1):
-    """edge_index [2, E] int64 = (source j, target i), sorted by (i, j); torch_cluster CUDA semantics."""
+    """edge_index [2, E] int64 = (source j, target i), sorted by (i, j); torch_cluster CUDA semantics, any
+    max_num_neighbors."""
     if loop or flow != 'source_to_target':
         raise NotImplementedError("radius_graph: only loop=False, flow='source_to_target' (the reference's use)")
-    g = ops.build_graph(x, batch, r, max_num_neighbors=max_num_neighbors)
+    if int(max_num_neighbors) <= 63:
+        g = ops.build_graph(x, batch, r, max_num_neighbors=max_num_neighbors)
+    else:                                           # beyond the capped builder's neighbour table
+        g = ops.radius_graph_dense(x, batch, r, max_num_neighbors=max_num_neighbors)
     return g.edge_index
+
+
+# Tests only: run every edge on the heavy-edge geometry kernel, which otherwise takes the edges whose source has
+# in-degree > 64, to hold it bit for bit against the warp-per-edge kernel on the graphs both can run.
+_HEAVY_KERNEL_FOR_ALL_EDGES = False
 
 
 def _xyz_to_dat_sorted(pos, ei, n, use_torsion, knn_batch=None):
@@ -32,19 +41,18 @@ def _xyz_to_dat_sorted(pos, ei, n, use_torsion, knn_batch=None):
     g.trip_ptr = torch.empty(e + 1, dtype=torch.int32, device=dev)
     g.dist = torch.empty(max(e, 1), dtype=torch.float32, device=dev)[:e]
     ws = torch.empty(2 * e + 2, dtype=torch.int32, device=dev)
-    flags = torch.empty(4, dtype=torch.int32, device=dev)
+    flags = torch.empty(6, dtype=torch.int32, device=dev)
     call("dig3d_edges_to_csr", _p(pos.detach(), torch.float32, "pos"), _p(ei, torch.int64, "edge_index"), e, n,
          _p(g.src), _p(g.dst), _p(g.row_ptr), _p(ws), _p(g.trip_ptr), _p(g.dist), _p(flags), _stream())
     fl = flags.tolist()
     if fl[0] & 1:
         return None
-    if fl[0] & 2:
-        raise NotImplementedError("xyz_to_dat: in-degree above 64 is not supported by the geometry kernel")
-    g.n_triplets = int(fl[3])
+    t = (fl[4] & 0xFFFFFFFF) | (fl[5] << 32)                           # the int64 triplet total
+    ops.check_int32_total(t, "triplets")
+    g.n_triplets = t
+    n_heavy = e if _HEAVY_KERNEL_FOR_ALL_EDGES else fl[1]
     if knn_batch is None:
-        ops.triplet_geometry(g, pos, use_torsion=use_torsion, want_idx=False, want_idx64=True)
-        return g
-    t = g.n_triplets
+        return ops.triplet_geometry_any_degree(g, pos, int(bool(use_torsion)), n_heavy)
     n_graphs = int(knn_batch[-1].item()) + 1 if n else 0
     graph_ptr = torch.empty(n_graphs + 1, dtype=torch.int32, device=dev)
     call("dig3d_graph_ptr", _p(knn_batch, torch.int64, "batch"), n, n_graphs, _p(graph_ptr), _stream())
@@ -53,15 +61,7 @@ def _xyz_to_dat_sorted(pos, ei, n, use_torsion, knn_batch=None):
          _p(nn[1]), _stream())
     if n and int(nn.min()) < 0:
         raise ValueError("xyztodat: every graph needs at least three atoms (nearest and second-nearest neighbour)")
-    g.angle = torch.empty(t, dtype=torch.float32, device=dev)
-    g.torsion = torch.empty(t, dtype=torch.float32, device=dev)
-    g.idx_kj64 = torch.empty(t, dtype=torch.int64, device=dev)
-    g.idx_ji64 = torch.empty(t, dtype=torch.int64, device=dev)
-    if e and t:
-        call("dig3d_triplet_geometry_knn", _p(pos.detach(), torch.float32, "pos"), _p(g.src), _p(g.dst), _p(g.row_ptr),
-             _p(g.trip_ptr), e, _p(nn[0]), _p(nn[1]), _p(g.angle), _p(g.torsion), _p(g.idx_kj64), _p(g.idx_ji64),
-             _stream())
-    return g
+    return ops.triplet_geometry_any_degree(g, pos, 2, n_heavy, nn)
 
 
 def xyz_to_dat(pos, edge_index, num_nodes, use_torsion=False, _knn_batch=None):
@@ -72,11 +72,16 @@ def xyz_to_dat(pos, edge_index, num_nodes, use_torsion=False, _knn_batch=None):
     order is handled like the reference's SparseTensor does: the edges are sorted (stable, by target then source), the
     kernels run on the sorted list, and the results are mapped back: `dist` in the caller's edge order, triplets grouped
     by the caller's edge order with k ascending inside a group, `idx_kj` / `idx_ji` holding the caller's edge ids (the
-    re-ordering is index plumbing with torch; all geometry is computed by the kernels)."""
+    re-ordering is index plumbing with torch; all geometry is computed by the kernels).
+
+    Any in-degree: a node of in-degree d and out-degree d' has about d * d' triplets, and the torsion takes the min
+    over d candidates per triplet (the sets the reference materialises).  Raises ValueError for 2^31 edges or
+    triplets or more (int32 indices), before the triplet buffers are allocated."""
     if edge_index.dim() != 2 or edge_index.size(0) != 2:
         raise ValueError("edge_index must be [2, E]")
     e = edge_index.size(1)
     n = int(num_nodes)
+    ops.check_int32_total(e, "edges")
     ei = edge_index.contiguous()
     j, i = ei[0], ei[1]
     if e and (int(ei.min()) < 0 or int(ei.max()) >= n):

@@ -8,7 +8,7 @@
  * Conventions (all entry points):
  *   - plain pointers + sizes, no torch types; all pointers are DEVICE pointers unless named *_host;
  *   - caller owns every buffer (no allocation, no synchronisation inside except the one read-back of
- *     dig3d_radius_graph_pbc_count; the only process-wide state are the
+ *     dig3d_radius_graph_pbc_count and dig3d_radius_graph_dense_count; the only process-wide state are the
  *     experiment switches dig3d_tc_set_fast_swish / dig3d_tc_trace / dig3d_linear_set_config and a thread-local
  *     error string);
  *   - `stream` is a cudaStream_t passed as void*;
@@ -57,6 +57,19 @@ int dig3d_graph_ptr(const int64_t* batch, int64_t n_nodes, int64_t n_graphs, int
 int dig3d_radius_neighbors(const float* pos, const int64_t* batch, const int32_t* ptr, int64_t n_nodes,
                            int64_t n_graphs, double cutoff, int32_t cap, int32_t* nbr, int32_t* deg, void* stream);
 
+/* Radius graph for any max_num_neighbors, without the nbr[N][cap] table (csrc/graph_dense.cu): the semantics of
+ * dig3d_radius_neighbors + dig3d_edge_fill at cap = max_num_neighbors + 1, in two passes.
+ * _count: counts[n_nodes] (workspace), row_ptr[n_nodes+1]; info [2] int64 on the device, zeroed by the caller, whose
+ * info[1] may carry dig3d_validate_nodes' flags (int32 at byte offset 8).  The stream is synchronised once and
+ * info_host[0] = E, info_host[1] = those flags; E >= 2^31 returns DIG3D_EINVAL (info_host still written).
+ * _fill: src / dst [E] int32 and edge_index [2,E] int64 (nullable), sorted by (target, source). */
+int dig3d_radius_graph_dense_count(const float* pos, const int64_t* batch, const int32_t* graph_ptr, int64_t n_nodes,
+                                   int64_t n_graphs, double cutoff, int64_t max_num_neighbors, int32_t* counts,
+                                   int32_t* row_ptr, int64_t* info, int64_t* info_host, void* stream);
+int dig3d_radius_graph_dense_fill(const float* pos, const int64_t* batch, const int32_t* graph_ptr, int64_t n_nodes,
+                                  int64_t n_graphs, double cutoff, int64_t max_num_neighbors, const int32_t* row_ptr,
+                                  int64_t n_edges, int64_t* edge_index, int32_t* src, int32_t* dst, void* stream);
+
 /* Index validation (the reference's nn.Embedding / scatter raise a device-side assert for these; e.g.
  * spherenet.py:86 `self.emb(x)`): ORs into *flags (caller-zeroed) bit 0 = a batch id outside [0, n_graphs),
  * bit 1 = batch not sorted ascending, bit 2 = an atomic number outside [0, z_rows) (z nullable). */
@@ -101,8 +114,10 @@ int dig3d_edge_fill_out(const float* pos, const int32_t* nbr, const int32_t* deg
 
 /* CSR / triplet offsets / distances for a CALLER-SUPPLIED edge_index [2,E] int64 sorted by (target, source)
  * (the entry of xyz_to_dat(pos, edge_index, num_nodes, ...), utils/geometric_computing.py:12).
- * cnt_ws: [2E+2] int32 workspace; flags[0] != 0 afterwards => edge_index unsorted or out of range;
- * flags[3] = number of triplets. */
+ * cnt_ws: [2E+2] int32 workspace; flags: [6] int32, 8-byte aligned, written afterwards as
+ * flags[0] != 0 => edge_index unsorted or out of range; flags[1] = heavy edges (source in-degree > 64);
+ * flags[2] = E; flags[3] = number of triplets T as int32; flags[4..5] = T as int64 (T >= 2^31 wraps flags[3] and
+ * trip_ptr: the caller must refuse it before any triplet kernel runs). */
 int dig3d_edges_to_csr(const float* pos, const int64_t* edge_index, int64_t n_edges, int64_t n_nodes, int32_t* src,
                        int32_t* dst, int32_t* row_ptr, int32_t* cnt_ws, int32_t* trip_ptr, float* dist,
                        int32_t* flags, void* stream);
@@ -117,6 +132,18 @@ int dig3d_triplet_geometry(const float* pos, const int32_t* src, const int32_t* 
                            const int32_t* trip_ptr, int64_t n_edges, int32_t use_torsion, float* angle,
                            float* torsion, int32_t* idx_kj, int32_t* idx_ji, int64_t* idx_kj64,
                            int64_t* idx_ji64, void* stream);
+
+/* dig3d_triplet_geometry (use_torsion 0 / 1) and dig3d_triplet_geometry_knn (use_torsion 2, nn1 / nn2 of dig3d_knn2)
+ * at ANY in-degree, with the int64 indices.  The edges whose source has in-degree <= 64 run the warp-per-edge kernel of
+ * those entry points; the n_heavy others (flags[1] of dig3d_edges_to_csr) run a CTA-per-edge kernel that folds the
+ * torsion min across shared-memory tiles of planes.  Both call the same per-triplet device code, so a triplet's bits
+ * do not depend on which kernel computed it.  0 < n_heavy < n_edges: the heavy edges are compacted on the device into
+ * heavy_ws [n_heavy + 1]; n_heavy == n_edges runs every edge on the heavy kernel (no list, heavy_ws unused). */
+int dig3d_triplet_geometry_any_degree(const float* pos, const int32_t* src, const int32_t* dst,
+                                      const int32_t* row_ptr, const int32_t* trip_ptr, int64_t n_edges,
+                                      int64_t n_heavy, int32_t use_torsion, const int32_t* nn1, const int32_t* nn2,
+                                      int32_t* heavy_ws, float* angle, float* torsion, int64_t* idx_kj64,
+                                      int64_t* idx_ji64, void* stream);
 
 /* ------------------------------------------------------------------ basis
  * dist_emb / angle_emb / torsion_emb      spherenet/features.py:167-263, dimenetpp/features.py:149-220
