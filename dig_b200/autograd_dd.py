@@ -70,7 +70,10 @@ class _ColSum(torch.autograd.Function):
     def forward(ctx, dy):
         dy = _c(dy)
         ctx.rows = dy.size(0)
-        ptr = torch.tensor([0, dy.size(0)], dtype=torch.int32, device=dy.device)
+        # [0, rows] written by fills on the device: a tensor built from a host list (or an item assignment) is a
+        # synchronous copy, one host wait per bias of every force evaluation
+        ptr = torch.zeros(2, dtype=torch.int32, device=dy.device)
+        ptr[1:].fill_(dy.size(0))
         return ops.segment_sum(dy, ptr).view(-1)
 
     @staticmethod

@@ -156,35 +156,43 @@ class run():
         step, SURVEY.md Appendix C.7); values are identical."""
         model.eval()
         preds, targets, preds_force, targets_force = [], [], [], []
-        if not energy_and_force and torch.device(device).type == "cuda":
+        if torch.device(device).type == "cuda":
             # several batches in flight (dig_b200/pipeline.py): the copy, graph kernels and count readback of batch n+1
-            # overlap the interaction blocks of batch n; values identical to the plain loop below
-            pipe = InferencePipeline(model, device)
+            # overlap the interaction blocks (with forces, also the backward) of batch n; values identical to the plain
+            # loop below
+            pipe = InferencePipeline(model, device, forces=energy_and_force)
 
             def feed():
                 for batch_data in tqdm(data_loader):
                     targets.append(batch_data.y.unsqueeze(1))
+                    if energy_and_force:
+                        targets_force.append(batch_data.force)
                     yield batch_data
-            for out in pipe.map(feed()):
+            for res in pipe.map(feed()):
+                out, force = res if energy_and_force else (res, None)
                 preds.append(out.clone())
-            input_dict = {"y_true": torch.cat(targets, dim=0).to(device), "y_pred": torch.cat(preds, dim=0).to(device)}
-            return evaluation.eval(input_dict)['mae']
-        for step, batch_data in enumerate(tqdm(data_loader)):
-            batch_data = batch_data.to(device)
-            if energy_and_force:
-                out = model(batch_data)
-                force = -grad(outputs=out, inputs=batch_data.pos, grad_outputs=torch.ones_like(out),
-                              create_graph=True, retain_graph=True)[0]
-                preds_force.append(force.detach_())
-                targets_force.append(batch_data.force)
-            else:
-                with torch.no_grad():
+                if energy_and_force:
+                    preds_force.append(force.clone())
+        else:
+            for step, batch_data in enumerate(tqdm(data_loader)):
+                batch_data = batch_data.to(device)
+                if energy_and_force:
                     out = model(batch_data)
-            preds.append(out.detach())
-            targets.append(batch_data.y.unsqueeze(1))
-        input_dict = {"y_true": torch.cat(targets, dim=0), "y_pred": torch.cat(preds, dim=0)}
+                    force = -grad(outputs=out, inputs=batch_data.pos, grad_outputs=torch.ones_like(out),
+                                  create_graph=True, retain_graph=True)[0]
+                    preds_force.append(force.detach_())
+                    targets_force.append(batch_data.force)
+                else:
+                    with torch.no_grad():
+                        out = model(batch_data)
+                preds.append(out.detach())
+                targets.append(batch_data.y.unsqueeze(1))
+
+        def cat(ts):                     # the pipeline's lists hold host tensors: the MAE is reduced on `device` either way
+            return torch.cat(ts, dim=0).to(device)
+        input_dict = {"y_true": cat(targets), "y_pred": cat(preds)}
         if energy_and_force:
-            input_dict_force = {"y_true": torch.cat(targets_force, dim=0), "y_pred": torch.cat(preds_force, dim=0)}
+            input_dict_force = {"y_true": cat(targets_force), "y_pred": cat(preds_force)}
             energy_mae = evaluation.eval(input_dict)['mae']
             force_mae = evaluation.eval(input_dict_force)['mae']
             print({'Energy MAE': energy_mae, 'Force MAE': force_mae})
