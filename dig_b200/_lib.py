@@ -125,6 +125,8 @@ SIGNATURES = {
                            POINTER(SchnetBlockWeights), P, P, P, P],
     "dig3d_schnet_readout": [P, c_int64, c_int32, P, P, P, P, c_int32, P, P],
     "dig3d_comenet_geometry": [P, P, P, P, P, P, P, c_int64, c_int64, c_double, P, P, P, P, P],
+    "dig3d_comenet_features_bwd": [P, P, P, P, P, P, P, P, c_int64, c_int64, c_double, P, P, P, P, P],
+    "dig3d_comenet_features_tangent": [P, P, P, P, P, c_int64, c_int64, c_double, P, P, P, P],
     "dig3d_comenet_embed": [P, P, c_int64, P, P],
     "dig3d_pbc_edge_vectors": [P, P, P, P, P, c_int64, P, P, P],
     "dig3d_comenet_geometry_edges": [P, P, P, P, P, c_int64, c_int64, c_double, P, P, P, P, P, P],
@@ -152,6 +154,8 @@ SIGNATURES = {
     "dig3d_sphere_triplet_gather_bwd": [P, P, P, P, P, P, P, P, c_int64, P, P, P, P, P, P, P, P],
     "dig3d_graphnorm": [P, P, c_int64, c_int32, P, P, P, c_double, P, P, P, P],
     "dig3d_graphnorm_bwd": [P, P, P, c_int64, c_int32, P, P, P, P, P, P, P, P, P],
+    "dig3d_graphnorm_tangent": [P, P, P, c_int64, c_int32, P, P, P, P, P, P],
+    "dig3d_graphnorm_tangent_bwd": [P, P, P, P, c_int64, c_int32, P, P, P, P, P, P, P, P, P],
     "dig3d_edge_dist_bwd": [P, P, P, P, P, c_int64, P, P],
     "dig3d_triplet_angle_bwd": [P, P, P, P, P, P, c_int64, P, P],
     "dig3d_edge_basis_bwd": [P, c_int64, c_double, c_int32, P, c_int32, c_int32, P, P, P, P],

@@ -555,6 +555,35 @@ def geometry(pos, g, n_out):
     return _Geometry.apply(pos, g, n_out)
 
 
+class _ComenetFeatures(torch.autograd.Function):
+    """ComENet's feature1 [E,12] / feature2 [E,6] as functions of pos: the values ops.comenet_geometry computed (bit for
+    bit the inference features), backward = ops.comenet_features_bwd (csrc/comenet.cu, deterministic)."""
+
+    @staticmethod
+    def forward(ctx, pos, g, cutoff, f1, f2):
+        ctx.g, ctx.cutoff = g, cutoff
+        ctx.save_for_backward(pos)
+        ctx.set_materialize_grads(False)
+        return f1.detach(), f2.detach()
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, df1, df2):
+        (pos,) = ctx.saved_tensors
+        g = ctx.g
+        if (df1 is None and df2 is None) or not ctx.needs_input_grad[0]:
+            return (None,) * 5
+        e = g.n_edges
+        df1 = torch.zeros(e, 12, dtype=torch.float32, device=pos.device) if df1 is None else _c(df1)
+        df2 = torch.zeros(e, 6, dtype=torch.float32, device=pos.device) if df2 is None else _c(df2)
+        return ops.comenet_features_bwd(g, pos, ctx.cutoff, df1, df2), None, None, None, None
+
+
+def comenet_features(pos, g, cutoff, f1, f2):
+    """(f1, f2) of ops.comenet_geometry(g, pos, cutoff), differentiable in pos."""
+    return _ComenetFeatures.apply(pos, g, cutoff, f1, f2)
+
+
 def schnet_edge_features(dist, offset, coeff, cutoff):
     return _SchnetEdgeFeatures.apply(dist, offset, coeff, cutoff)
 

@@ -1,4 +1,4 @@
-"""Training ON forces for the DimeNet family (reference run.py:110-123) without a reverse-over-reverse pass.
+"""Training ON forces for the DimeNet family and ComENet (reference run.py:110-123) without a reverse-over-reverse pass.
 
 The reference takes `force = -grad(out, pos, create_graph=True)` and backpropagates `e_loss + p * f_loss`; torch.autograd
 then differentiates the first backward a second time.  For a loss L_F(force) the parameter gradient is
@@ -16,6 +16,7 @@ that carries a grad_fn (`_ForceOp`), and `loss.backward()` reaches the parameter
   dual primitives       (value, tangent) pairs over the first-order Functions of dig_b200.autograd; a tangent of None is
                         an exact zero (embeddings, biases)
   _EdgeBasisTangent     d(rbf0)/d(dist) * dist_dot, differentiable in dist_emb.freq
+  graphnorm_dual        GraphNorm and its tangent (ComENet), differentiable in h, h_dot, weight and mean_scale
   energy_with_force     wraps a model's differentiable forward + dual forward
 """
 import torch
@@ -68,6 +69,44 @@ def gather_rows_dual(x, xd, idx):
 
 def segment_sum_dual(x, xd, ptr, idx):
     return ag.segment_sum(x, ptr, idx), (None if xd is None else ag.segment_sum(xd, ptr, idx))
+
+
+class _GraphNormDual(torch.autograd.Function):
+    """(GraphNorm(h), its tangent along h_dot): one forward (ops.graphnorm, whose shift / std the tangent kernel reuses)
+    and one tangent kernel; backward sums GraphNorm's backward and the tangent's reverse mode (csrc/train_ops.cu)."""
+
+    @staticmethod
+    def forward(ctx, h, hd, weight, bias, mean_scale, graph_ptr, eps):
+        h, hd = _c(h), _c(hd)
+        w, ms = weight.detach(), mean_scale.detach()
+        y, shift, std = ops.graphnorm(h, graph_ptr, w, bias.detach(), ms, eps)
+        yd = ops.graphnorm_tangent(h, hd, graph_ptr, w, ms, shift, std)
+        ctx.save_for_backward(h, hd, weight, mean_scale, shift, std, graph_ptr)
+        ctx.set_materialize_grads(False)
+        return y, yd
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dy, dyd):
+        h, hd, weight, mean_scale, shift, std, graph_ptr = ctx.saved_tensors
+        w, ms = weight.detach(), mean_scale.detach()
+        dh = dhd = dw = db = dms = None
+        if dy is not None:
+            dh, dw, db, dms = ops.graphnorm_bwd(h, _c(dy), graph_ptr, w, ms, shift, std)
+        if dyd is not None:
+            dh2, dhd, dw2, dms2 = ops.graphnorm_tangent_bwd(h, hd, _c(dyd), graph_ptr, w, ms, shift, std)
+            if dh is None:
+                dh, dw, dms = dh2, dw2, dms2
+            else:
+                dh, dw, dms = ops.ewise(dh, dh2, 1), ops.ewise(dw, dw2, 1), ops.ewise(dms, dms2, 1)
+        return dh, dhd, dw, db, dms, None, None
+
+
+def graphnorm_dual(h, hd, module, graph_ptr):
+    """GraphNorm holder `module` (weight, bias, mean_scale, eps) applied to h, with the tangent along hd."""
+    if hd is None:
+        return ag.graphnorm(h, module, graph_ptr), None
+    return _GraphNormDual.apply(h, hd, module.weight, module.bias, module.mean_scale, graph_ptr, module.eps)
 
 
 def triplet_gather_dual(x, xd, s, sd, t, td, w_s, w_t, g):

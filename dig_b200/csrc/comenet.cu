@@ -95,6 +95,69 @@ __device__ __forceinline__ f3 edge_vec(const float* __restrict__ pos, const int3
 __device__ __forceinline__ f3 neg3(const f3 a) { return {-a.x, -a.y, -a.z}; }
 __device__ __forceinline__ float fold_pi(float t) { return t < 0.f ? __fadd_rn(t, 3.14159274101257324f) : t; }
 
+// The edges whose vectors the angles of edge e = (j -> i) read (comenet.py:331-354): e itself, i's nearest and
+// second-nearest in-edges, and the reference edges of i and of j.
+struct ComenetEdgeRefs {
+  int e0i, e1i, iref, jref;
+};
+__device__ __forceinline__ ComenetEdgeRefs comenet_edge_refs(const int32_t* __restrict__ src,
+                                                             const int32_t* __restrict__ dst,
+                                                             const int32_t* __restrict__ a0_in,
+                                                             const int32_t* __restrict__ a1_in,
+                                                             const int32_t* __restrict__ a0_out,
+                                                             const int32_t* __restrict__ a1_out, int e) {
+  const int j = src[e], i = dst[e];
+  const int e0i = a0_in[i], e1i = a1_in[i], e0j = a0_out[j], e1j = a1_out[j];
+  const int n0 = src[e0i], n0_j = dst[e0j];
+  return {e0i, e1i, (n0 == j) ? e1i : e0i,                               // comenet.py:344-348
+          (n0_j == i) ? e1j : e0j};                                      // comenet.py:350-354
+}
+
+// theta / phi / tau of one edge with the intermediates their derivatives need.  The forward kernel and the two force
+// kernels below evaluate the angles with this one function, so the derivatives are taken at the bit-equal angles.
+struct ComenetEdgeGeom {
+  f3 pji, in0, in1, iref, jref;      // the five edge vectors
+  f3 pl1, pl2, c2, q1, q2, c3;       // planes; c2 = pl1 x pl2, c3 = q1 x q2
+  float a1, b1;                      // theta = fold(atan2(b1, a1))
+  float d;                           // |pji|
+  float a2, s2;                      // phi = fold(atan2(s2 / d, a2))
+  float a3, s3;                      // tau = fold(atan2(s3 / d, a3))
+  float theta, phi, tau;
+};
+template <bool FROM_VEC>
+__device__ __forceinline__ ComenetEdgeGeom comenet_edge_geom(const float* __restrict__ pos,
+                                                             const int32_t* __restrict__ src,
+                                                             const int32_t* __restrict__ dst, int e,
+                                                             const ComenetEdgeRefs r) {
+  ComenetEdgeGeom G;
+  G.pji = edge_vec<FROM_VEC>(pos, src, dst, e);
+  G.in0 = edge_vec<FROM_VEC>(pos, src, dst, r.e0i);
+  G.in1 = edge_vec<FROM_VEC>(pos, src, dst, r.e1i);
+  G.iref = edge_vec<FROM_VEC>(pos, src, dst, r.iref);
+  G.jref = edge_vec<FROM_VEC>(pos, src, dst, r.jref);
+  const f3 mji = neg3(G.pji);
+  // theta                                                                comenet.py:365-368
+  G.pl1 = cross_aten(mji, G.in0);
+  G.b1 = norm3_aten(G.pl1);
+  G.a1 = sum3_aten(mul3(mji, G.in0));
+  G.theta = fold_pi(atan2f(G.b1, G.a1));
+  // phi                                                                  comenet.py:371-377
+  G.d = norm3_aten(G.pji);
+  G.pl2 = cross_aten(mji, G.in1);
+  G.c2 = cross_aten(G.pl1, G.pl2);
+  G.s2 = sum3_aten(mul3(G.c2, G.pji));
+  G.a2 = sum3_aten(mul3(G.pl1, G.pl2));
+  G.phi = fold_pi(atan2f(__fdiv_rn(G.s2, G.d), G.a2));
+  // tau                                                                  comenet.py:380-385
+  G.q1 = cross_aten(G.pji, G.jref);
+  G.q2 = cross_aten(G.pji, G.iref);
+  G.c3 = cross_aten(G.q1, G.q2);
+  G.s3 = sum3_aten(mul3(G.c3, G.pji));
+  G.a3 = sum3_aten(mul3(G.q1, G.q2));
+  G.tau = fold_pi(atan2f(__fdiv_rn(G.s3, G.d), G.a3));
+  return G;
+}
+
 // theta / phi / tau and the two basis features of every edge
 template <bool FROM_VEC>
 __global__ void comenet_edge_features_kernel(const float* __restrict__ pos, const float* __restrict__ dist,
@@ -105,27 +168,9 @@ __global__ void comenet_edge_features_kernel(const float* __restrict__ pos, cons
                                              float* __restrict__ f2, float* __restrict__ angles) {
   const int e = blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= n_edges) return;
-  const int j = src[e], i = dst[e];
-  const int e0i = a0_in[i], e1i = a1_in[i], e0j = a0_out[j], e1j = a1_out[j];
-  const int n0 = src[e0i], n0_j = dst[e0j];
-  const int idx_iref = (n0 == j) ? e1i : e0i;                            // comenet.py:344-348
-  const int idx_jref = (n0_j == i) ? e1j : e0j;                          // comenet.py:350-354
-  const f3 pos_ji = edge_vec<FROM_VEC>(pos, src, dst, e);
-  const f3 pos_in0 = edge_vec<FROM_VEC>(pos, src, dst, e0i), pos_in1 = edge_vec<FROM_VEC>(pos, src, dst, e1i);
-  const f3 pos_iref = edge_vec<FROM_VEC>(pos, src, dst, idx_iref), pos_jref = edge_vec<FROM_VEC>(pos, src, dst, idx_jref);
-  const f3 mji = neg3(pos_ji);
-  // theta                                                                comenet.py:365-368
-  const f3 pl1 = cross_aten(mji, pos_in0);
-  const float theta = fold_pi(atan2f(norm3_aten(pl1), sum3_aten(mul3(mji, pos_in0))));
-  // phi                                                                  comenet.py:371-377
-  const float dist_ji = norm3_aten(pos_ji);
-  const f3 pl2 = cross_aten(mji, pos_in1);
-  const float phi = fold_pi(atan2f(__fdiv_rn(sum3_aten(mul3(cross_aten(pl1, pl2), pos_ji)), dist_ji),
-                                   sum3_aten(mul3(pl1, pl2))));
-  // tau                                                                  comenet.py:380-385
-  const f3 q1 = cross_aten(pos_ji, pos_jref), q2 = cross_aten(pos_ji, pos_iref);
-  const float tau = fold_pi(atan2f(__fdiv_rn(sum3_aten(mul3(cross_aten(q1, q2), pos_ji)), dist_ji),
-                                   sum3_aten(mul3(q1, q2))));
+  const ComenetEdgeGeom G = comenet_edge_geom<FROM_VEC>(
+      pos, src, dst, e, comenet_edge_refs(src, dst, a0_in, a1_in, a0_out, a1_out, e));
+  const float theta = G.theta, phi = G.phi, tau = G.tau;
   if (angles) { angles[3 * (size_t)e] = theta; angles[3 * (size_t)e + 1] = phi; angles[3 * (size_t)e + 2] = tau; }
   // features                                                             comenet/features.py:289-295,340-348
   const float x = __fmul_rn(dist[e], inv_cutoff);
@@ -141,6 +186,278 @@ __global__ void comenet_edge_features_kernel(const float* __restrict__ pos, cons
   for (int h = 0; h < 4; ++h)
 #pragma unroll
     for (int r = 0; r < 3; ++r) f1[(size_t)e * NF1 + h * 3 + r] = __fmul_rn(rb[(h == 0 ? 0 : 1) * 3 + r], ylm[h]);
+}
+
+// ------------------------------------------------------------------ forces: derivatives of feature1 / feature2 in pos
+// Reverse mode (dig3d_comenet_features_bwd) and forward mode (dig3d_comenet_features_tangent) of the kernel above for
+// the reference's op sequence (comenet.py:297-385, features.py:289-348) with ATen's derivative conventions where a
+// value is singular: the norm of a zero vector and atan2(0, 0) pass no gradient (norm_backward / atan2_backward mask
+// them).  The reference-atom argmins are piecewise constant: no derivative.
+// Aliased cross products.  When two of the vectors a cross product reads are the same edge -- routine: j is i's nearest
+// in-neighbour on one in-edge of every node (pos_in0 == pos_ji), a node with a single in-edge has e0i == e1i, a node
+// with a single out-edge is its own jref -- the product is a x a, identically zero as a function of the positions, and
+// its derivative is exactly zero.  ATen's value is the FMA rounding residue of a x a (SURVEY.md 5.9b), and autograd
+// differentiates the bilinear form instead: two opposite terms of size |g| / |residue| (~1e7 |g| for phi) that only
+// cancel to the last bits of their own size, so torch's forces on such graphs carry O(|g|) noise that changes with
+// the order of its sums (run to run on the CPU with several threads, and with every atomic order on the GPU).  These
+// kernels take the exact derivative: the terms of an aliased product are zero.  Both kernels use the same partial
+// derivatives and the same rule, so one is exactly the transpose of the other.
+__device__ __forceinline__ f3 add3(const f3 a, const f3 b) { return {a.x + b.x, a.y + b.y, a.z + b.z}; }
+__device__ __forceinline__ f3 scale3(const f3 a, float s) { return {a.x * s, a.y * s, a.z * s}; }
+__device__ __forceinline__ f3 axpy3(float s, const f3 a, const f3 b) {
+  return {fmaf(s, a.x, b.x), fmaf(s, a.y, b.y), fmaf(s, a.z, b.z)};
+}
+__device__ __forceinline__ float dot3(const f3 a, const f3 b) { return fmaf(a.x, b.x, fmaf(a.y, b.y, a.z * b.z)); }
+__device__ __forceinline__ f3 cross3(const f3 a, const f3 b) {
+  return {a.y * b.z - a.z * b.y, a.z * b.x - a.x * b.z, a.x * b.y - a.y * b.x};
+}
+// d atan2(y, x) / dy and / dx; both 0 at (0, 0) as in ATen's atan2_backward
+__device__ __forceinline__ void atan2_partials(float y, float x, float& py, float& px) {
+  const float den = fmaf(x, x, y * y);
+  py = den == 0.f ? 0.f : x / den;
+  px = den == 0.f ? 0.f : -y / den;
+}
+
+// d(theta, phi, tau)/d(its inputs) at one edge: the scalar partials shared by both modes
+struct ComenetEdgePartials {
+  float th_b1, th_a1;                // theta
+  float ph_b2, ph_a2;                // phi (b2 = s2 / d)
+  float ta_b3, ta_a3;                // tau (b3 = s3 / d)
+  float inv_b1;                      // 1 / |pl1|, 0 for pl1 == 0 (norm_backward)
+  float inv_d;                       // 1 / d (the features' vecs.norm(): 0 for d == 0)
+  // cross products whose two operands are the same edge vector (derivative exactly zero, see above)
+  bool pl1_0, pl2_0, c2_0, q1_0, q2_0, c3_0;
+};
+__device__ __forceinline__ ComenetEdgePartials comenet_edge_partials(const ComenetEdgeGeom& G,
+                                                                     const ComenetEdgeRefs r, int e) {
+  ComenetEdgePartials P;
+  P.pl1_0 = r.e0i == e;              // pl1 = (-pji) x in0
+  P.pl2_0 = r.e1i == e;              // pl2 = (-pji) x in1
+  P.c2_0 = r.e0i == r.e1i;           // pl1 x pl2 with pl1 == pl2
+  P.q1_0 = r.jref == e;              // q1 = pji x jref
+  P.q2_0 = r.iref == e;              // q2 = pji x iref
+  P.c3_0 = r.iref == r.jref;         // q1 x q2 with q1 == q2
+  atan2_partials(G.b1, G.a1, P.th_b1, P.th_a1);
+  atan2_partials(__fdiv_rn(G.s2, G.d), G.a2, P.ph_b2, P.ph_a2);
+  atan2_partials(__fdiv_rn(G.s3, G.d), G.a3, P.ta_b3, P.ta_a3);
+  P.inv_b1 = G.b1 == 0.f ? 0.f : 1.0f / G.b1;
+  P.inv_d = G.d == 0.f ? 0.f : 1.0f / G.d;
+  return P;
+}
+
+// the basis at x = dist / cutoff and its derivatives (the generated closed forms of basis_gemnet_2_3)
+struct ComenetEdgeBasis {
+  float rb[6], rbd[6], y0[2], y0d[2], ylm[4], ylmt[4], ylmp[4];
+};
+__device__ __forceinline__ void comenet_edge_basis(float x, const ComenetEdgeGeom& G, ComenetEdgeBasis& B) {
+  basis_gemnet_2_3::bessel(x, B.rb);
+  basis_gemnet_2_3::bessel_dx(x, B.rbd);
+  basis_gemnet_2_3::yl0(G.tau, B.y0);
+  basis_gemnet_2_3::yl0_dtheta(G.tau, B.y0d);
+  basis_gemnet_2_3::ylm(G.theta, G.phi, B.ylm);
+  basis_gemnet_2_3::ylm_dtheta(G.theta, G.phi, B.ylmt);
+  basis_gemnet_2_3::ylm_dphi(G.theta, G.phi, B.ylmp);
+}
+
+// Pass 1: per edge e, d(loss)/d(edge vector) of the five vectors its angles read, written to work[e][role][3] with
+// roles 0 = pji (e itself), 1 = in0 (e0i), 2 = in1 (e1i), 3 = iref, 4 = jref.
+__global__ void comenet_features_bwd_edge_kernel(const float* __restrict__ pos, const float* __restrict__ dist,
+                                                 const int32_t* __restrict__ src, const int32_t* __restrict__ dst,
+                                                 const int32_t* __restrict__ a0_in, const int32_t* __restrict__ a1_in,
+                                                 const int32_t* __restrict__ a0_out, const int32_t* __restrict__ a1_out,
+                                                 int n_edges, float inv_cutoff, const float* __restrict__ df1,
+                                                 const float* __restrict__ df2, float* __restrict__ work) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= n_edges) return;
+  const ComenetEdgeRefs rf = comenet_edge_refs(src, dst, a0_in, a1_in, a0_out, a1_out, e);
+  const ComenetEdgeGeom G = comenet_edge_geom<false>(pos, src, dst, e, rf);
+  const ComenetEdgePartials P = comenet_edge_partials(G, rf, e);
+  ComenetEdgeBasis B;
+  comenet_edge_basis(__fmul_rn(dist[e], inv_cutoff), G, B);
+  // features -> d(rbf), d theta, d phi, d tau                            features.py:289-295,340-348
+  float grb[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+  float gth = 0.f, gph = 0.f, gta = 0.f;
+#pragma unroll
+  for (int l = 0; l < 2; ++l)
+#pragma unroll
+    for (int r = 0; r < 3; ++r) {
+      const float g = __ldg(df2 + (size_t)e * NF2 + l * 3 + r);
+      grb[l * 3 + r] = fmaf(g, B.y0[l], grb[l * 3 + r]);
+      gta = fmaf(g * B.rb[l * 3 + r], B.y0d[l], gta);
+    }
+#pragma unroll
+  for (int h = 0; h < 4; ++h)
+#pragma unroll
+    for (int r = 0; r < 3; ++r) {
+      const int k = (h == 0 ? 0 : 1) * 3 + r;
+      const float g = __ldg(df1 + (size_t)e * NF1 + h * 3 + r);
+      grb[k] = fmaf(g, B.ylm[h], grb[k]);
+      gth = fmaf(g * B.rb[k], B.ylmt[h], gth);
+      gph = fmaf(g * B.rb[k], B.ylmp[h], gph);
+    }
+  float gx = 0.f;
+#pragma unroll
+  for (int k = 0; k < 6; ++k) gx = fmaf(grb[k], B.rbd[k], gx);
+  const float gdist = gx * inv_cutoff;
+  // angles -> vectors
+  const f3 M = neg3(G.pji);
+  f3 gP = scale3(G.pji, gdist * P.inv_d), gM = {0.f, 0.f, 0.f}, gA = {0.f, 0.f, 0.f};
+  // theta = atan2(|pl1|, M . in0)
+  const float g_a1 = gth * P.th_a1;
+  f3 gpl1 = scale3(G.pl1, gth * P.th_b1 * P.inv_b1);
+  gM = axpy3(g_a1, G.in0, gM);
+  gA = axpy3(g_a1, M, gA);
+  // phi = atan2(s2 / d, pl1 . pl2), s2 = (pl1 x pl2) . pji
+  const float g_b2 = gph * P.ph_b2, g_a2 = gph * P.ph_a2;
+  const float g_s2 = g_b2 / G.d;
+  float g_d = -g_b2 * G.s2 / (G.d * G.d);
+  const f3 gc2 = P.c2_0 ? f3{0.f, 0.f, 0.f} : scale3(G.pji, g_s2);
+  gP = axpy3(g_s2, G.c2, gP);
+  gpl1 = add3(gpl1, axpy3(g_a2, G.pl2, cross3(G.pl2, gc2)));
+  f3 gpl2 = axpy3(g_a2, G.pl1, cross3(gc2, G.pl1));
+  if (P.pl1_0) gpl1 = {0.f, 0.f, 0.f};
+  if (P.pl2_0) gpl2 = {0.f, 0.f, 0.f};
+  // tau = atan2(s3 / d, q1 . q2), s3 = (q1 x q2) . pji, q1 = pji x jref, q2 = pji x iref
+  const float g_b3 = gta * P.ta_b3, g_a3 = gta * P.ta_a3;
+  const float g_s3 = g_b3 / G.d;
+  g_d -= g_b3 * G.s3 / (G.d * G.d);
+  const f3 gc3 = P.c3_0 ? f3{0.f, 0.f, 0.f} : scale3(G.pji, g_s3);
+  gP = axpy3(g_s3, G.c3, gP);
+  f3 gq1 = axpy3(g_a3, G.q2, cross3(G.q2, gc3));
+  f3 gq2 = axpy3(g_a3, G.q1, cross3(gc3, G.q1));
+  if (P.q1_0) gq1 = {0.f, 0.f, 0.f};
+  if (P.q2_0) gq2 = {0.f, 0.f, 0.f};
+  gP = add3(gP, add3(cross3(G.jref, gq1), cross3(G.iref, gq2)));
+  const f3 gS = cross3(gq1, G.pji), gR = cross3(gq2, G.pji);
+  // d = sqrt(sum(pji^2)) of phi / tau
+  gP = axpy3(g_d / G.d, G.pji, gP);
+  // pl1 = M x in0, pl2 = M x in1
+  gM = add3(gM, add3(cross3(G.in0, gpl1), cross3(G.in1, gpl2)));
+  gA = add3(gA, cross3(gpl1, M));
+  const f3 gB = cross3(gpl2, M);
+  gP = sub3(gP, gM);
+  float* w = work + (size_t)e * 15;
+  const f3 out[5] = {gP, gA, gB, gR, gS};
+#pragma unroll
+  for (int k = 0; k < 5; ++k) { w[3 * k] = out[k].x; w[3 * k + 1] = out[k].y; w[3 * k + 2] = out[k].z; }
+}
+
+// Pass 2: dvec[e'] = the sum, in edge order, of every pass-1 contribution to edge e'.  An edge e reads e' as in0 / in1 /
+// iref only if both end in the same node (dst[e] == dst[e']): the in-edges of dst[e']; as jref only if both start in the
+// same node: the out-edges of src[e'].  No atomics: the result is the same bits run to run.
+__global__ void comenet_features_bwd_gather_kernel(const int32_t* __restrict__ src, const int32_t* __restrict__ dst,
+                                                   const int32_t* __restrict__ row_ptr,
+                                                   const int32_t* __restrict__ out_ptr,
+                                                   const int32_t* __restrict__ out_list,
+                                                   const int32_t* __restrict__ a0_in, const int32_t* __restrict__ a1_in,
+                                                   const int32_t* __restrict__ a0_out,
+                                                   const int32_t* __restrict__ a1_out, int n_edges,
+                                                   const float* __restrict__ work, float* __restrict__ dvec) {
+  const int ep = blockIdx.x * blockDim.x + threadIdx.x;
+  if (ep >= n_edges) return;
+  const int j = src[ep], i = dst[ep];
+  const float* w = work + (size_t)ep * 15;
+  float ax = w[0], ay = w[1], az = w[2];
+  {
+    const int e0i = a0_in[i], e1i = a1_in[i], n0 = src[e0i];
+    for (int e = row_ptr[i]; e < row_ptr[i + 1]; ++e) {
+      const int iref = (n0 == src[e]) ? e1i : e0i;
+      const float* c = work + (size_t)e * 15;
+      if (e0i == ep) { ax += c[3]; ay += c[4]; az += c[5]; }
+      if (e1i == ep) { ax += c[6]; ay += c[7]; az += c[8]; }
+      if (iref == ep) { ax += c[9]; ay += c[10]; az += c[11]; }
+    }
+  }
+  {
+    const int e0j = a0_out[j], e1j = a1_out[j], n0_j = dst[e0j];
+    for (int k = out_ptr[j]; k < out_ptr[j + 1]; ++k) {
+      const int e = out_list[k];
+      const int jref = (n0_j == dst[e]) ? e1j : e0j;
+      if (jref == ep) {
+        const float* c = work + (size_t)e * 15;
+        ax += c[12]; ay += c[13]; az += c[14];
+      }
+    }
+  }
+  dvec[3 * (size_t)ep] = ax; dvec[3 * (size_t)ep + 1] = ay; dvec[3 * (size_t)ep + 2] = az;
+}
+
+// Pass 3: vec[e] = pos[src[e]] - pos[dst[e]]  ->  dpos[n] = sum of dvec over n's out-edges - sum over its in-edges
+__global__ void comenet_features_bwd_node_kernel(const int32_t* __restrict__ row_ptr,
+                                                 const int32_t* __restrict__ out_ptr,
+                                                 const int32_t* __restrict__ out_list, int n_nodes,
+                                                 const float* __restrict__ dvec, float* __restrict__ dpos) {
+  const int n = blockIdx.x * blockDim.x + threadIdx.x;
+  if (n >= n_nodes) return;
+  float ax = 0.f, ay = 0.f, az = 0.f;
+  for (int k = out_ptr[n]; k < out_ptr[n + 1]; ++k) {
+    const int e = out_list[k];
+    ax += dvec[3 * (size_t)e]; ay += dvec[3 * (size_t)e + 1]; az += dvec[3 * (size_t)e + 2];
+  }
+  for (int e = row_ptr[n]; e < row_ptr[n + 1]; ++e) {
+    ax -= dvec[3 * (size_t)e]; ay -= dvec[3 * (size_t)e + 1]; az -= dvec[3 * (size_t)e + 2];
+  }
+  dpos[3 * (size_t)n] = ax; dpos[3 * (size_t)n + 1] = ay; dpos[3 * (size_t)n + 2] = az;
+}
+
+// Forward mode: f1_dot / f2_dot of every edge along the per-atom displacement cvec [N, 3]
+__global__ void comenet_features_tangent_kernel(const float* __restrict__ pos, const float* __restrict__ dist,
+                                                const int32_t* __restrict__ src, const int32_t* __restrict__ dst,
+                                                const int32_t* __restrict__ a0_in, const int32_t* __restrict__ a1_in,
+                                                const int32_t* __restrict__ a0_out, const int32_t* __restrict__ a1_out,
+                                                int n_edges, float inv_cutoff, const float* __restrict__ cvec,
+                                                float* __restrict__ f1_dot, float* __restrict__ f2_dot) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= n_edges) return;
+  const ComenetEdgeRefs r = comenet_edge_refs(src, dst, a0_in, a1_in, a0_out, a1_out, e);
+  const ComenetEdgeGeom G = comenet_edge_geom<false>(pos, src, dst, e, r);
+  const ComenetEdgePartials P = comenet_edge_partials(G, r, e);
+  ComenetEdgeBasis B;
+  comenet_edge_basis(__fmul_rn(dist[e], inv_cutoff), G, B);
+  const f3 zero = {0.f, 0.f, 0.f};
+  const f3 dP = edge_vec<false>(cvec, src, dst, e), dA = edge_vec<false>(cvec, src, dst, r.e0i);
+  const f3 dB = edge_vec<false>(cvec, src, dst, r.e1i), dR = edge_vec<false>(cvec, src, dst, r.iref);
+  const f3 dS = edge_vec<false>(cvec, src, dst, r.jref);
+  const f3 M = neg3(G.pji), dM = neg3(dP);
+  const float ddist = dot3(G.pji, dP) * P.inv_d;
+  // theta
+  const f3 dpl1 = P.pl1_0 ? zero : add3(cross3(dM, G.in0), cross3(M, dA));
+  const float da1 = dot3(dM, G.in0) + dot3(M, dA);
+  const float db1 = dot3(G.pl1, dpl1) * P.inv_b1;
+  const float dth = fmaf(P.th_b1, db1, P.th_a1 * da1);
+  // phi
+  const float dd = dot3(G.pji, dP) / G.d;
+  const f3 dpl2 = P.pl2_0 ? zero : add3(cross3(dM, G.in1), cross3(M, dB));
+  const float da2 = dot3(dpl1, G.pl2) + dot3(G.pl1, dpl2);
+  const f3 dc2 = P.c2_0 ? zero : add3(cross3(dpl1, G.pl2), cross3(G.pl1, dpl2));
+  const float ds2 = dot3(dc2, G.pji) + dot3(G.c2, dP);
+  const float db2 = ds2 / G.d - G.s2 * dd / (G.d * G.d);
+  const float dph = fmaf(P.ph_b2, db2, P.ph_a2 * da2);
+  // tau
+  const f3 dq1 = P.q1_0 ? zero : add3(cross3(dP, G.jref), cross3(G.pji, dS));
+  const f3 dq2 = P.q2_0 ? zero : add3(cross3(dP, G.iref), cross3(G.pji, dR));
+  const float da3 = dot3(dq1, G.q2) + dot3(G.q1, dq2);
+  const f3 dc3 = P.c3_0 ? zero : add3(cross3(dq1, G.q2), cross3(G.q1, dq2));
+  const float ds3 = dot3(dc3, G.pji) + dot3(G.c3, dP);
+  const float db3 = ds3 / G.d - G.s3 * dd / (G.d * G.d);
+  const float dta = fmaf(P.ta_b3, db3, P.ta_a3 * da3);
+  // features
+  const float dx = ddist * inv_cutoff;
+#pragma unroll
+  for (int l = 0; l < 2; ++l)
+#pragma unroll
+    for (int q = 0; q < 3; ++q) {
+      const int k = l * 3 + q;
+      f2_dot[(size_t)e * NF2 + k] = fmaf(B.rbd[k] * dx, B.y0[l], B.rb[k] * B.y0d[l] * dta);
+    }
+#pragma unroll
+  for (int h = 0; h < 4; ++h)
+#pragma unroll
+    for (int q = 0; q < 3; ++q) {
+      const int k = (h == 0 ? 0 : 1) * 3 + q;
+      f1_dot[(size_t)e * NF1 + h * 3 + q] =
+          fmaf(B.rbd[k] * dx, B.ylm[h], B.rb[k] * fmaf(B.ylmt[h], dth, B.ylmp[h] * dph));
+    }
 }
 
 // ------------------------------------------------------------------ OCP variant: arbitrary edge lists, periodic images
@@ -552,6 +869,45 @@ int dig3d_comenet_geometry(const float* pos, const float* dist, const int32_t* s
         pos, dist, src, dst, a0i, a1i, a0o, a1o, (int)n_edges, 1.0f / (float)cutoff, feature1, feature2, angles);
     DIG3D_LAUNCH_CHECK();
   }
+  return DIG3D_OK;
+}
+
+int dig3d_comenet_features_bwd(const float* pos, const float* dist, const int32_t* src, const int32_t* dst,
+                               const int32_t* row_ptr, const int32_t* out_ptr, const int32_t* out_list,
+                               const int32_t* refs, int64_t n_nodes, int64_t n_edges, double cutoff,
+                               const float* dfeature1, const float* dfeature2, float* work, float* dpos,
+                               void* stream) {
+  DIG3D_REQUIRE(pos && dist && src && dst && row_ptr && out_ptr && out_list && refs && dfeature1 && dfeature2 &&
+                    work && dpos, "comenet_features_bwd: null pointer");
+  if (n_nodes == 0) return DIG3D_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int32_t* a0i = refs; const int32_t* a1i = refs + n_nodes;
+  const int32_t* a0o = refs + 2 * n_nodes; const int32_t* a1o = refs + 3 * n_nodes;
+  float* dvec = work + 15 * n_edges;
+  if (n_edges) {
+    comenet_features_bwd_edge_kernel<<<ceil_div(n_edges, 128), 128, 0, st>>>(
+        pos, dist, src, dst, a0i, a1i, a0o, a1o, (int)n_edges, 1.0f / (float)cutoff, dfeature1, dfeature2, work);
+    DIG3D_LAUNCH_CHECK();
+    comenet_features_bwd_gather_kernel<<<ceil_div(n_edges, 128), 128, 0, st>>>(
+        src, dst, row_ptr, out_ptr, out_list, a0i, a1i, a0o, a1o, (int)n_edges, work, dvec);
+    DIG3D_LAUNCH_CHECK();
+  }
+  comenet_features_bwd_node_kernel<<<ceil_div(n_nodes, 128), 128, 0, st>>>(row_ptr, out_ptr, out_list, (int)n_nodes,
+                                                                           dvec, dpos);
+  DIG3D_LAUNCH_CHECK();
+  return DIG3D_OK;
+}
+
+int dig3d_comenet_features_tangent(const float* pos, const float* dist, const int32_t* src, const int32_t* dst,
+                                   const int32_t* refs, int64_t n_nodes, int64_t n_edges, double cutoff,
+                                   const float* cvec, float* feature1_dot, float* feature2_dot, void* stream) {
+  DIG3D_REQUIRE(pos && dist && src && dst && refs && cvec && feature1_dot && feature2_dot,
+                "comenet_features_tangent: null pointer");
+  if (n_nodes == 0 || n_edges == 0) return DIG3D_OK;
+  comenet_features_tangent_kernel<<<ceil_div(n_edges, 128), 128, 0, (cudaStream_t)stream>>>(
+      pos, dist, src, dst, refs, refs + n_nodes, refs + 2 * n_nodes, refs + 3 * n_nodes, (int)n_edges,
+      1.0f / (float)cutoff, cvec, feature1_dot, feature2_dot);
+  DIG3D_LAUNCH_CHECK();
   return DIG3D_OK;
 }
 

@@ -391,6 +391,92 @@ __global__ void graphnorm_bwd_kernel(const float* __restrict__ h, const float* _
   }
 }
 
+// Forward mode of GraphNorm (force training, autograd_jvp.py) along a tangent h_dot, from the forward's shift / std.
+// Per graph and channel, with n nodes, o = h - shift, std = sqrt(mean(o^2) + eps):
+//   o_dot = h_dot - mean_scale * mean(h_dot)      std_dot = mean(o * o_dot) / std
+//   y_dot = weight * (o_dot / std - o * std_dot / std^2)
+__global__ void graphnorm_tangent_kernel(const float* __restrict__ h, const float* __restrict__ hd,
+                                         const int32_t* __restrict__ graph_ptr, int width,
+                                         const float* __restrict__ weight, const float* __restrict__ mean_scale,
+                                         const float* __restrict__ shift, const float* __restrict__ stdv,
+                                         float* __restrict__ yd) {
+  const int g = blockIdx.x;
+  const int n0 = graph_ptr[g], n1 = graph_ptr[g + 1];
+  if (n1 <= n0) return;
+  const float cnt = (float)(n1 - n0);
+  for (int c = threadIdx.x; c < width; c += blockDim.x) {
+    const float sh = shift[(size_t)g * width + c], sd = stdv[(size_t)g * width + c];
+    const float w = __ldg(weight + c), ms = __ldg(mean_scale + c);
+    float sum_d = 0.f;
+    for (int n = n0; n < n1; ++n) sum_d += hd[(size_t)n * width + c];
+    const float shd = ms * (sum_d / cnt);
+    float A = 0.f;
+    for (int n = n0; n < n1; ++n) {
+      const size_t k = (size_t)n * width + c;
+      A = fmaf(h[k] - sh, hd[k] - shd, A);
+    }
+    const float r = 1.0f / sd;
+    const float sdd = A / cnt * r;
+    for (int n = n0; n < n1; ++n) {
+      const size_t k = (size_t)n * width + c;
+      yd[k] = w * ((hd[k] - shd) * r - (h[k] - sh) * sdd * r * r);
+    }
+  }
+}
+
+// Reverse mode of graphnorm_tangent_kernel: gy = d loss / d y_dot -> d h, d h_dot, d weight, d mean_scale.
+// With mu = mean(h), mud = mean(h_dot), r = 1/std, u = w gy, and sums over the graph's nodes:
+//   d std_dot = -r^2 sum(u o)          d std = sum(u (2 o std_dot r^3 - o_dot r^2)) - d std_dot std_dot r
+//   d o_k = -u_k std_dot r^2 + (d std_dot o_dot_k + d std o_k) r / n      d o_dot_k = u_k r + d std_dot o_k r / n
+//   d h_k = d o_k - mean_scale sum(d o) / n            d h_dot_k = d o_dot_k - mean_scale sum(d o_dot) / n
+//   d weight += sum(gy (o_dot r - o std_dot r^2))      d mean_scale += -mu sum(d o) - mud sum(d o_dot)
+__global__ void graphnorm_tangent_bwd_kernel(const float* __restrict__ h, const float* __restrict__ hd,
+                                             const float* __restrict__ gy, const int32_t* __restrict__ graph_ptr,
+                                             int width, const float* __restrict__ weight,
+                                             const float* __restrict__ mean_scale, const float* __restrict__ shift,
+                                             const float* __restrict__ stdv, float* __restrict__ dh,
+                                             float* __restrict__ dhd, float* __restrict__ dweight,
+                                             float* __restrict__ dmean_scale) {
+  const int g = blockIdx.x;
+  const int n0 = graph_ptr[g], n1 = graph_ptr[g + 1];
+  if (n1 <= n0) return;
+  const float cnt = (float)(n1 - n0);
+  for (int c = threadIdx.x; c < width; c += blockDim.x) {
+    const float sh = shift[(size_t)g * width + c], sd = stdv[(size_t)g * width + c];
+    const float w = __ldg(weight + c), ms = __ldg(mean_scale + c);
+    float S = 0.f, Sd = 0.f;
+    for (int n = n0; n < n1; ++n) { S += h[(size_t)n * width + c]; Sd += hd[(size_t)n * width + c]; }
+    const float mu = S / cnt, mud = Sd / cnt, shd = ms * mud;
+    float A = 0.f, G = 0.f, Go = 0.f, God = 0.f, So = 0.f, Sod = 0.f;
+    for (int n = n0; n < n1; ++n) {
+      const size_t k = (size_t)n * width + c;
+      const float o = h[k] - sh, od = hd[k] - shd, gk = gy[k];
+      A = fmaf(o, od, A);
+      G += gk;
+      Go = fmaf(gk, o, Go);
+      God = fmaf(gk, od, God);
+      So += o;
+      Sod += od;
+    }
+    const float r = 1.0f / sd, r2 = r * r;
+    const float sdd = A / cnt * r;
+    const float g_sdd = -w * Go * r2;
+    const float g_sd = w * (2.0f * sdd * r2 * r * Go - God * r2) - g_sdd * sdd * r;
+    const float a_o = g_sdd * r / cnt, b_o = g_sd * r / cnt;          // d o_k = -w gy_k sdd r^2 + a_o od_k + b_o o_k
+    const float sum_do = -w * G * sdd * r2 + a_o * Sod + b_o * So;
+    const float sum_dod = w * G * r + a_o * So;
+    const float back_o = ms * sum_do / cnt, back_od = ms * sum_dod / cnt;
+    for (int n = n0; n < n1; ++n) {
+      const size_t k = (size_t)n * width + c;
+      const float o = h[k] - sh, od = hd[k] - shd, gk = gy[k];
+      dh[k] = -w * gk * sdd * r2 + a_o * od + b_o * o - back_o;
+      dhd[k] = w * gk * r + a_o * o - back_od;
+    }
+    atomicAdd(dweight + c, God * r - Go * sdd * r2);
+    atomicAdd(dmean_scale + c, -mu * sum_do - mud * sum_dod);
+  }
+}
+
 template <int NOUT, int K, int TM = 64, int MINB = 1>
 static int launch_linear_tiled(const float* x, int64_t rows, const float* w, const float* b, float* y, float* act_out,
                                int groups, cudaStream_t st) {
@@ -617,6 +703,31 @@ int dig3d_graphnorm_bwd(const float* h, const float* dy, const int32_t* graph_pt
   if (n_graphs == 0) return DIG3D_OK;
   graphnorm_bwd_kernel<<<(int)n_graphs, width < 256 ? width : 256, 0, (cudaStream_t)stream>>>(
       h, dy, graph_ptr, width, weight, mean_scale, shift, stdv, dx, dweight, dbias, dmean_scale);
+  DIG3D_LAUNCH_CHECK();
+  return DIG3D_OK;
+}
+
+int dig3d_graphnorm_tangent(const float* h, const float* h_dot, const int32_t* graph_ptr, int64_t n_graphs,
+                            int32_t width, const float* weight, const float* mean_scale, const float* shift,
+                            const float* stdv, float* y_dot, void* stream) {
+  DIG3D_REQUIRE(h && h_dot && graph_ptr && weight && mean_scale && shift && stdv && y_dot && width > 0,
+                "graphnorm_tangent: bad arguments");
+  if (n_graphs == 0) return DIG3D_OK;
+  graphnorm_tangent_kernel<<<(int)n_graphs, width < 256 ? width : 256, 0, (cudaStream_t)stream>>>(
+      h, h_dot, graph_ptr, width, weight, mean_scale, shift, stdv, y_dot);
+  DIG3D_LAUNCH_CHECK();
+  return DIG3D_OK;
+}
+
+int dig3d_graphnorm_tangent_bwd(const float* h, const float* h_dot, const float* dy_dot, const int32_t* graph_ptr,
+                                int64_t n_graphs, int32_t width, const float* weight, const float* mean_scale,
+                                const float* shift, const float* stdv, float* dh, float* dh_dot, float* dweight,
+                                float* dmean_scale, void* stream) {
+  DIG3D_REQUIRE(h && h_dot && dy_dot && graph_ptr && weight && mean_scale && shift && stdv && dh && dh_dot &&
+                    dweight && dmean_scale && width > 0, "graphnorm_tangent_bwd: bad arguments");
+  if (n_graphs == 0) return DIG3D_OK;
+  graphnorm_tangent_bwd_kernel<<<(int)n_graphs, width < 256 ? width : 256, 0, (cudaStream_t)stream>>>(
+      h, h_dot, dy_dot, graph_ptr, width, weight, mean_scale, shift, stdv, dh, dh_dot, dweight, dmean_scale);
   DIG3D_LAUNCH_CHECK();
   return DIG3D_OK;
 }

@@ -56,7 +56,8 @@ class Graph3D:
     __slots__ = ("n_nodes", "n_graphs", "n_edges", "n_triplets", "cap", "graph_ptr", "batch",
                  "row_ptr", "src", "dst", "edge_index", "dist", "vec", "trip_ptr",
                  "angle", "torsion", "idx_kj", "idx_ji", "idx_kj64", "idx_ji64",
-                 "out_ptr", "out_list", "pos_in")      # out-edge lists (CSR by source), None for graphs built without them
+                 "out_ptr", "out_list", "pos_in",      # out-edge lists (CSR by source), None for graphs built without them
+                 "comenet_refs")                       # ComENet's reference atoms (comenet_geometry)
 
     def __init__(self):
         for s in self.__slots__:
@@ -515,6 +516,8 @@ def radius_graph_pbc(pos, cell, natoms, radius, max_num_neighbors_threshold):
 
 # ----------------------------------------------------------------------------- ComENet
 def comenet_geometry(g, pos, cutoff, want_angles=False):
+    """-> (feature1 [E,12], feature2 [E,6], angles [E,3] or None).  The reference atoms it chose stay on the graph
+    (g.comenet_refs) for the force kernels below."""
     dev = pos.device
     e, n = g.n_edges, g.n_nodes
     refs = torch.empty(4 * max(n, 1) + 2, dtype=torch.int32, device=dev)   # + the two batch-wide "empty segment" flags
@@ -524,7 +527,42 @@ def comenet_geometry(g, pos, cutoff, want_angles=False):
     call("dig3d_comenet_geometry", _p(pos.detach(), torch.float32, "pos"), _p(g.dist), _p(g.src), _p(g.dst),
          _p(g.row_ptr), _p(g.graph_ptr), _p(g.batch, torch.int64), n, e, float(cutoff), _p(refs), _p(f1), _p(f2),
          _p(angles) if want_angles else None, _stream())
+    g.comenet_refs = refs
     return f1, f2, angles
+
+
+def _comenet_force_inputs(g, pos):
+    if getattr(g, "comenet_refs", None) is None:
+        raise ValueError("ComENet forces need the reference atoms of ops.comenet_geometry(g, pos, ...) on the graph")
+    if g.out_ptr is None or g.out_list is None:
+        raise ValueError("ComENet forces need the graph's out-edge lists (ops.build_graph)")
+    return _p(pos.detach(), torch.float32, "pos")
+
+
+def comenet_features_bwd(g, pos, cutoff, df1, df2):
+    """dpos [N, 3] = d loss / d pos through comenet_geometry's feature1 / feature2 given their gradients df1 [E,12] /
+    df2 [E,6].  Deterministic (no float atomics)."""
+    p = _comenet_force_inputs(g, pos)
+    e, n = g.n_edges, g.n_nodes
+    dpos = torch.empty(n, 3, dtype=F32, device=pos.device)
+    work = torch.empty(max(18 * e, 1), dtype=F32, device=pos.device)
+    if n:
+        call("dig3d_comenet_features_bwd", p, _p(g.dist), _p(g.src), _p(g.dst), _p(g.row_ptr), _p(g.out_ptr),
+             _p(g.out_list), _p(g.comenet_refs), n, e, float(cutoff), _p(df1, F32, "df1"), _p(df2, F32, "df2"),
+             _p(work), _p(dpos), _stream())
+    return dpos
+
+
+def comenet_features_tangent(g, pos, cutoff, cvec):
+    """(feature1_dot [E,12], feature2_dot [E,6]) along the per-atom displacement cvec [N, 3]."""
+    p = _comenet_force_inputs(g, pos)
+    e, n = g.n_edges, g.n_nodes
+    f1d = torch.empty(max(e, 1), 12, dtype=F32, device=pos.device)[:e]
+    f2d = torch.empty(max(e, 1), 6, dtype=F32, device=pos.device)[:e]
+    if e:
+        call("dig3d_comenet_features_tangent", p, _p(g.dist), _p(g.src), _p(g.dst), _p(g.comenet_refs), n, e,
+             float(cutoff), _p(cvec, F32, "cvec"), _p(f1d), _p(f2d), _stream())
+    return f1d, f2d
 
 
 def comenet_embed(z, emb_weight):
@@ -1117,6 +1155,28 @@ def graphnorm_bwd(h, dy, graph_ptr, weight, mean_scale, shift, std):
     call("dig3d_graphnorm_bwd", _p(h, F32, "h"), _p(dy, F32, "dy"), _p(graph_ptr, torch.int32), g, wd, _p(weight, F32),
          _p(mean_scale, F32), _p(shift), _p(std), _p(dx), _p(dw), _p(db), _p(dms), _stream())
     return dx, dw, db, dms
+
+
+def graphnorm_tangent(h, hd, graph_ptr, weight, mean_scale, shift, std):
+    """y_dot of GraphNorm along h_dot, from graphnorm's shift / std."""
+    g, wd = graph_ptr.numel() - 1, h.size(1)
+    yd = torch.empty_like(h)
+    call("dig3d_graphnorm_tangent", _p(h, F32, "h"), _p(hd, F32, "h_dot"), _p(graph_ptr, torch.int32), g, wd,
+         _p(weight, F32), _p(mean_scale, F32), _p(shift), _p(std), _p(yd), _stream())
+    return yd
+
+
+def graphnorm_tangent_bwd(h, hd, dyd, graph_ptr, weight, mean_scale, shift, std):
+    """-> (dh, dh_dot, dweight, dmean_scale) of graphnorm_tangent given dy_dot."""
+    g, wd = graph_ptr.numel() - 1, h.size(1)
+    dh = torch.empty_like(h)
+    dhd = torch.empty_like(h)
+    dw = torch.zeros(wd, device=h.device, dtype=F32)
+    dms = torch.zeros(wd, device=h.device, dtype=F32)
+    call("dig3d_graphnorm_tangent_bwd", _p(h, F32, "h"), _p(hd, F32, "h_dot"), _p(dyd, F32, "dy_dot"),
+         _p(graph_ptr, torch.int32), g, wd, _p(weight, F32), _p(mean_scale, F32), _p(shift), _p(std), _p(dh), _p(dhd),
+         _p(dw), _p(dms), _stream())
+    return dh, dhd, dw, dms
 
 
 # ---------------------------------------------------------------------------------------------------------------

@@ -13,6 +13,7 @@ import torch
 from torch import nn
 
 from ... import autograd as ag
+from ... import autograd_jvp as jv
 from ... import ops
 from ._common import glorot, require_cuda, wants_grad
 
@@ -133,13 +134,19 @@ class SimpleInteractionBlock(nn.Module):
 
 
 class ComENet(nn.Module):
-    r"""Drop-in for dig.threedgraph.method.ComENet (same constructor arguments and defaults).
-    This round's kernels are compiled for hidden_channels=256, middle_channels=64, num_radial=3,
-    num_spherical=2 (the class defaults); other sizes raise at construction."""
+    r"""Drop-in for dig.threedgraph.method.ComENet (same constructor arguments and defaults, in the same order).
+    The fused inference kernels are compiled for hidden_channels=256, middle_channels=64 and <= 8 output layers; other
+    widths run the generic CUDA primitives.  num_radial=3, num_spherical=2 (the class defaults) are required.
+
+    `energy_and_force=True` (an extension at the end of the argument list, as SchNet / DimeNetPP / SphereNet have it in
+    the reference): forward calls `pos.requires_grad_()`.  Whenever pos requires grad -- set by this flag or by the caller
+    -- the energy is differentiable in pos (forces = -grad(E, pos)), and in training mode twice, for training on forces
+    (run.train(..., energy_and_force=True))."""
 
     def __init__(self, cutoff=8.0, num_layers=4, hidden_channels=256, middle_channels=64, out_channels=1,
-                 num_radial=3, num_spherical=2, num_output_layers=3):
+                 num_radial=3, num_spherical=2, num_output_layers=3, energy_and_force=False):
         super().__init__()
+        self.energy_and_force = energy_and_force
         if (num_radial, num_spherical) != (3, 2):
             raise NotImplementedError(
                 "the ComENet geometry/basis kernel is generated for num_radial=3, num_spherical=2 "
@@ -200,6 +207,15 @@ class ComENet(nn.Module):
         g = ops.build_graph(pos, batch, self.cutoff, num_graphs=getattr(data, "num_graphs", None),
                             want_edge_index=False, z=z, z_rows=self.emb.emb.num_embeddings)
         f1, f2, _ = ops.comenet_geometry(g, pos, self.cutoff)
+        if torch.is_grad_enabled() and pos.requires_grad:
+            # forces: f1 / f2 carry the position gradient (csrc/comenet.cu); the graph's input-gradient GEMMs stay exact
+            if self.training and any(p.requires_grad for p in self.parameters()):
+                # training ON forces (run.py:110-123): reverse over forward mode, dig_b200/autograd_jvp.py
+                return jv.energy_with_force(
+                    lambda p: self._exact(self._forward_train, z, g, *ag.comenet_features(p, g, self.cutoff, f1, f2)),
+                    lambda p, c: self._exact(self._forward_dual, z, g, p, c, f1, f2),
+                    pos, tuple(self.parameters()))
+            return self._exact(self._forward_train, z, g, *ag.comenet_features(pos, g, self.cutoff, f1, f2))
         if wants_grad(self) or self._generic:
             return self._forward_train(z, g, f1, f2)
         dense = os.environ.get("DIG3D_COMENET_DENSE", "h16")
@@ -373,5 +389,46 @@ class ComENet(nn.Module):
         x = lin(self.lin_out, x)
         return ag.segment_sum(x, g.graph_ptr, g.batch)
 
+    @staticmethod
+    def _exact(fn, *args):
+        """Run fn with the input-gradient GEMMs of the recorded graph kept exact (graphs that carry forces)."""
+        ag.EXACT_BACKWARD[0] = True
+        try:
+            return fn(*args)
+        finally:
+            ag.EXACT_BACKWARD[0] = False
+
+    def _forward_dual(self, z, g, pos, cvec, f1, f2):
+        """(E, E_dot): _forward_train op for op, carried with its directional derivative along the per-atom displacement
+        cvec [N, 3], on the first-order primitives so that E_dot is differentiable in the parameters (autograd_jvp.py).
+        The features and their tangents (ops.comenet_features_tangent) carry no parameters: constants here; the
+        embedding rows carry no tangent."""
+        f1d, f2d = ops.comenet_features_tangent(g, pos.detach(), self.cutoff, cvec)
+        lin, lsd, addd = jv.lin_dual, jv.lin_swish_dual, jv.add_dual
+        x, xd = ag.swish(ag.gather_rows(self.emb.emb.weight, z)), None                  # comenet.py:125-127
+        for blk in self.interaction_blocks:                                             # comenet.py:195-215
+            x, xd = lsd(blk.lin, x, xd)
+            hs = []
+            for conv, lf, l, feat, feat_d in ((blk.conv1, blk.lin_feature1, blk.lin1, f1, f1d),
+                                              (blk.conv2, blk.lin_feature2, blk.lin2, f2, f2d)):
+                w, wd = lin(lf.lin2, *lin(lf.lin1, feat, feat_d))
+                m, md = jv.mul_dual(w, wd, *jv.gather_rows_dual(x, xd, g.src))
+                agg, agg_d = jv.segment_sum_dual(m, md, g.row_ptr, g.dst)
+                h, hd = addd(*lin(conv.lin_rel, agg, agg_d), *lin(conv.lin_root, x, xd))
+                hs.append(lsd(l, h, hd))
+            cat = torch.cat([hs[0][0], hs[1][0]], 1)                                     # copies only
+            cat_d = torch.cat([hs[0][1], hs[1][1]], 1)
+            h, hd = addd(*lin(blk.lin_cat, cat, cat_d), x, xd)
+            for l in blk.lins:
+                h, hd = addd(*lsd(l, h, hd), h, hd)
+            h, hd = jv.graphnorm_dual(h, hd, blk.norm, g.graph_ptr)
+            x, xd = lin(blk.final, h, hd)
+        for l in self.lins:
+            x, xd = lsd(l, x, xd)
+        x, xd = lin(self.lin_out, x, xd)
+        return jv.segment_sum_dual(x, xd, g.graph_ptr, g.batch)
+
     def forward(self, batch_data):
+        if self.energy_and_force:
+            batch_data.pos.requires_grad_()
         return self._forward(batch_data)

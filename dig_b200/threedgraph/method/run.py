@@ -7,7 +7,8 @@ dig_b200.data.DataLoader (same constructor use, concatenating collate).
 `val` (inference, the reference's eval loop) runs the fused forward kernels; `train` runs the differentiable
 training path (dig_b200/autograd.py: hand-written forward + backward kernels, torch.autograd keeps the tape)
 for the models that have one, and raises for a model whose forward returns a non-differentiable output.
-Force training (energy_and_force=True) needs a double backward and raises in the models.
+Force training (energy_and_force=True) needs a double backward: SchNet, DimeNet++, SphereNet and ComENet have one
+(autograd_dd.py / autograd_jvp.py); for a model without one, `train` raises.
 """
 import os
 
@@ -135,8 +136,8 @@ class run():
                     raise NotImplementedError(
                         "run.train(energy_and_force=True): the force loss needs d(force)/d(parameters), i.e. a double "
                         "backward through the model; this model has no second-order path (SchNet: autograd_dd.py, "
-                        "DimeNet++ / SphereNet: autograd_jvp.py) -- training on forces would silently ignore the force "
-                        "term")
+                        "DimeNet++ / SphereNet / ComENet: autograd_jvp.py) -- training on forces would silently ignore "
+                        "the force term")
                 e_loss = loss_func(out, batch_data.y.unsqueeze(1))
                 f_loss = loss_func(force, batch_data.force)
                 loss = e_loss + p * f_loss

@@ -436,6 +436,21 @@ int dig3d_comenet_geometry(const float* pos, const float* dist, const int32_t* s
                            const int32_t* row_ptr, const int32_t* graph_ptr, const int64_t* batch,
                            int64_t n_nodes, int64_t n_edges, double cutoff, int32_t* refs, float* feature1,
                            float* feature2, float* angles, void* stream);
+/* Forces through the geometry above (refs: the buffer dig3d_comenet_geometry filled for the same pos and graph).
+ * features_bwd: dpos[N,3] (every row written) = d loss / d pos given dfeature1 [E,12] / dfeature2 [E,6], with ATen's
+ * conventions at singular points (a zero vector's norm and atan2(0, 0) pass no gradient) and no float atomics: three
+ * passes (per edge: the five edge-vector gradients into work[0, 15E); per edge: their sum, in edge order, into
+ * work[15E, 18E); per node: out-edges minus in-edges).  work: [18 * E] floats; out_ptr / out_list: the out-edge lists
+ * of dig3d_edge_fill_out.  features_tangent: feature1_dot [E,12] / feature2_dot [E,6] along the per-atom displacement
+ * cvec [N,3], the transpose of features_bwd. */
+int dig3d_comenet_features_bwd(const float* pos, const float* dist, const int32_t* src, const int32_t* dst,
+                               const int32_t* row_ptr, const int32_t* out_ptr, const int32_t* out_list,
+                               const int32_t* refs, int64_t n_nodes, int64_t n_edges, double cutoff,
+                               const float* dfeature1, const float* dfeature2, float* work, float* dpos,
+                               void* stream);
+int dig3d_comenet_features_tangent(const float* pos, const float* dist, const int32_t* src, const int32_t* dst,
+                                   const int32_t* refs, int64_t n_nodes, int64_t n_edges, double cutoff,
+                                   const float* cvec, float* feature1_dot, float* feature2_dot, void* stream);
 
 /* ComENet-OCP (reference dig/threedgraph/method/comenet/ocp/comenet-ocp.py:343-474): the graph arrives as an arbitrary
  * edge list with periodic images.  dig3d_pbc_edge_vectors = ocpmodels' get_pbc_distances (distance_vec = pos[row] -
@@ -581,6 +596,17 @@ int dig3d_graphnorm(const float* h, const int32_t* graph_ptr, int64_t n_graphs, 
 int dig3d_graphnorm_bwd(const float* h, const float* dy, const int32_t* graph_ptr, int64_t n_graphs, int32_t width,
                         const float* weight, const float* mean_scale, const float* shift, const float* stdv, float* dx,
                         float* dweight, float* dbias, float* dmean_scale, void* stream);
+/* GraphNorm's forward mode (force training) from the forward's shift / stdv: with o = h - shift,
+ * y_dot = weight * (o_dot / std - o * std_dot / std^2), o_dot = h_dot - mean_scale * mean(h_dot),
+ * std_dot = mean(o * o_dot) / std; every row of y_dot written.  tangent_bwd: the gradients of y_dot given dy_dot;
+ * dh / dh_dot every row written, dweight / dmean_scale [width] accumulated with atomics (zeroed by the caller). */
+int dig3d_graphnorm_tangent(const float* h, const float* h_dot, const int32_t* graph_ptr, int64_t n_graphs,
+                            int32_t width, const float* weight, const float* mean_scale, const float* shift,
+                            const float* stdv, float* y_dot, void* stream);
+int dig3d_graphnorm_tangent_bwd(const float* h, const float* h_dot, const float* dy_dot, const int32_t* graph_ptr,
+                                int64_t n_graphs, int32_t width, const float* weight, const float* mean_scale,
+                                const float* shift, const float* stdv, float* dh, float* dh_dot, float* dweight,
+                                float* dmean_scale, void* stream);
 /* ---- position gradients (forces = -dE/dpos; reference run.py:126,165 takes them with torch.autograd.grad) ----
  * edge_dist_bwd: dpos[N,3] += d|pos_i - pos_j| (atomics; dpos initialised by the caller).
  * triplet_angle_bwd: dpos += d angle[t] for angle = atan2(|ji x jk|, ji.jk) (geometric_computing.py:43-48).
