@@ -584,6 +584,37 @@ def comenet_features(pos, g, cutoff, f1, f2):
     return _ComenetFeatures.apply(pos, g, cutoff, f1, f2)
 
 
+class _ComenetOcpFeatures(torch.autograd.Function):
+    """ComENet-OCP's feature1 [E,12] / feature2 [E,6] (target-sorted edge order) as functions of pos and cell: the values
+    the energy-only forward computes, bit for bit; backward = ops.comenet_ocp_features_bwd for dpos and, through its
+    dvec, ops.pbc_cell_bwd for dcell (csrc/comenet.cu, deterministic).  First order only in the cell."""
+
+    @staticmethod
+    def forward(ctx, pos, cell, gv, cutoff, f1, f2):
+        ctx.gv, ctx.cutoff = gv, cutoff
+        ctx.set_materialize_grads(False)
+        return f1.detach(), f2.detach()
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, df1, df2):
+        gv = ctx.gv
+        want_pos, want_cell = ctx.needs_input_grad[:2]
+        if (df1 is None and df2 is None) or not (want_pos or want_cell):
+            return (None,) * 6
+        e, dev = gv.n_edges, gv.vec.device
+        df1 = torch.zeros(e, 12, dtype=torch.float32, device=dev) if df1 is None else _c(df1)
+        df2 = torch.zeros(e, 6, dtype=torch.float32, device=dev) if df2 is None else _c(df2)
+        dpos, dvec = ops.comenet_ocp_features_bwd(gv, ctx.cutoff, df1, df2)
+        dcell = ops.pbc_cell_bwd(dvec, gv.cell_offsets, gv.row_ptr, gv.graph_ptr, gv.n_graphs) if want_cell else None
+        return (dpos if want_pos else None), dcell, None, None, None, None
+
+
+def comenet_ocp_features(pos, cell, gv, cutoff, f1, f2):
+    """(f1, f2) of ComENet-OCP's geometry over the graph view gv, differentiable in pos and cell."""
+    return _ComenetOcpFeatures.apply(pos, cell, gv, cutoff, f1, f2)
+
+
 def schnet_edge_features(dist, offset, coeff, cutoff):
     return _SchnetEdgeFeatures.apply(dist, offset, coeff, cutoff)
 

@@ -228,15 +228,35 @@ struct ComenetEdgePartials {
   // cross products whose two operands are the same edge vector (derivative exactly zero, see above)
   bool pl1_0, pl2_0, c2_0, q1_0, q2_0, c3_0;
 };
+// Whether the edge vectors v1 (edge e1) and v2 (edge e2) lie on one line as functions of the inputs, so that their cross
+// product is identically zero: the same edge, or -- FROM_VEC, periodic images -- two self-image edges of one atom
+// (row == col: vec = offset . cell) whose vectors are exactly parallel (offsets o and -o, or o and 2o, which is routine
+// in a cell smaller than twice the nearest-neighbour distance).  Exactness: the products of fp32 values are exact in
+// fp64.
+__device__ __forceinline__ bool exactly_parallel(const f3 a, const f3 b) {
+  const double ax = a.x, ay = a.y, az = a.z, bx = b.x, by = b.y, bz = b.z;
+  return ay * bz == az * by && az * bx == ax * bz && ax * by == ay * bx;
+}
+template <bool FROM_VEC>
+__device__ __forceinline__ bool on_one_line(int e1, int e2, const f3 v1, const f3 v2, const int32_t* __restrict__ src,
+                                            const int32_t* __restrict__ dst) {
+  if (e1 == e2) return true;
+  if (!FROM_VEC) return false;
+  return src[e1] == dst[e1] && src[e2] == dst[e2] && dst[e1] == dst[e2] && exactly_parallel(v1, v2);
+}
+
+template <bool FROM_VEC>
 __device__ __forceinline__ ComenetEdgePartials comenet_edge_partials(const ComenetEdgeGeom& G,
-                                                                     const ComenetEdgeRefs r, int e) {
+                                                                     const ComenetEdgeRefs r, int e,
+                                                                     const int32_t* __restrict__ src,
+                                                                     const int32_t* __restrict__ dst) {
   ComenetEdgePartials P;
-  P.pl1_0 = r.e0i == e;              // pl1 = (-pji) x in0
-  P.pl2_0 = r.e1i == e;              // pl2 = (-pji) x in1
-  P.c2_0 = r.e0i == r.e1i;           // pl1 x pl2 with pl1 == pl2
-  P.q1_0 = r.jref == e;              // q1 = pji x jref
-  P.q2_0 = r.iref == e;              // q2 = pji x iref
-  P.c3_0 = r.iref == r.jref;         // q1 x q2 with q1 == q2
+  P.pl1_0 = on_one_line<FROM_VEC>(r.e0i, e, G.in0, G.pji, src, dst);        // pl1 = (-pji) x in0
+  P.pl2_0 = on_one_line<FROM_VEC>(r.e1i, e, G.in1, G.pji, src, dst);        // pl2 = (-pji) x in1
+  P.c2_0 = on_one_line<FROM_VEC>(r.e0i, r.e1i, G.in0, G.in1, src, dst);     // pl1 x pl2 with pl1 || pl2
+  P.q1_0 = on_one_line<FROM_VEC>(r.jref, e, G.jref, G.pji, src, dst);       // q1 = pji x jref
+  P.q2_0 = on_one_line<FROM_VEC>(r.iref, e, G.iref, G.pji, src, dst);       // q2 = pji x iref
+  P.c3_0 = on_one_line<FROM_VEC>(r.iref, r.jref, G.iref, G.jref, src, dst); // q1 x q2 with q1 || q2
   atan2_partials(G.b1, G.a1, P.th_b1, P.th_a1);
   atan2_partials(__fdiv_rn(G.s2, G.d), G.a2, P.ph_b2, P.ph_a2);
   atan2_partials(__fdiv_rn(G.s3, G.d), G.a3, P.ta_b3, P.ta_a3);
@@ -260,7 +280,9 @@ __device__ __forceinline__ void comenet_edge_basis(float x, const ComenetEdgeGeo
 }
 
 // Pass 1: per edge e, d(loss)/d(edge vector) of the five vectors its angles read, written to work[e][role][3] with
-// roles 0 = pji (e itself), 1 = in0 (e0i), 2 = in1 (e1i), 3 = iref, 4 = jref.
+// roles 0 = pji (e itself), 1 = in0 (e0i), 2 = in1 (e1i), 3 = iref, 4 = jref.  FROM_VEC: the OCP variant, the edge
+// vectors read from `pos` = vec [E, 3] (see edge_vec).
+template <bool FROM_VEC>
 __global__ void comenet_features_bwd_edge_kernel(const float* __restrict__ pos, const float* __restrict__ dist,
                                                  const int32_t* __restrict__ src, const int32_t* __restrict__ dst,
                                                  const int32_t* __restrict__ a0_in, const int32_t* __restrict__ a1_in,
@@ -270,8 +292,8 @@ __global__ void comenet_features_bwd_edge_kernel(const float* __restrict__ pos, 
   const int e = blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= n_edges) return;
   const ComenetEdgeRefs rf = comenet_edge_refs(src, dst, a0_in, a1_in, a0_out, a1_out, e);
-  const ComenetEdgeGeom G = comenet_edge_geom<false>(pos, src, dst, e, rf);
-  const ComenetEdgePartials P = comenet_edge_partials(G, rf, e);
+  const ComenetEdgeGeom G = comenet_edge_geom<FROM_VEC>(pos, src, dst, e, rf);
+  const ComenetEdgePartials P = comenet_edge_partials<FROM_VEC>(G, rf, e, src, dst);
   ComenetEdgeBasis B;
   comenet_edge_basis(__fmul_rn(dist[e], inv_cutoff), G, B);
   // features -> d(rbf), d theta, d phi, d tau                            features.py:289-295,340-348
@@ -400,7 +422,9 @@ __global__ void comenet_features_bwd_node_kernel(const int32_t* __restrict__ row
   dpos[3 * (size_t)n] = ax; dpos[3 * (size_t)n + 1] = ay; dpos[3 * (size_t)n + 2] = az;
 }
 
-// Forward mode: f1_dot / f2_dot of every edge along the per-atom displacement cvec [N, 3]
+// Forward mode: f1_dot / f2_dot of every edge along the per-atom displacement cvec [N, 3].  FROM_VEC: the edge vectors
+// are read from `pos` = vec [E, 3]; their tangent is still cvec[src] - cvec[dst] (the cell is held fixed).
+template <bool FROM_VEC>
 __global__ void comenet_features_tangent_kernel(const float* __restrict__ pos, const float* __restrict__ dist,
                                                 const int32_t* __restrict__ src, const int32_t* __restrict__ dst,
                                                 const int32_t* __restrict__ a0_in, const int32_t* __restrict__ a1_in,
@@ -410,8 +434,8 @@ __global__ void comenet_features_tangent_kernel(const float* __restrict__ pos, c
   const int e = blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= n_edges) return;
   const ComenetEdgeRefs r = comenet_edge_refs(src, dst, a0_in, a1_in, a0_out, a1_out, e);
-  const ComenetEdgeGeom G = comenet_edge_geom<false>(pos, src, dst, e, r);
-  const ComenetEdgePartials P = comenet_edge_partials(G, r, e);
+  const ComenetEdgeGeom G = comenet_edge_geom<FROM_VEC>(pos, src, dst, e, r);
+  const ComenetEdgePartials P = comenet_edge_partials<FROM_VEC>(G, r, e, src, dst);
   ComenetEdgeBasis B;
   comenet_edge_basis(__fmul_rn(dist[e], inv_cutoff), G, B);
   const f3 zero = {0.f, 0.f, 0.f};
@@ -479,6 +503,40 @@ __global__ void pbc_edge_vectors_kernel(const float* __restrict__ pos, const int
   v.z = __fadd_rn(v.z, __fmaf_rn(o2, c[8], __fmaf_rn(o1, c[5], __fmul_rn(o0, c[2]))));
   vec[3 * (size_t)e] = v.x; vec[3 * (size_t)e + 1] = v.y; vec[3 * (size_t)e + 2] = v.z;
   dist[e] = norm3_aten(v);
+}
+
+// The cell term of the kernel above: dcell[g][a][b] = sum over graph g's edges of cell_offsets[e][a] * dvec[e][b].  One
+// CTA per graph over its contiguous edge range (target-sorted order); each thread sums a fixed stride of edges, then a
+// fixed shared-memory tree: no float atomics, the same bits run to run.
+constexpr int CELL_BWD_THREADS = 256;
+__global__ void __launch_bounds__(CELL_BWD_THREADS)
+pbc_cell_bwd_kernel(const float* __restrict__ dvec, const float* __restrict__ cell_offsets,
+                    const int32_t* __restrict__ row_ptr, const int32_t* __restrict__ graph_ptr,
+                    float* __restrict__ dcell) {
+  __shared__ float red[9][CELL_BWD_THREADS];
+  const int g = blockIdx.x, t = threadIdx.x;
+  const int lo = row_ptr[graph_ptr[g]], hi = row_ptr[graph_ptr[g + 1]];
+  float acc[9];
+#pragma unroll
+  for (int k = 0; k < 9; ++k) acc[k] = 0.f;
+  for (int e = lo + t; e < hi; e += CELL_BWD_THREADS) {
+    const f3 o = load3(cell_offsets, e), d = load3(dvec, e);
+    const float oa[3] = {o.x, o.y, o.z}, db[3] = {d.x, d.y, d.z};
+#pragma unroll
+    for (int a = 0; a < 3; ++a)
+#pragma unroll
+      for (int b = 0; b < 3; ++b) acc[3 * a + b] = fmaf(oa[a], db[b], acc[3 * a + b]);
+  }
+#pragma unroll
+  for (int k = 0; k < 9; ++k) red[k][t] = acc[k];
+  __syncthreads();
+  for (int s = CELL_BWD_THREADS / 2; s > 0; s >>= 1) {
+    if (t < s)
+#pragma unroll
+      for (int k = 0; k < 9; ++k) red[k][t] += red[k][t + s];
+    __syncthreads();
+  }
+  if (t < 9) dcell[(size_t)g * 9 + t] = red[t][0];
 }
 
 // scatter_min + argmin over an UNSORTED index (comenet-ocp.py:374-399) as a 64-bit atomicMin of
@@ -872,20 +930,22 @@ int dig3d_comenet_geometry(const float* pos, const float* dist, const int32_t* s
   return DIG3D_OK;
 }
 
-int dig3d_comenet_features_bwd(const float* pos, const float* dist, const int32_t* src, const int32_t* dst,
-                               const int32_t* row_ptr, const int32_t* out_ptr, const int32_t* out_list,
-                               const int32_t* refs, int64_t n_nodes, int64_t n_edges, double cutoff,
-                               const float* dfeature1, const float* dfeature2, float* work, float* dpos,
-                               void* stream) {
-  DIG3D_REQUIRE(pos && dist && src && dst && row_ptr && out_ptr && out_list && refs && dfeature1 && dfeature2 &&
-                    work && dpos, "comenet_features_bwd: null pointer");
+}  // extern "C"
+
+// The three passes of the features backward (pos [N,3], or FROM_VEC: vec [E,3]) and the tangent kernel's launch
+template <bool FROM_VEC>
+static int comenet_features_bwd_launch(const float* pos, const float* dist, const int32_t* src, const int32_t* dst,
+                                       const int32_t* row_ptr, const int32_t* out_ptr, const int32_t* out_list,
+                                       const int32_t* refs, int64_t n_nodes, int64_t n_edges, double cutoff,
+                                       const float* dfeature1, const float* dfeature2, float* work, float* dpos,
+                                       void* stream) {
   if (n_nodes == 0) return DIG3D_OK;
   cudaStream_t st = (cudaStream_t)stream;
   const int32_t* a0i = refs; const int32_t* a1i = refs + n_nodes;
   const int32_t* a0o = refs + 2 * n_nodes; const int32_t* a1o = refs + 3 * n_nodes;
   float* dvec = work + 15 * n_edges;
   if (n_edges) {
-    comenet_features_bwd_edge_kernel<<<ceil_div(n_edges, 128), 128, 0, st>>>(
+    comenet_features_bwd_edge_kernel<FROM_VEC><<<ceil_div(n_edges, 128), 128, 0, st>>>(
         pos, dist, src, dst, a0i, a1i, a0o, a1o, (int)n_edges, 1.0f / (float)cutoff, dfeature1, dfeature2, work);
     DIG3D_LAUNCH_CHECK();
     comenet_features_bwd_gather_kernel<<<ceil_div(n_edges, 128), 128, 0, st>>>(
@@ -898,15 +958,66 @@ int dig3d_comenet_features_bwd(const float* pos, const float* dist, const int32_
   return DIG3D_OK;
 }
 
+template <bool FROM_VEC>
+static int comenet_features_tangent_launch(const float* pos, const float* dist, const int32_t* src, const int32_t* dst,
+                                           const int32_t* refs, int64_t n_nodes, int64_t n_edges, double cutoff,
+                                           const float* cvec, float* feature1_dot, float* feature2_dot, void* stream) {
+  if (n_nodes == 0 || n_edges == 0) return DIG3D_OK;
+  comenet_features_tangent_kernel<FROM_VEC><<<ceil_div(n_edges, 128), 128, 0, (cudaStream_t)stream>>>(
+      pos, dist, src, dst, refs, refs + n_nodes, refs + 2 * n_nodes, refs + 3 * n_nodes, (int)n_edges,
+      1.0f / (float)cutoff, cvec, feature1_dot, feature2_dot);
+  DIG3D_LAUNCH_CHECK();
+  return DIG3D_OK;
+}
+
+extern "C" {
+
+int dig3d_comenet_features_bwd(const float* pos, const float* dist, const int32_t* src, const int32_t* dst,
+                               const int32_t* row_ptr, const int32_t* out_ptr, const int32_t* out_list,
+                               const int32_t* refs, int64_t n_nodes, int64_t n_edges, double cutoff,
+                               const float* dfeature1, const float* dfeature2, float* work, float* dpos,
+                               void* stream) {
+  DIG3D_REQUIRE(pos && dist && src && dst && row_ptr && out_ptr && out_list && refs && dfeature1 && dfeature2 &&
+                    work && dpos, "comenet_features_bwd: null pointer");
+  return comenet_features_bwd_launch<false>(pos, dist, src, dst, row_ptr, out_ptr, out_list, refs, n_nodes, n_edges,
+                                            cutoff, dfeature1, dfeature2, work, dpos, stream);
+}
+
 int dig3d_comenet_features_tangent(const float* pos, const float* dist, const int32_t* src, const int32_t* dst,
                                    const int32_t* refs, int64_t n_nodes, int64_t n_edges, double cutoff,
                                    const float* cvec, float* feature1_dot, float* feature2_dot, void* stream) {
   DIG3D_REQUIRE(pos && dist && src && dst && refs && cvec && feature1_dot && feature2_dot,
                 "comenet_features_tangent: null pointer");
-  if (n_nodes == 0 || n_edges == 0) return DIG3D_OK;
-  comenet_features_tangent_kernel<<<ceil_div(n_edges, 128), 128, 0, (cudaStream_t)stream>>>(
-      pos, dist, src, dst, refs, refs + n_nodes, refs + 2 * n_nodes, refs + 3 * n_nodes, (int)n_edges,
-      1.0f / (float)cutoff, cvec, feature1_dot, feature2_dot);
+  return comenet_features_tangent_launch<false>(pos, dist, src, dst, refs, n_nodes, n_edges, cutoff, cvec,
+                                                feature1_dot, feature2_dot, stream);
+}
+
+int dig3d_comenet_features_bwd_vec(const float* vec, const float* dist, const int32_t* src, const int32_t* dst,
+                                   const int32_t* row_ptr, const int32_t* out_ptr, const int32_t* out_list,
+                                   const int32_t* refs, int64_t n_nodes, int64_t n_edges, double cutoff,
+                                   const float* dfeature1, const float* dfeature2, float* work, float* dpos,
+                                   void* stream) {
+  DIG3D_REQUIRE(vec && dist && src && dst && row_ptr && out_ptr && out_list && refs && dfeature1 && dfeature2 &&
+                    work && dpos, "comenet_features_bwd_vec: null pointer");
+  return comenet_features_bwd_launch<true>(vec, dist, src, dst, row_ptr, out_ptr, out_list, refs, n_nodes, n_edges,
+                                           cutoff, dfeature1, dfeature2, work, dpos, stream);
+}
+
+int dig3d_comenet_features_tangent_vec(const float* vec, const float* dist, const int32_t* src, const int32_t* dst,
+                                       const int32_t* refs, int64_t n_nodes, int64_t n_edges, double cutoff,
+                                       const float* cvec, float* feature1_dot, float* feature2_dot, void* stream) {
+  DIG3D_REQUIRE(vec && dist && src && dst && refs && cvec && feature1_dot && feature2_dot,
+                "comenet_features_tangent_vec: null pointer");
+  return comenet_features_tangent_launch<true>(vec, dist, src, dst, refs, n_nodes, n_edges, cutoff, cvec,
+                                               feature1_dot, feature2_dot, stream);
+}
+
+int dig3d_pbc_cell_bwd(const float* dvec, const float* cell_offsets, const int32_t* row_ptr, const int32_t* graph_ptr,
+                       int64_t n_graphs, float* dcell, void* stream) {
+  DIG3D_REQUIRE(dvec && cell_offsets && row_ptr && graph_ptr && dcell, "pbc_cell_bwd: null pointer");
+  if (n_graphs == 0) return DIG3D_OK;
+  pbc_cell_bwd_kernel<<<(int)n_graphs, CELL_BWD_THREADS, 0, (cudaStream_t)stream>>>(dvec, cell_offsets, row_ptr,
+                                                                                     graph_ptr, dcell);
   DIG3D_LAUNCH_CHECK();
   return DIG3D_OK;
 }

@@ -565,6 +565,50 @@ def comenet_features_tangent(g, pos, cutoff, cvec):
     return f1d, f2d
 
 
+def comenet_ocp_features_bwd(gv, cutoff, df1, df2):
+    """ComENet-OCP: (dpos [N, 3], dvec [E, 3]) = d loss / d pos and d loss / d(distance vector) through the features of
+    dig3d_comenet_geometry_edges, given their gradients df1 [E,12] / df2 [E,6] in the target-sorted edge order of the
+    graph view `gv` (comenet_ocp.ComENet._edge_geometry: vec, dist, src, dst, row_ptr, out_ptr, out_list, refs in that
+    order).  Deterministic (no float atomics)."""
+    e, n = gv.n_edges, gv.n_nodes
+    dev = gv.vec.device
+    if e == 0:
+        return torch.zeros(n, 3, dtype=F32, device=dev), torch.zeros(0, 3, dtype=F32, device=dev)
+    dpos = torch.empty(n, 3, dtype=F32, device=dev)
+    work = torch.empty(18 * e, dtype=F32, device=dev)
+    if n:
+        call("dig3d_comenet_features_bwd_vec", _p(gv.vec, F32, "vec"), _p(gv.dist), _p(gv.src), _p(gv.dst),
+             _p(gv.row_ptr), _p(gv.out_ptr), _p(gv.out_list), _p(gv.refs), n, e, float(cutoff), _p(df1, F32, "df1"),
+             _p(df2, F32, "df2"), _p(work), _p(dpos), _stream())
+    return dpos, work[15 * e:18 * e].view(e, 3)
+
+
+def comenet_ocp_features_tangent(gv, cutoff, cvec):
+    """(feature1_dot [E,12], feature2_dot [E,6]) of ComENet-OCP along the per-atom displacement cvec [N, 3], the cell held
+    fixed, in the graph view's target-sorted edge order."""
+    e, n = gv.n_edges, gv.n_nodes
+    dev = gv.vec.device
+    f1d = torch.empty(max(e, 1), 12, dtype=F32, device=dev)[:e]
+    f2d = torch.empty(max(e, 1), 6, dtype=F32, device=dev)[:e]
+    if e:
+        call("dig3d_comenet_features_tangent_vec", _p(gv.vec, F32, "vec"), _p(gv.dist), _p(gv.src), _p(gv.dst),
+             _p(gv.refs), n, e, float(cutoff), _p(cvec, F32, "cvec"), _p(f1d), _p(f2d), _stream())
+    return f1d, f2d
+
+
+def pbc_cell_bwd(dvec, cell_offsets, row_ptr, graph_ptr, n_graphs):
+    """dcell [G, 3, 3] = sum over each graph's edges of cell_offsets[e]^T dvec[e] (the cell term of get_pbc_distances'
+    distance_vec = pos[row] - pos[col] + cell_offsets . cell); edges in target-sorted order, graph g's edges
+    row_ptr[graph_ptr[g]] .. row_ptr[graph_ptr[g + 1]].  Deterministic (no float atomics)."""
+    if dvec.numel() == 0:
+        return torch.zeros(n_graphs, 3, 3, dtype=F32, device=dvec.device)
+    dcell = torch.empty(n_graphs, 3, 3, dtype=F32, device=dvec.device)
+    if n_graphs:
+        call("dig3d_pbc_cell_bwd", _p(dvec, F32, "dvec"), _p(cell_offsets, F32, "cell_offsets"), _p(row_ptr),
+             _p(graph_ptr), n_graphs, _p(dcell), _stream())
+    return dcell
+
+
 def comenet_embed(z, emb_weight):
     n = z.numel()
     x = torch.empty(n, emb_weight.size(1), dtype=torch.float32, device=emb_weight.device)

@@ -133,6 +133,75 @@ class SimpleInteractionBlock(nn.Module):
             m.reset_parameters()
 
 
+# ---------------------------------------------------------------------- the block sequence over a graph view
+# ComENet and ComENet-OCP (comenet_ocp.py) run the same op sequence after their geometry: the embedding, the interaction
+# blocks (reference comenet.py:195-215, comenet-ocp.py:241-266) and the output head.  The functions below take the model
+# (emb, interaction_blocks, lins, lin_out) and a graph view with src / dst / row_ptr (edges sorted by target), graph_ptr
+# and batch, so that both classes share one differentiable loop and one dual loop.
+def comenet_energy(model, z, g, f1, f2):
+    """Differentiable forward (reference comenet.py:386-399 and SimpleInteractionBlock.forward :195-215, op for op) over
+    dig_b200.autograd's primitives; the geometry features f1 / f2 carry no parameters."""
+    swish_, lin = ag.swish, ag.lin
+    x = swish_(ag.gather_rows(model.emb.emb.weight, z))                    # comenet.py:125-127
+    for blk in model.interaction_blocks:
+        x = ag.lin_swish(blk.lin, x)
+        hs = []
+        for conv, lf, l, feat in ((blk.conv1, blk.lin_feature1, blk.lin1, f1),
+                                  (blk.conv2, blk.lin_feature2, blk.lin2, f2)):
+            w = lin(lf.lin2, lin(lf.lin1, feat))                            # TwoLayerLinear, no bias / act
+            agg = ag.segment_sum(ag.mul(w, ag.gather_rows(x, g.src)), g.row_ptr, g.dst)     # GraphConv, aggr='add'
+            h = ag.add(lin(conv.lin_rel, agg), lin(conv.lin_root, x))
+            hs.append(ag.lin_swish(l, h))
+        h = ag.add(lin(blk.lin_cat, torch.cat(hs, 1)), x)
+        for l in blk.lins:
+            h = ag.add(ag.lin_swish(l, h), h)
+        h = ag.graphnorm(h, blk.norm, g.graph_ptr)
+        x = lin(blk.final, h)
+    for l in model.lins:
+        x = ag.lin_swish(l, x)
+    x = lin(model.lin_out, x)
+    return ag.segment_sum(x, g.graph_ptr, g.batch)
+
+
+def comenet_energy_dual(model, z, g, f1, f2, f1d, f2d):
+    """(E, E_dot): comenet_energy op for op, carried with its directional derivative given the feature tangents f1d / f2d
+    (along a per-atom displacement), on the first-order primitives so that E_dot is differentiable in the parameters
+    (autograd_jvp.py).  The features and their tangents carry no parameters: constants here; the embedding rows carry
+    no tangent."""
+    lin, lsd, addd = jv.lin_dual, jv.lin_swish_dual, jv.add_dual
+    x, xd = ag.swish(ag.gather_rows(model.emb.emb.weight, z)), None                 # comenet.py:125-127
+    for blk in model.interaction_blocks:                                            # comenet.py:195-215
+        x, xd = lsd(blk.lin, x, xd)
+        hs = []
+        for conv, lf, l, feat, feat_d in ((blk.conv1, blk.lin_feature1, blk.lin1, f1, f1d),
+                                          (blk.conv2, blk.lin_feature2, blk.lin2, f2, f2d)):
+            w, wd = lin(lf.lin2, *lin(lf.lin1, feat, feat_d))
+            m, md = jv.mul_dual(w, wd, *jv.gather_rows_dual(x, xd, g.src))
+            agg, agg_d = jv.segment_sum_dual(m, md, g.row_ptr, g.dst)
+            h, hd = addd(*lin(conv.lin_rel, agg, agg_d), *lin(conv.lin_root, x, xd))
+            hs.append(lsd(l, h, hd))
+        cat = torch.cat([hs[0][0], hs[1][0]], 1)                                     # copies only
+        cat_d = torch.cat([hs[0][1], hs[1][1]], 1)
+        h, hd = addd(*lin(blk.lin_cat, cat, cat_d), x, xd)
+        for l in blk.lins:
+            h, hd = addd(*lsd(l, h, hd), h, hd)
+        h, hd = jv.graphnorm_dual(h, hd, blk.norm, g.graph_ptr)
+        x, xd = lin(blk.final, h, hd)
+    for l in model.lins:
+        x, xd = lsd(l, x, xd)
+    x, xd = lin(model.lin_out, x, xd)
+    return jv.segment_sum_dual(x, xd, g.graph_ptr, g.batch)
+
+
+def exact_backward(fn, *args):
+    """Run fn with the input-gradient GEMMs of the recorded graph kept exact (graphs that carry forces)."""
+    ag.EXACT_BACKWARD[0] = True
+    try:
+        return fn(*args)
+    finally:
+        ag.EXACT_BACKWARD[0] = False
+
+
 class ComENet(nn.Module):
     r"""Drop-in for dig.threedgraph.method.ComENet (same constructor arguments and defaults, in the same order).
     The fused inference kernels are compiled for hidden_channels=256, middle_channels=64 and <= 8 output layers; other
@@ -366,67 +435,14 @@ class ComENet(nn.Module):
         return u
 
     def _forward_train(self, z, g, f1, f2):
-        """Differentiable forward (reference comenet.py:386-399 and SimpleInteractionBlock.forward :195-215, op for op)
-        over dig_b200.autograd's primitives; the geometry features f1 / f2 carry no parameters."""
-        swish_, lin = ag.swish, ag.lin
-        x = swish_(ag.gather_rows(self.emb.emb.weight, z))                     # comenet.py:125-127
-        for blk in self.interaction_blocks:
-            x = ag.lin_swish(blk.lin, x)
-            hs = []
-            for conv, lf, l, feat in ((blk.conv1, blk.lin_feature1, blk.lin1, f1),
-                                      (blk.conv2, blk.lin_feature2, blk.lin2, f2)):
-                w = lin(lf.lin2, lin(lf.lin1, feat))                            # TwoLayerLinear, no bias / act
-                agg = ag.segment_sum(ag.mul(w, ag.gather_rows(x, g.src)), g.row_ptr, g.dst)     # GraphConv, aggr='add'
-                h = ag.add(lin(conv.lin_rel, agg), lin(conv.lin_root, x))
-                hs.append(ag.lin_swish(l, h))
-            h = ag.add(lin(blk.lin_cat, torch.cat(hs, 1)), x)
-            for l in blk.lins:
-                h = ag.add(ag.lin_swish(l, h), h)
-            h = ag.graphnorm(h, blk.norm, g.graph_ptr)
-            x = lin(blk.final, h)
-        for l in self.lins:
-            x = ag.lin_swish(l, x)
-        x = lin(self.lin_out, x)
-        return ag.segment_sum(x, g.graph_ptr, g.batch)
+        return comenet_energy(self, z, g, f1, f2)
 
-    @staticmethod
-    def _exact(fn, *args):
-        """Run fn with the input-gradient GEMMs of the recorded graph kept exact (graphs that carry forces)."""
-        ag.EXACT_BACKWARD[0] = True
-        try:
-            return fn(*args)
-        finally:
-            ag.EXACT_BACKWARD[0] = False
+    _exact = staticmethod(exact_backward)
 
     def _forward_dual(self, z, g, pos, cvec, f1, f2):
-        """(E, E_dot): _forward_train op for op, carried with its directional derivative along the per-atom displacement
-        cvec [N, 3], on the first-order primitives so that E_dot is differentiable in the parameters (autograd_jvp.py).
-        The features and their tangents (ops.comenet_features_tangent) carry no parameters: constants here; the
-        embedding rows carry no tangent."""
-        f1d, f2d = ops.comenet_features_tangent(g, pos.detach(), self.cutoff, cvec)
-        lin, lsd, addd = jv.lin_dual, jv.lin_swish_dual, jv.add_dual
-        x, xd = ag.swish(ag.gather_rows(self.emb.emb.weight, z)), None                  # comenet.py:125-127
-        for blk in self.interaction_blocks:                                             # comenet.py:195-215
-            x, xd = lsd(blk.lin, x, xd)
-            hs = []
-            for conv, lf, l, feat, feat_d in ((blk.conv1, blk.lin_feature1, blk.lin1, f1, f1d),
-                                              (blk.conv2, blk.lin_feature2, blk.lin2, f2, f2d)):
-                w, wd = lin(lf.lin2, *lin(lf.lin1, feat, feat_d))
-                m, md = jv.mul_dual(w, wd, *jv.gather_rows_dual(x, xd, g.src))
-                agg, agg_d = jv.segment_sum_dual(m, md, g.row_ptr, g.dst)
-                h, hd = addd(*lin(conv.lin_rel, agg, agg_d), *lin(conv.lin_root, x, xd))
-                hs.append(lsd(l, h, hd))
-            cat = torch.cat([hs[0][0], hs[1][0]], 1)                                     # copies only
-            cat_d = torch.cat([hs[0][1], hs[1][1]], 1)
-            h, hd = addd(*lin(blk.lin_cat, cat, cat_d), x, xd)
-            for l in blk.lins:
-                h, hd = addd(*lsd(l, h, hd), h, hd)
-            h, hd = jv.graphnorm_dual(h, hd, blk.norm, g.graph_ptr)
-            x, xd = lin(blk.final, h, hd)
-        for l in self.lins:
-            x, xd = lsd(l, x, xd)
-        x, xd = lin(self.lin_out, x, xd)
-        return jv.segment_sum_dual(x, xd, g.graph_ptr, g.batch)
+        """(E, E_dot) along the per-atom displacement cvec [N, 3] (comenet_energy_dual); the feature tangents come from
+        ops.comenet_features_tangent."""
+        return comenet_energy_dual(self, z, g, f1, f2, *ops.comenet_features_tangent(g, pos.detach(), self.cutoff, cvec))
 
     def forward(self, batch_data):
         if self.energy_and_force:

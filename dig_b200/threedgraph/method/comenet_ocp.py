@@ -11,16 +11,24 @@ cell, natoms`: the periodic graph is built on the GPU (radius_graph_pbc, cap 50)
 Kernels: radius_graph_pbc -> dig3d_radius_graph_pbc_count / _fill; get_pbc_distances -> dig3d_pbc_edge_vectors; the four scatter_min / argmin over the unsorted edge list and the
 angle / basis features -> dig3d_comenet_geometry_edges; the interaction blocks run on the generic CUDA primitives of
 dig_b200.autograd (forward and backward), with the edges re-ordered by target once (stable: a segmented sum instead of
-atomics).  There is no fused block kernel for this variant yet (the fused ComENet block is compiled for middle = 64)."""
+atomics).  There is no fused block kernel for this variant yet (the fused ComENet block is compiled for middle = 64).
+The block sequence is comenet.comenet_energy / comenet_energy_dual, shared with the molecular model.
+
+Forces and cell gradients: dig3d_comenet_features_bwd_vec / _tangent_vec differentiate the features in the distance
+vectors on the target-sorted edges, dig3d_pbc_cell_bwd sums the cell term per structure (ag.comenet_ocp_features)."""
+from types import SimpleNamespace
+
 import torch
 from torch import nn
 
 from ... import autograd as ag
+from ... import autograd_jvp as jv
 from ... import ops
 from ...ops import _p, _stream, call
 from ..utils.pbc import radius_graph_pbc
 from ._common import require_cuda
-from .comenet import EdgeGraphConv, EmbeddingBlock, GraphNorm, Linear
+from .comenet import (EdgeGraphConv, EmbeddingBlock, GraphNorm, Linear, comenet_energy, comenet_energy_dual,
+                      exact_backward)
 
 
 class HeteroLinear(nn.Module):
@@ -78,7 +86,14 @@ class SimpleInteractionBlock(nn.Module):
 
 
 class ComENet(nn.Module):
-    r"""Drop-in for the `comenet` model of reference comenet-ocp.py:269-484 (registered with the OCP registry there)."""
+    r"""Drop-in for the `comenet` model of reference comenet-ocp.py:269-484 (registered with the OCP registry there).
+
+    Forces and cell gradients are taken the reference's way, from the energy: with `data.pos.requires_grad_()`,
+    `F = -torch.autograd.grad(E.sum(), data.pos)[0]`; with `data.cell.requires_grad_()`, `grad(E.sum(), data.cell)` is
+    dE/dcell [G, 3, 3] (from which a stress is built).  The energy is bit for bit the energy-only forward's; the geometry
+    and cell kernels have no float atomics.  In training mode, `grad(E, pos, create_graph=True)` is differentiable in
+    the parameters (training on forces); that path refuses a cell that requires grad (no second order in the cell).
+    `regress_forces=True` stays refused: the reference returns no forces with it either."""
 
     def __init__(self, num_atoms, bond_feat_dim, num_targets=1, otf_graph=False, use_pbc=True, regress_forces=False,
                  hidden_channels=128, num_blocks=4, num_radial=32, num_spherical=7, cutoff=6.0, num_output_layers=3,
@@ -127,8 +142,16 @@ class ComENet(nn.Module):
 
     # ------------------------------------------------------------------ geometry
     def _geometry(self, data):
+        """(src, dst, row_ptr, feature1, feature2) in the target-sorted edge order (see _edge_geometry)."""
+        gv, f1, f2 = self._edge_geometry(data)
+        return gv.src, gv.dst, gv.row_ptr, f1, f2
+
+    def _edge_geometry(self, data, forces=False):
         """get_pbc_distances (zero-length edges dropped) + reference atoms + features; everything returned in an edge
-        order sorted by target (stable), which is what the segmented sums of the blocks need."""
+        order sorted by target (stable), which is what the segmented sums of the blocks need.  Returns a graph view
+        (src, dst, row_ptr, n_nodes, n_edges) and the features.  forces=True adds what the force kernels read, permuted
+        to that order: vec / dist / cell_offsets, the reference atoms with every edge id renamed to its sorted position,
+        and the out-edge lists by source."""
         pos, ei = data.pos, data.edge_index
         dev = pos.device
         e = ei.size(1)
@@ -140,13 +163,14 @@ class ComENet(nn.Module):
             raise ValueError("ComENet-OCP: sum(neighbors) must equal the number of edges")
         vec = torch.empty(e, 3, dtype=torch.float32, device=dev)
         dist = torch.empty(e, dtype=torch.float32, device=dev)
+        offsets = data.cell_offsets.to(torch.float32).contiguous()
         call("dig3d_pbc_edge_vectors", _p(pos.detach(), torch.float32, "pos"), _p(ei, torch.int64, "edge_index"),
-             _p(data.cell.to(torch.float32).contiguous(), torch.float32, "cell"),
-             _p(data.cell_offsets.to(torch.float32).contiguous(), torch.float32, "cell_offsets"), _p(edge_graph), e,
-             _p(vec), _p(dist), _stream())
+             _p(data.cell.detach().to(torch.float32).contiguous(), torch.float32, "cell"),
+             _p(offsets, torch.float32, "cell_offsets"), _p(edge_graph), e, _p(vec), _p(dist), _stream())
         keep = dist != 0                                   # the reference drops zero-length (self-image) edges
         if not bool(keep.all()):                           # rare: index plumbing only
             ei, vec, dist = ei[:, keep].contiguous(), vec[keep].contiguous(), dist[keep].contiguous()
+            offsets, edge_graph = offsets[keep], edge_graph[keep]
             e = ei.size(1)
         if e and (int(ei.min()) < 0 or int(ei.max()) >= n):
             raise ValueError("ComENet-OCP: edge_index holds node ids outside [0, num_nodes)")
@@ -161,8 +185,20 @@ class ComENet(nn.Module):
         dst_s = ei[1][perm]
         row_ptr = torch.zeros(n + 1, dtype=torch.int32, device=dev)
         row_ptr[1:] = torch.cumsum(torch.bincount(dst_s, minlength=n), 0).to(torch.int32)
-        return (ei[0][perm].to(torch.int32).contiguous(), dst_s.to(torch.int32).contiguous(), row_ptr,
-                f1[perm].contiguous(), f2[perm].contiguous())
+        gv = SimpleNamespace(src=ei[0][perm].to(torch.int32).contiguous(), dst=dst_s.to(torch.int32).contiguous(),
+                             row_ptr=row_ptr, n_nodes=n, n_edges=e)
+        if forces:
+            # the force kernels run on the sorted order too: the refs only change names, so the features, the tie rule
+            # (first edge in the original order) and the derivatives are those of the forward
+            inv = torch.empty(e, dtype=torch.int32, device=dev)
+            inv[perm] = torch.arange(e, dtype=torch.int32, device=dev)
+            gv.refs = inv[refs[:4 * n].long()].contiguous() if e else torch.zeros(4 * n, dtype=torch.int32, device=dev)
+            gv.vec, gv.dist = vec[perm].contiguous(), dist[perm].contiguous()
+            gv.cell_offsets, gv.edge_graph = offsets[perm].contiguous(), edge_graph[perm]
+            gv.out_list = torch.sort(gv.src, stable=True).indices.to(torch.int32)   # out-edges by source, in edge order
+            gv.out_ptr = torch.zeros(n + 1, dtype=torch.int32, device=dev)
+            gv.out_ptr[1:] = torch.cumsum(torch.bincount(gv.src, minlength=n), 0).to(torch.int32)
+        return gv, f1[perm].contiguous(), f2[perm].contiguous()
 
     # ------------------------------------------------------------------ forward
     def forward(self, data):
@@ -179,7 +215,10 @@ class ComENet(nn.Module):
              self.emb.emb.num_embeddings, _p(flags), _stream())
         if self.otf_graph:                                                   # comenet-ocp.py:343-350
             data.edge_index, data.cell_offsets, data.neighbors = radius_graph_pbc(data, self.cutoff, 50)
-        src, dst, row_ptr, f1, f2 = self._geometry(data)
+        pos, cell = data.pos, data.cell
+        wants_pos, wants_cell = pos.requires_grad, isinstance(cell, torch.Tensor) and cell.requires_grad
+        forces = torch.is_grad_enabled() and (wants_pos or wants_cell)
+        gv, f1, f2 = self._edge_geometry(data, forces=forces)
         if int(flags.item()):
             raise ValueError("ComENet-OCP: batch ids / atomic numbers out of range")
         if self.hetero:
@@ -189,26 +228,22 @@ class ComENet(nn.Module):
             raise NotImplementedError("ComENet-OCP hetero=True: the reference applies per-node tag masks to per-edge "
                                       "features (comenet-ocp.py:243) and fails for E != N; hetero=False is the shipped "
                                       "configuration")
-        swish_, lin = ag.swish, ag.lin
-
-        def tlin(module, x, act=False):          # `lin(x, tags)` of the reference with hetero=False: a plain Linear
-            return ag.lin_swish(module, x) if act else lin(module, x)
-        x = swish_(ag.gather_rows(self.emb.emb.weight, z))
-        for blk in self.interaction_blocks:                                    # comenet-ocp.py:241-266
-            x = tlin(blk.lin, x, act=True)
-            hs = []
-            for conv, lf, l, feat in ((blk.conv1, blk.lin_feature1, blk.lin1, f1),
-                                      (blk.conv2, blk.lin_feature2, blk.lin2, f2)):
-                w = lin(lf.lin2, lin(lf.lin1, feat))
-                agg = ag.segment_sum(ag.mul(w, ag.gather_rows(x, src)), row_ptr, dst)
-                h = ag.add(lin(conv.lin_rel, agg), lin(conv.lin_root, x))
-                hs.append(ag.lin_swish(l, h))
-            h = ag.add(lin(blk.lin_cat, torch.cat(hs, 1)), x)
-            for l in blk.lins:
-                h = ag.add(tlin(l, h, act=True), h)
-            h = ag.graphnorm(h, blk.norm, graph_ptr)
-            x = tlin(blk.final, h)
-        for l in self.lins:
-            x = tlin(l, x, act=True)
-        x = tlin(self.lin_out, x)
-        return ag.segment_sum(x, graph_ptr, batch)                             # energy = scatter(x, batch)  :469
+        gv.graph_ptr, gv.batch, gv.n_graphs = graph_ptr, batch, num_graphs
+        if not forces:
+            return comenet_energy(self, z, gv, f1, f2)                     # energy = scatter(x, batch)  :469
+        if wants_cell and gv.n_edges and not torch.equal(gv.edge_graph.long(), batch[gv.dst.long()]):
+            raise ValueError("ComENet-OCP: the cell gradient needs every edge in the structure of its target atom "
+                             "(neighbors must count the edges of each structure in batch order)")
+        if self.training and wants_pos and any(p.requires_grad for p in self.parameters()):
+            # training on forces: reverse over forward mode (dig_b200/autograd_jvp.py); no second order in the cell
+            if wants_cell:
+                raise NotImplementedError("ComENet-OCP: training on forces with cell.requires_grad (the cell gradient "
+                                          "differentiated again) is not implemented; detach the cell")
+            cell_c = cell.detach()
+            return jv.energy_with_force(
+                lambda p: exact_backward(comenet_energy, self, z, gv,
+                                         *ag.comenet_ocp_features(p, cell_c, gv, self.cutoff, f1, f2)),
+                lambda p, c: exact_backward(comenet_energy_dual, self, z, gv, f1, f2,
+                                            *ops.comenet_ocp_features_tangent(gv, self.cutoff, c)),
+                pos, tuple(self.parameters()))
+        return exact_backward(comenet_energy, self, z, gv, *ag.comenet_ocp_features(pos, cell, gv, self.cutoff, f1, f2))

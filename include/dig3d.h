@@ -465,6 +465,29 @@ int dig3d_comenet_geometry_edges(const float* vec, const float* dist, const int6
                                  const int32_t* dst, int64_t n_nodes, int64_t n_edges, double cutoff, int32_t* refs,
                                  unsigned long long* keys, float* feature1, float* feature2, float* angles,
                                  void* stream);
+/* Forces and cell gradients through the geometry above.  The gather and node passes of dig3d_comenet_features_bwd need
+ * CSR edge order, so these run on the edges sorted by target: vec [E,3] / dist [E] / src / dst permuted, row_ptr over
+ * the targets, out_ptr / out_list the out-edge lists by source in that order, refs [4 * N] the refs of
+ * dig3d_comenet_geometry_edges with every edge id mapped to its sorted position (the flags are not read).
+ * features_bwd_vec: dig3d_comenet_features_bwd with the edge vectors read from vec: work[15E, 18E) = dvec [E,3] =
+ * d loss / d vec, dpos [N,3] = sum over out-edges - sum over in-edges of dvec (a self-image edge cancels).  Besides one
+ * edge read twice, a cross product of two self-image edges of one atom with exactly parallel vectors (its images at +a
+ * and -a) is aliased too: identically zero as a function of the cell, derivative zero.
+ * features_tangent_vec: feature1_dot [E,12] / feature2_dot [E,6] along the per-atom displacement cvec [N,3], the cell
+ * held fixed (vec_dot[e] = cvec[src] - cvec[dst]); the transpose of features_bwd_vec's dpos.
+ * pbc_cell_bwd: dcell [G,3,3], dcell[g][a][b] = sum over the edges of graph g of cell_offsets[e][a] * dvec[e][b]; graph
+ * g's edges are [row_ptr[graph_ptr[g]], row_ptr[graph_ptr[g + 1]]) (edges grouped by the graph of their target).  One
+ * CTA per graph, a fixed-shape reduction and no float atomics: the same bits run to run. */
+int dig3d_comenet_features_bwd_vec(const float* vec, const float* dist, const int32_t* src, const int32_t* dst,
+                                   const int32_t* row_ptr, const int32_t* out_ptr, const int32_t* out_list,
+                                   const int32_t* refs, int64_t n_nodes, int64_t n_edges, double cutoff,
+                                   const float* dfeature1, const float* dfeature2, float* work, float* dpos,
+                                   void* stream);
+int dig3d_comenet_features_tangent_vec(const float* vec, const float* dist, const int32_t* src, const int32_t* dst,
+                                       const int32_t* refs, int64_t n_nodes, int64_t n_edges, double cutoff,
+                                       const float* cvec, float* feature1_dot, float* feature2_dot, void* stream);
+int dig3d_pbc_cell_bwd(const float* dvec, const float* cell_offsets, const int32_t* row_ptr, const int32_t* graph_ptr,
+                       int64_t n_graphs, float* dcell, void* stream);
 
 /* Periodic radius graph = ocpmodels' radius_graph_pbc(data, radius, max_num_neighbors) (2022), called by ComENet-OCP
  * with otf_graph=True (comenet-ocp.py:343-350).  pos [N,3], cell [B,3,3] (rows = lattice vectors), natoms [B] int64.
