@@ -210,13 +210,16 @@ __global__ void act_bwd_kernel(const float* __restrict__ x, const float* __restr
   dx[i] = dy[i] * d;
 }
 // second order: d/dx of (dy * act'(x)) contracted with g:  out = g * dy * act''(x)
-//   swish'' = s (1 - s) (2 + x (1 - 2 s)),  ssp'' = s (1 - s)
+//   swish'' = s (1 - s) (2 + x (1 - 2 s)),  ssp'' = s (1 - s)  (0 for x > 20, where the forward is the identity)
 __global__ void act_bwd2_kernel(const float* __restrict__ x, const float* __restrict__ dy, const float* __restrict__ g,
                                 int64_t n, int mode, float* __restrict__ out) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  const float v = x[i], s = sigmoid_f(v);
-  const float d2 = mode == 0 ? s * (1.0f - s) * (2.0f + v * (1.0f - 2.0f * s)) : mode == 1 ? s * (1.0f - s) : 0.0f;
+  // 1 - s as sigmoid(-x): 1.0f - s cancels as s -> 1 (17 % off at x = 15, 0 from x ~ 17)
+  const float v = x[i], s = sigmoid_f(v), sm = sigmoid_f(-v);
+  const float d2 = mode == 0   ? s * sm * (2.0f + v * (1.0f - 2.0f * s))
+                   : mode == 1 ? (v > 20.0f ? 0.0f : s * sm)
+                               : 0.0f;
   out[i] = g[i] * dy[i] * d2;
 }
 // y = a * b (b broadcast over rows when b_rows == 1 is NOT needed here: same shape), y = a + b, y = alpha * a

@@ -51,6 +51,30 @@ form, plus the rounding of the scaled argument: below 2^-20 of |t| either way (T
 Underflow: the kernels keep fp32 subnormals (no flush to zero), so a rounding below 2^-126 is off by at most half the
 subnormal spacing, 2^-150, ABSOLUTE (ETA): every op adds one ETA per rounding it counts.  It only matters where the
 values themselves are ~1e-40, e.g. the edge features of edges at the cutoff, whose envelope goes to zero.
+SchNet (csrc/schnet.cu, the training kernels of csrc/train_ops.cu / train_geom.cu).  Libdevice expf, log1pf, cosf and
+sinf are within 2 ulp (4u of the result, u = 2^-24); the products, sums and quotients round once each:
+  * ssp(t) = (t > 20 ? t : log1pf(expf(t))) - ln2_f (`ssp`): Lipschitz 1, so an input error passes unchanged.  expf's
+    4u enter log1p as 4u * e^t / (1 + e^t) = 4u sigmoid(t), log1pf adds 4u of softplus(t), the subtraction u of the
+    result.  The t > 20 branch is exact (the identity); an input error that straddles 20 may take the other branch,
+    which differs by log1p(e^-20) < 2.1e-9.  Below t = -87 e^t is subnormal or 0: absolute, and far below u * ln2.
+  * gauss = expf(c_f * (d - mu)^2) (`gauss`): the argument a = c_f ((d - mu)^2) takes three roundings, t = d - mu
+    counted twice by the square (4u relative, c_f = fp32(coeff) being what the kernel receives), which exp turns into
+    a relative error 4u |a| (magnified by |a|, up to ~1e3 for a Gaussian far from the edge), plus expf's own 4u;
+    subnormal results 4 ETA absolute (2 ulp).
+  * C = 0.5 (cosf((d pi_f) inv_f) + 1) (`cutoff_fn`): pi_f and inv_f = fp32(1/cutoff) are kernel inputs.  The
+    argument x takes two roundings (2u |x|, moved by |sin x|), cosf 4u |cos x|, the + 1 one u.  Near C = 0 (x -> pi)
+    cos x = -1 + O(C) and its 4u is an ABSOLUTE term next to C: the bound there is ~2u, not relative to C.
+  * the cfconv aggregation (schnet_cfconv_kernel's tile_segment_accumulate): per 64-edge tile a running fp32 sum over
+    each target's edges; a target whose edges cross a tile boundary gets two partial sums, added onto the zeroed row
+    by atomics (the first is exact).  With at most 64 edges per target (33 under the neighbour cap) that is c - 1
+    roundings for c in-edges, inside `index_add`'s c.
+  * act' and act'' (`act_d1`, `act_d2`): s = sigmoid_f(x) = 1 / (1 + expf(-x)) is within 6u of s (4u expf, the add,
+    the division); sm = sigmoid_f(-x) = 1 - s likewise, with no cancellation.  swish' = s (1 + x (1 - s)) evaluates
+    1.0f - s, whose error is 6u s (absolute): <= 12u s (1 + |x| (1 - s)) + 7u |x| s^2.  swish'' = s sm (2 + x (1 - 2s))
+    (1 - 2 s is exact after s): <= 17u s sm (2 + |x| |1 - 2s|) + 12u |x| s^2 sm.  ssp' = s: 6u s; ssp'' = s sm: 13u s
+    sm, and 0 for x > 20 (the forward is the identity there, as in torch's softplus with threshold 20).  For |x| > 87
+    s or sm is subnormal or 0: 2^-126 ABSOLUTE on each (SIG_FLOOR), times the factors it multiplies.  The kernel's
+    dx = dy * d and out = (g * dy) * d2 add one and two roundings.
 """
 import torch
 
@@ -231,6 +255,76 @@ def graphnorm(h, graph_ptr, weight, bias, mean_scale, eps):
     e_y = aw * e_o / sdlg + aw * o.abs() * esdg / (sdg * sdlg) + 3 * U * t_a + U * (b.abs() + t_a) + 4 * ETA
     m_y = aw * (h.m + m_sh[gid]) / sdg + b.abs()
     return Bounded(y, m_y, e_y), Bounded(sh, m_sh, e_sh), Bounded(sd, sd, e_sd)
+
+
+LN2_F = 0.693147182464599609375     # fp32(ln 2), the constant the kernels subtract
+PI_F = 3.14159274101257324           # fp32(pi)
+SIG_FLOOR = 2.0 ** -126              # sigmoid_f(x) or sigmoid_f(-x) subnormal or 0 (|x| > 87): absolute error
+
+
+def f32(x):
+    """The fp32 value the kernel receives for a host double."""
+    return float(torch.tensor(x, dtype=torch.float32))
+
+
+def ssp(x):
+    """Shifted softplus with threshold 20 (see the module docstring)."""
+    t = x.v
+    hi = t + x.e                                     # sigmoid and softplus are increasing: their largest value in reach
+    v = torch.nn.functional.softplus(t, threshold=20.0) - LN2_F
+    e = (x.e + 4 * U * torch.sigmoid(hi) + 4 * U * torch.nn.functional.softplus(hi) + U * (v.abs() + x.e)
+         + 2.1e-9 * ((t - 20.0).abs() <= x.e) + 2 * ETA)
+    return Bounded(v, x.m, e)
+
+
+def gauss(dist, offset, coeff):
+    """expf(c_f * (d - mu)^2) for exact fp32 dist [E] and offset [G] -> [E, G]."""
+    c = f32(coeff)
+    t = dist.detach().double()[:, None] - offset.detach().double()[None, :]
+    a = c * t * t
+    v = torch.exp(a)
+    rel = torch.expm1(4 * U * a.abs() + 2 * abs(c) * ETA) * (1 + 4 * U) + 4 * U
+    return Bounded(v, v, v * rel + 4 * ETA)
+
+
+def cutoff_fn(dist, cutoff):
+    """0.5 (cosf((d pi_f) inv_f) + 1) for exact fp32 dist [E], inv_f = fp32(1 / cutoff)."""
+    x = dist.detach().double() * PI_F * f32(1.0 / cutoff)
+    ex = 2 * U * x.abs() * (1 + 2 * U)
+    c = torch.cos(x)
+    e_cos = x.sin().abs() * ex + ex * ex / 2 + 4 * U * (c.abs() + ex)
+    e_sum = e_cos + U * ((c + 1).abs() + e_cos)
+    v = 0.5 * (c + 1)
+    return Bounded(v, v, 0.5 * e_sum + ETA)
+
+
+def act_d1(x, mode):
+    """act'(x) (mode 0 swish, 1 ssp, 2 relu) of exact fp32 x, as act_bwd_kernel evaluates it."""
+    x = x.detach().double()
+    s, sm, ax = torch.sigmoid(x), torch.sigmoid(-x), x.abs()
+    if mode == 0:
+        v = s * (1 + x * sm)
+        e = 12 * U * s * (1 + ax * sm) + 7 * U * ax * s * s + SIG_FLOOR * (1 + 2 * ax)
+    elif mode == 1:
+        v, e = s, 6 * U * s + SIG_FLOOR
+    else:
+        v, e = (x > 0).double(), torch.zeros_like(x)
+    return Bounded(v, v.abs(), e)
+
+
+def act_d2(x, mode):
+    """act''(x) of exact fp32 x, as act_bwd2_kernel evaluates it (ssp'' = 0 above the threshold 20)."""
+    x = x.detach().double()
+    s, sm, ax = torch.sigmoid(x), torch.sigmoid(-x), x.abs()
+    if mode == 0:
+        v = s * sm * (2 + x * (1 - 2 * s))
+        e = 17 * U * s * sm * (2 + ax * (1 - 2 * s).abs()) + 12 * U * ax * s * s * sm + SIG_FLOOR * (2 + 2 * ax)
+    elif mode == 1:
+        keep = (x <= 20).double()
+        v, e = keep * s * sm, keep * (13 * U * s * sm + SIG_FLOOR)
+    else:
+        v, e = torch.zeros_like(x), torch.zeros_like(x)
+    return Bounded(v, v.abs(), e)
 
 
 def split16(x, scale):

@@ -12,7 +12,8 @@ variance, a dropped eps and an ignored mean_scale), each emulated in fp32 in its
 import pytest
 import torch
 
-from fp64_bound import Bounded, filter_sum, fold, graphnorm, linear, split16
+from fp64_bound import (LN2_F, PI_F, U, Bounded, act_d1, act_d2, cutoff_fn, filter_sum, fold, gauss, graphnorm, linear,
+                        mul, split16, ssp)
 from helpers import rel_err
 
 ROWS, K, N = 512, 128, 128
@@ -248,3 +249,124 @@ def test_graphnorm_bound_rejects_a_wrong_kernel(fault):
     y_ref[:, cols].check(_gn_emulate(h, ptr, w, b, ms)[:, cols])
     with pytest.raises(AssertionError, match="outside the bound|non-finite"):
         y_ref[:, cols].check(y[:, cols], f"graphnorm with {fault}")
+
+
+# ------------------------------------------------------------------------------------------------ SchNet ops, act', act''
+def _ssp32(x):
+    """ssp in the kernels' fp32 order: (x > 20 ? x : log1pf(expf(x))) - fp32(ln 2)."""
+    return torch.where(x > 20, x, torch.log1p(torch.exp(x))) - torch.tensor(LN2_F)
+
+
+def _sigmoid32(x):
+    return 1.0 / (1.0 + torch.exp(-x))
+
+
+def _act_x():
+    """Dense around 0, dense over [8, 20] and around the ssp threshold, out to the expf under- / overflow at +-88."""
+    return torch.cat([torch.linspace(-100, 100, 4001), torch.linspace(-3, 3, 2001), torch.linspace(8, 20, 3001),
+                      torch.linspace(19.99, 20.01, 201)]).float()
+
+
+def test_ssp_bound_accepts_the_kernel_order():
+    """Near ssp = -ln 2 (x < -8) the subtraction's half-ulp rounding (2^-25) is the whole error and the bound u |v| is
+    0.69 u: the emulation reaches ~0.72 of it there."""
+    x = _act_x()
+    assert ssp(Bounded.exact(x)).check(_ssp32(x), "ssp") < 0.8
+
+
+def test_ssp_bound_rejects_the_unshifted_softplus():
+    x = _act_x()
+    with pytest.raises(AssertionError, match="outside the bound"):
+        ssp(Bounded.exact(x)).check(_ssp32(x) + torch.tensor(LN2_F), "softplus without the shift")
+
+
+def _d_case(n=512, cutoff=10.0, g=50, seed=6):
+    """Distances over [0, cutoff] with coincident atoms (d = 0) and pairs at 0.99 - 1.0 x cutoff; Gaussian centres of
+    the model (far ones underflow into subnormals and 0)."""
+    gen = torch.Generator().manual_seed(seed)
+    d = torch.cat([torch.zeros(2), torch.rand(n, generator=gen) * cutoff,
+                   cutoff * (0.99 + 0.01 * torch.rand(64, generator=gen)), torch.tensor([cutoff])]).float()
+    offset = torch.linspace(0.0, cutoff, g)
+    return d, offset, -0.5 / (offset[1] - offset[0]).item() ** 2
+
+
+def _gauss32(d, offset, coeff):
+    t = d[:, None] - offset[None, :]
+    return torch.exp(torch.tensor(coeff, dtype=torch.float32) * (t * t))
+
+
+def _cut32(d, cutoff):
+    x = (d * torch.tensor(PI_F, dtype=torch.float32)) * torch.tensor(1.0 / cutoff, dtype=torch.float32)
+    return 0.5 * (torch.cos(x) + 1.0)
+
+
+@pytest.mark.parametrize("g", [2, 50, 64, 70])
+def test_gauss_and_cutoff_bounds_accept_the_kernel_order(g):
+    d, offset, coeff = _d_case(g=g)
+    gs = _gauss32(d, offset, coeff)
+    assert (gs[gs > 0] < 2.0 ** -126).any() or g == 2                # subnormal Gaussians are part of the case
+    # the argument's rounding, magnified by |a|, is the whole error of a far Gaussian: the emulation (the kernel's own
+    # fp32 argument) reaches 0.9 of its worst case there
+    assert gauss(d, offset, coeff).check(gs, f"gauss G={g}") < 0.95
+    assert cutoff_fn(d, 10.0).check(_cut32(d, 10.0), "cutoff") < 0.8
+
+
+def test_gauss_bound_rejects_an_unrounded_coefficient_and_the_cutoff_bound_a_relative_model():
+    d, offset, coeff = _d_case()
+    ref = gauss(d, offset, coeff)
+    t = d.double()[:, None] - offset.double()[None, :]
+    with pytest.raises(AssertionError, match="outside the bound"):  # (coeff + 1e-4 relative): far Gaussians move
+        ref.check(torch.exp(coeff * (1 + 1e-4) * t * t).float(), "coeff off by 1e-4")
+    c = cutoff_fn(d, 10.0)
+    near = d > 9.9
+    assert (c.e[near] > 16 * U * c.v[near]).any()                    # the absolute term near C = 0
+    with pytest.raises(AssertionError, match="outside the bound"):
+        c.check(_cut32(d, 10.0 * (1 + 1e-6)), "cutoff 1e-6 off")
+
+
+def _filter(d, offset, coeff, w0, b0, w2, b2, fault=None):
+    """update_e's filter in fp32: W = (ssp(gauss @ w0^T + b0) @ w2^T + b2) * C, with a seeded fault."""
+    h = _ssp32(_gauss32(d, offset, coeff) @ w0.T + b0)
+    f = h @ w2.T + (0.0 if fault == "no_b2" else b2)
+    c = _cut32(d, 10.0)
+    w = f * c[:, None]
+    return w * c[:, None] if fault == "cutoff_twice" else w
+
+
+@pytest.mark.parametrize("fault", [None, "no_b2", "cutoff_twice"])
+def test_filter_bound_accepts_the_kernel_order_and_rejects_a_seeded_fault(fault):
+    d, offset, coeff = _d_case(g=50)
+    gen = torch.Generator().manual_seed(7)
+    a0, a2 = (6.0 / (50 + 64)) ** 0.5, (6.0 / 128) ** 0.5
+    w0 = ((torch.rand(64, 50, generator=gen) * 2 - 1) * a0 * 300).float()   # pre-activations beyond +-88
+    w2 = ((torch.rand(64, 64, generator=gen) * 2 - 1) * a2).float()
+    b0, b2 = (0.1 * (torch.rand(2, 64, generator=gen) * 2 - 1)).float()
+    pre = linear(gauss(d, offset, coeff), w0, b0, "fp32")
+    assert (pre.v > 20).any() and (pre.v < -88).any()
+    ref = mul(linear(ssp(pre), w2, b2, "fp32"), cutoff_fn(d, 10.0)[:, None])
+    y = _filter(d, offset, coeff, w0, b0, w2, b2, fault)
+    if fault is None:
+        assert ref.check(y, "filter") < 0.5
+    else:
+        with pytest.raises(AssertionError, match="outside the bound"):
+            ref.check(y, f"filter with {fault}")
+
+
+@pytest.mark.parametrize("mode", [0, 1, 2])
+def test_act_derivative_bounds_accept_the_kernel_order(mode):
+    x = _act_x()
+    s, sm = _sigmoid32(x), _sigmoid32(-x)
+    d1 = [s * (1.0 + x * (1.0 - s)), s, (x > 0).float()][mode]
+    d2 = [s * sm * (2.0 + x * (1.0 - 2.0 * s)), torch.where(x > 20, 0.0, s * sm), torch.zeros_like(x)][mode]
+    assert act_d1(x, mode).check(d1, f"act' mode {mode}") < 0.5
+    assert act_d2(x, mode).check(d2, f"act'' mode {mode}") < 0.5
+
+
+@pytest.mark.parametrize("mode", [0, 1])
+def test_act_second_derivative_bound_rejects_the_cancelling_one_minus_s(mode):
+    """1.0f - s loses every digit of 1 - s as s -> 1: the parent kernel's form at x in [10, 17]."""
+    x = torch.linspace(10, 17, 701).float()
+    s = _sigmoid32(x)
+    y = s * (1.0 - s) * (2.0 + x * (1.0 - 2.0 * s)) if mode == 0 else s * (1.0 - s)
+    with pytest.raises(AssertionError, match="outside the bound"):
+        act_d2(x, mode).check(y, f"act'' mode {mode} with 1 - s")

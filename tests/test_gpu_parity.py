@@ -302,7 +302,7 @@ def test_full_size_config_properties():
     assert rel_err(single[0].cpu().numpy(), full[5].cpu().numpy()) < 2e-6
 
 
-@pytest.mark.parametrize("hidden,layers", [(32, 2), (128, 3)])
+@pytest.mark.parametrize("hidden,layers", [(32, 2), (64, 2), (128, 3)])
 def test_schnet_parity(hidden, layers):
     """BASELINE configs[0] (SchNet 2-layer h=32, 16 x 12 atoms, cutoff 10) + the class-default width."""
     from dig_b200.threedgraph.method import SchNet
@@ -321,6 +321,25 @@ def test_schnet_parity(hidden, layers):
     assert rel_err(u.cpu().numpy(), ref.cpu().numpy()) < TOL
     if hidden == 32 and layers == 2:      # the fixture case: vs the real reference on CPU
         assert rel_err(u.cpu().numpy(), g["energy_f32"]) < TOL
+
+
+def test_schnet_parity_with_three_outputs():
+    """update_u with out_channels = 3 on the fused path: the readout's per-channel warp sums and the graph sum."""
+    from dig_b200.threedgraph.method import SchNet
+    from oracle import restated
+    dev = torch.device("cuda:0")
+    _, z, pos, batch = case_inputs("schnet_cfg1", dev)
+    model = SchNet(num_layers=2, hidden_channels=64, num_filters=64, out_channels=3, cutoff=10.0)
+    assert not model._generic
+    sd = formula_state_dict(model.state_dict(), seed=2)
+    model.load_state_dict(sd)
+    model = model.to(dev)
+    with torch.no_grad():
+        u = model(_batch(z, pos, batch))
+    ref = restated.schnet_forward({k: v.to(dev) for k, v in sd.items()}, z, pos, batch, cutoff=10.0, num_layers=2)
+    assert u.shape == (16, 3)
+    for c in range(3):
+        assert rel_err(u[:, c].cpu().numpy(), ref[:, c].cpu().numpy()) < TOL
 
 
 def _comenet_setup():

@@ -45,18 +45,67 @@ def test_linear_fwd_bwd(rows, k, nout):
         assert rel_err(a.cpu().numpy(), r.cpu().numpy()) < 2e-5
 
 
-@pytest.mark.parametrize("mode", [0, 1])
-def test_activations_fwd_bwd(mode):
+def _placed(x, aligned):
+    """x in a 16-byte aligned buffer (the float4 kernels) or in the misaligned view buf[1:] of one (the scalar ones)."""
+    buf = torch.empty(x.numel() + 4, device="cuda:0")
+    view = buf[:x.numel()] if aligned else buf[1:x.numel() + 1]
+    return view.copy_(x.to("cuda:0"))
+
+
+@pytest.mark.parametrize("aligned", [True, False])
+@pytest.mark.parametrize("mode", [0, 1, 2])
+def test_activations_fwd_bwd(mode, aligned):
+    """act / act_bwd against the fp64 bound per element (tests/fp64_bound.py: swish, ssp, act'), on n = 4000 in an
+    aligned buffer (float4 kernels) and in a misaligned view (scalar kernels); both paths give the same bits."""
     from dig_b200 import autograd as ag
-    dev = torch.device("cuda:0")
-    x = torch.linspace(-30, 30, 4001, device=dev).requires_grad_(True)
-    y = ag.swish(x) if mode == 0 else ag.ssp(x)
-    y.backward(torch.ones_like(y))
-    x2 = x.detach().double().requires_grad_(True)
-    y2 = x2 * torch.sigmoid(x2) if mode == 0 else torch.nn.functional.softplus(x2) - np.log(2.0)
-    y2.backward(torch.ones_like(y2))
-    assert (y.detach().double() - y2.detach()).abs().max().item() < 2e-6 * 30
-    assert (x.grad.double() - x2.grad).abs().max().item() < 2e-6
+    from dig_b200 import ops
+    from fp64_bound import Bounded, act_d1, mul, ssp, swish
+    gen = torch.Generator().manual_seed(mode)
+    x_c = (torch.rand(4000, generator=gen, dtype=torch.float64) * 60 - 30).float()
+    dy_c = torch.randn(4000, generator=gen).float()
+    x, dy = _placed(x_c, aligned).requires_grad_(True), _placed(dy_c, aligned)
+    y = [ag.swish, ag.ssp, ag.relu][mode](x)
+    y.backward(dy)
+    xb = Bounded.exact(x_c)
+    ref_y = [swish(xb), ssp(xb), Bounded(xb.v.clamp_min(0), xb.m, xb.e)][mode]
+    ref_y.check(y.detach().cpu(), f"act mode {mode}")
+    mul(Bounded.exact(dy_c), act_d1(x_c, mode)).check(x.grad.cpu(), f"act_bwd mode {mode}")
+    x_o, dy_o = _placed(x_c, not aligned), _placed(dy_c, not aligned)
+    assert torch.equal(ops.act(x_o, mode), y.detach())
+    assert torch.equal(ops.act_bwd(x_o, dy_o, mode), x.grad)
+
+
+def _act_bwd2_x():
+    """[-100, 100]: dense around 0, dense over [8, 20] and around the ssp threshold at 20."""
+    return torch.cat([torch.linspace(-100, 100, 20001), torch.linspace(-4, 4, 8001), torch.linspace(8, 20, 12001),
+                      torch.linspace(19.9, 20.1, 2001), torch.tensor([20.0, -88.0, 88.0, 0.0])]).float()
+
+
+@pytest.mark.parametrize("mode", [0, 1, 2])
+def test_act_bwd2_matches_fp64_double_backward(mode):
+    """out = g * dy * act''(x) against torch.autograd's double backward in fp64 (swish, softplus with threshold 20 - ln 2,
+    relu), element by element: a few ulp of the magnitude s (1 - s) (2 + |x| |1 - 2s|) of act'' plus a subnormal floor
+    (tests/fp64_bound.py, act_d2).  1 - s evaluated as 1.0f - s loses every digit of it as s -> 1 (from x ~ 8).
+    fp64's own 1 - s cancels too (beyond x ~ 25 at fp32's precision), so the reference is act_d2's closed form with
+    sigmoid(-x), held to torch's double backward within fp64's 1e-14."""
+    from dig_b200 import ops
+    from fp64_bound import Bounded, act_d2, mul
+    x = _act_bwd2_x()
+    gen = torch.Generator().manual_seed(11)
+    dy = (torch.rand(x.numel(), generator=gen) + 0.5).float()
+    g = (torch.rand(x.numel(), generator=gen) * 2 - 1).float()
+    out = ops.act_bwd2(x.to("cuda:0"), dy.to("cuda:0"), g.to("cuda:0"), mode).cpu()
+    x2 = x.double().requires_grad_(True)
+    y2 = [lambda t: t * torch.sigmoid(t), lambda t: torch.nn.functional.softplus(t, threshold=20.0) - np.log(2.0),
+          torch.relu][mode](x2)
+    (gx,) = torch.autograd.grad(y2, x2, dy.double(), create_graph=True)
+    (ref,) = torch.autograd.grad(gx, x2, g.double(), allow_unused=True) if mode != 2 else (torch.zeros_like(x2),)
+    bound = mul(mul(Bounded.exact(g), Bounded.exact(dy)), act_d2(x, mode))
+    # act_d2's closed form is torch's act''.  Except at x = 20 itself for softplus: torch's forward and first backward
+    # switch to the identity at x > 20 but its double backward masks x >= 20; the kernel follows the forward.
+    keep = x != 20.0 if mode == 1 else torch.ones_like(x, dtype=torch.bool)
+    assert torch.allclose(bound.v[keep], ref.detach()[keep], rtol=1e-9, atol=1e-14)
+    bound.check(out, f"act_bwd2 mode {mode}")
 
 
 def test_gather_scatter_segment_bwd():
