@@ -70,6 +70,9 @@ SIGNATURES = {
     "dig3d_edges_to_csr": [P, P, c_int64, c_int64, P, P, P, P, P, P, P, P],
     "dig3d_triplet_geometry": [P, P, P, P, P, c_int64, c_int32, P, P, P, P, P, P, P],
     "dig3d_triplet_geometry_any_degree": [P, P, P, P, P, c_int64, c_int64, c_int32, P, P, P, P, P, P, P, P],
+    "dig3d_triplet_geometry_any_degree_arg": [P, P, P, P, P, c_int64, c_int64, P, P, P, P, P, P, P],
+    "dig3d_triplet_torsion_bwd_arg": [P, P, P, P, P, P, P, c_int64, P, P],
+    "dig3d_triplet_geometry_bwd2": [P, P, P, P, P, P, P, P, P, c_int64, P, P, P, P],
     "dig3d_radius_graph_dense_count": [P, P, P, c_int64, c_int64, c_double, c_int64, P, P, P, P, P],
     "dig3d_radius_graph_dense_fill": [P, P, P, c_int64, c_int64, c_double, c_int64, P, c_int64, P, P, P, P],
     "dig3d_edge_basis": [P, c_int64, c_double, c_int32, P, c_int32, c_int32, P, P, P],

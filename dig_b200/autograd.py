@@ -528,7 +528,10 @@ class _Geometry(torch.autograd.Function):
         if dangle is not None:
             ops.triplet_angle_bwd(p, g, _c(dangle), dpos)
         if dtorsion is not None:
-            ops.triplet_torsion_bwd(p, g, _c(dtorsion), dpos)
+            if getattr(g, "tors_arg", None) is not None:      # xyz_to_dat's any-degree graph: the recorded candidates
+                ops.triplet_torsion_bwd_arg(p, g, _c(dtorsion), dpos)
+            else:
+                ops.triplet_torsion_bwd(p, g, _c(dtorsion), dpos)
         return dpos, None, None
 
 

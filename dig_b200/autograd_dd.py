@@ -265,6 +265,67 @@ class _Geometry(torch.autograd.Function):
         return _EdgeDistBwd.apply(pos, ddist, ctx.g), None
 
 
+class _TripletGeometryBwd(torch.autograd.Function):
+    """dpos of (ddist, dangle, dtorsion) through dist / angle / torsion (any in-degree; the torsion through g.tors_arg).
+    Its backward is triplet_geometry_bwd2 (+ edge_dist_bwd2): the JVPs of the geometry along d(loss)/d(dpos) and the
+    Hessian-vector products."""
+
+    @staticmethod
+    def forward(ctx, pos, ddist, dangle, dtorsion, g):
+        ctx.g = g
+        pos = _c(pos.detach())
+        ddist, dangle, dtorsion = (None if x is None else _c(x) for x in (ddist, dangle, dtorsion))
+        ctx.save_for_backward(pos, ddist, dangle, dtorsion)
+        dpos = torch.zeros_like(pos)
+        if ddist is not None:
+            ops.edge_dist_bwd(pos, g, ddist, dpos)
+        if dangle is not None:
+            ops.triplet_angle_bwd(pos, g, dangle, dpos)
+        if dtorsion is not None:
+            ops.triplet_torsion_bwd_arg(pos, g, dtorsion, dpos)
+        return dpos
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gd):
+        pos, ddist, dangle, dtorsion = ctx.saved_tensors
+        g, gd = ctx.g, _c(gd)
+        need = ctx.needs_input_grad
+        d_ddist = None
+        if ddist is not None:
+            d_ddist, d_pos = ops.edge_dist_bwd2(pos, g, ddist, gd)
+        else:
+            d_pos = torch.zeros_like(pos)
+        d_da, d_dt = None, None
+        if dangle is not None or dtorsion is not None:
+            d_da, d_dt = ops.triplet_geometry_bwd2(pos, g, dangle, dtorsion, gd, d_pos,
+                                                   want_dangle=dangle is not None and need[2],
+                                                   want_dtorsion=dtorsion is not None and need[3])
+        return d_pos, d_ddist if need[1] else None, d_da, d_dt, None
+
+
+class _TripletGeometry(torch.autograd.Function):
+    """(dist, angle[, torsion]) of xyz_to_dat's graph as twice-differentiable functions of pos: the values the graph
+    kernels computed, bit for bit."""
+
+    @staticmethod
+    def forward(ctx, pos, g, n_out):
+        ctx.g = g
+        ctx.save_for_backward(pos)
+        ctx.set_materialize_grads(False)
+        outs = [g.dist.detach().view(-1), g.angle.detach().view(-1)]
+        if n_out == 3:
+            outs.append(g.torsion.detach().view(-1))
+        return tuple(outs)
+
+    @staticmethod
+    def backward(ctx, ddist, dangle, dtorsion=None):
+        (pos,) = ctx.saved_tensors
+        if ddist is None and dangle is None and dtorsion is None:
+            return None, None, None
+        return _TripletGeometryBwd.apply(pos, ddist, dangle, dtorsion, ctx.g), None, None
+
+
 class _EdgeFeatBwd(torch.autograd.Function):
     @staticmethod
     def forward(ctx, dist, dgauss, dcut, offset, coeff, cutoff):
@@ -333,9 +394,16 @@ def segment_sum(x, ptr, idx):
 
 
 def geometry(pos, g, n_out=1):
-    if n_out != 1:
-        raise NotImplementedError("second-order geometry exists for edge lengths only (SchNet)")
-    return _Geometry.apply(pos, g)
+    """n_out = 1: dist (SchNet); 2: (dist, angle); 3: (dist, angle, torsion), the torsion only for a graph that carries
+    its winning candidates (g.tors_arg, set by xyz_to_dat's any-degree geometry)."""
+    if n_out == 1:
+        return _Geometry.apply(pos, g)
+    if n_out == 3 and getattr(g, "tors_arg", None) is None:
+        raise NotImplementedError("second-order torsions need the graph's winning candidates (g.tors_arg): "
+                                  "xyz_to_dat records them when pos requires grad")
+    if n_out not in (2, 3):
+        raise ValueError(f"n_out must be 1, 2 or 3, got {n_out}")
+    return _TripletGeometry.apply(pos, g, n_out)
 
 
 def schnet_edge_features(dist, offset, coeff, cutoff):

@@ -361,6 +361,21 @@ __device__ __forceinline__ float torsion_min_fold(float best, const f3 p1, const
   return best;
 }
 
+// The same fold, also recording the slot of the winner: strict `<` in ascending slot order keeps the first slot among
+// exactly equal minima (torch_scatter's CPU scatter_min arg rule); a tile folded after an earlier one passes slot0, its
+// first slot.  The kept value is the one fminf would keep: candidates are NaN or in (0, 2 pi], and fminf skips NaN too.
+__device__ __forceinline__ float torsion_min_fold_arg(float best, int& arg, const f3 p1, const float (*planes)[3],
+                                                      int n, int skip, const f3 pos_ji, const float dist_ji,
+                                                      int slot0) {
+  for (int c = 0; c < n; ++c) {
+    if (c == skip) continue;
+    const f3 p2 = {planes[c][0], planes[c][1], planes[c][2]};
+    const float tor = torsion_candidate(p1, p2, pos_ji, dist_ji);
+    if (tor < best) { best = tor; arg = slot0 + c; }
+  }
+  return best;
+}
+
 // Outputs of triplet t = (k -> j -> i) with k the in-edge kj of j and plane p1: the angle, the indices and the torsion
 // (use_torsion 1: `tor_min`, the min over all candidates folded by the caller; 2: G-SphereNet's single reference atom).
 __device__ __forceinline__ void triplet_emit(const float* __restrict__ pos, const f3 pj, const f3 pos_ji,
@@ -393,8 +408,11 @@ __device__ __forceinline__ void triplet_emit(const float* __restrict__ pos, cons
 // One warp per edge e = (j -> i) whose source j has at most max_deg <= GEO_MAXDEG in-edges (heavier edges are left to
 // triplet_geometry_heavy_kernel).  Lane s owns in-edge s of j (k = src[row_ptr[j]+s]), parks its plane in shared
 // memory and every lane then scans all candidates k_n.
+// ARG (use_torsion 1 only): also write tors_arg[t], the slot of the winning candidate among j's in-edges (-1 when no
+// candidate is finite).  tors_arg is the last parameter, so the ARG = false instantiations keep their parameter layout.
 constexpr int GEO_WARPS = 8;
 
+template <bool ARG = false>
 __global__ void __launch_bounds__(GEO_WARPS * 32)
 triplet_geometry_kernel(const float* __restrict__ pos, const int32_t* __restrict__ src,
                         const int32_t* __restrict__ dst, const int32_t* __restrict__ row_ptr,
@@ -402,7 +420,7 @@ triplet_geometry_kernel(const float* __restrict__ pos, const int32_t* __restrict
                         float* __restrict__ angle, float* __restrict__ torsion, int32_t* __restrict__ idx_kj,
                         int32_t* __restrict__ idx_ji, int64_t* __restrict__ idx_kj64,
                         int64_t* __restrict__ idx_ji64, const int32_t* __restrict__ nn1 = nullptr,
-                        const int32_t* __restrict__ nn2 = nullptr) {
+                        const int32_t* __restrict__ nn2 = nullptr, int32_t* __restrict__ tors_arg = nullptr) {
   __shared__ float planes[GEO_WARPS][GEO_MAXDEG][3];
   __shared__ int32_t ks[GEO_WARPS][GEO_MAXDEG];
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
@@ -431,7 +449,13 @@ triplet_geometry_kernel(const float* __restrict__ pos, const int32_t* __restrict
     if (s == p_i) continue;
     const f3 p1 = {planes[w][s][0], planes[w][s][1], planes[w][s][2]};
     float best = __int_as_float(0x7f800000);
-    if (use_torsion == 1) best = torsion_min_fold(best, p1, planes[w], d, p_i, pos_ji, dist_ji);
+    if constexpr (ARG) {
+      int arg = -1;
+      best = torsion_min_fold_arg(best, arg, p1, planes[w], d, p_i, pos_ji, dist_ji, 0);
+      tors_arg[t0 + s - (s > p_i ? 1 : 0)] = arg;
+    } else {
+      if (use_torsion == 1) best = torsion_min_fold(best, p1, planes[w], d, p_i, pos_ji, dist_ji);
+    }
     triplet_emit(pos, pj, pos_ji, dist_ji, ks[w][s], p1, t0 + s - (s > p_i ? 1 : 0), base + s, e, j, i, use_torsion,
                  best, angle, torsion, idx_kj, idx_ji, idx_kj64, idx_ji64, nn1, nn2);
   }
@@ -444,13 +468,15 @@ triplet_geometry_kernel(const float* __restrict__ pos, const int32_t* __restrict
 // is small next to the d^2 torsion candidates per edge.
 constexpr int HEAVY_THREADS = 128;
 
+template <bool ARG = false>
 __global__ void __launch_bounds__(HEAVY_THREADS)
 triplet_geometry_heavy_kernel(const float* __restrict__ pos, const int32_t* __restrict__ src,
                               const int32_t* __restrict__ dst, const int32_t* __restrict__ row_ptr,
                               const int32_t* __restrict__ trip_ptr, const int32_t* __restrict__ heavy,
                               int use_torsion, float* __restrict__ angle, float* __restrict__ torsion,
                               int64_t* __restrict__ idx_kj64, int64_t* __restrict__ idx_ji64,
-                              const int32_t* __restrict__ nn1, const int32_t* __restrict__ nn2) {
+                              const int32_t* __restrict__ nn1, const int32_t* __restrict__ nn2,
+                              int32_t* __restrict__ tors_arg = nullptr) {
   __shared__ float planes[HEAVY_THREADS][3];
   const int x = threadIdx.x;
   const int e = heavy ? heavy[blockIdx.x] : (int)blockIdx.x;
@@ -471,6 +497,7 @@ triplet_geometry_heavy_kernel(const float* __restrict__ pos, const int32_t* __re
       p1 = cross_aten(pos_ji, sub3(load3(pos, k), pj));
     }
     float best = __int_as_float(0x7f800000);
+    int arg = -1;
     if (use_torsion == 1) {
       for (int c0 = 0; c0 < d; c0 += HEAVY_THREADS) {
         __syncthreads();                                    // the previous tile has been read
@@ -480,10 +507,17 @@ triplet_geometry_heavy_kernel(const float* __restrict__ pos, const int32_t* __re
           planes[x][0] = pl.x; planes[x][1] = pl.y; planes[x][2] = pl.z;
         }
         __syncthreads();
-        if (s < d && s != p_i)
-          best = torsion_min_fold(best, p1, planes, min(HEAVY_THREADS, d - c0), p_i - c0, pos_ji, dist_ji);
+        if (s < d && s != p_i) {
+          if constexpr (ARG)
+            best = torsion_min_fold_arg(best, arg, p1, planes, min(HEAVY_THREADS, d - c0), p_i - c0, pos_ji, dist_ji,
+                                        c0);
+          else
+            best = torsion_min_fold(best, p1, planes, min(HEAVY_THREADS, d - c0), p_i - c0, pos_ji, dist_ji);
+        }
       }
     }
+    if constexpr (ARG)
+      if (s < d && s != p_i) tors_arg[t0 + s - (s > p_i ? 1 : 0)] = arg;
     if (s < d && s != p_i)
       triplet_emit(pos, pj, pos_ji, dist_ji, k, p1, t0 + s - (s > p_i ? 1 : 0), base + s, e, j, i, use_torsion, best,
                    angle, torsion, nullptr, nullptr, idx_kj64, idx_ji64, nn1, nn2);
@@ -670,16 +704,22 @@ int dig3d_triplet_geometry(const float* pos, const int32_t* src, const int32_t* 
   return DIG3D_OK;
 }
 
-int dig3d_triplet_geometry_any_degree(const float* pos, const int32_t* src, const int32_t* dst,
-                                      const int32_t* row_ptr, const int32_t* trip_ptr, int64_t n_edges,
-                                      int64_t n_heavy, int32_t use_torsion, const int32_t* nn1, const int32_t* nn2,
-                                      int32_t* heavy_ws, float* angle, float* torsion, int64_t* idx_kj64,
-                                      int64_t* idx_ji64, void* stream) {
+}  // extern "C"
+
+// The any-degree dispatcher, shared by dig3d_triplet_geometry_any_degree (ARG = false) and its _arg variant (ARG = true,
+// use_torsion 1, also writes tors_arg).
+template <bool ARG>
+static int triplet_geometry_any_degree_impl(const float* pos, const int32_t* src, const int32_t* dst,
+                                            const int32_t* row_ptr, const int32_t* trip_ptr, int64_t n_edges,
+                                            int64_t n_heavy, int32_t use_torsion, const int32_t* nn1,
+                                            const int32_t* nn2, int32_t* heavy_ws, float* angle, float* torsion,
+                                            int64_t* idx_kj64, int64_t* idx_ji64, int32_t* tors_arg, void* stream) {
   DIG3D_REQUIRE(pos && src && dst && row_ptr && trip_ptr && angle && idx_kj64 && idx_ji64,
                 "triplet_geometry_any_degree: null pointer");
   DIG3D_REQUIRE(use_torsion >= 0 && use_torsion <= 2, "triplet_geometry_any_degree: use_torsion=%d", use_torsion);
   DIG3D_REQUIRE(!use_torsion || torsion, "triplet_geometry_any_degree: torsion requested without output buffer");
   DIG3D_REQUIRE(use_torsion != 2 || (nn1 && nn2), "triplet_geometry_any_degree: the kNN torsion needs nn1 and nn2");
+  DIG3D_REQUIRE(!ARG || (use_torsion == 1 && tors_arg), "triplet_geometry_any_degree_arg: null tors_arg");
   DIG3D_REQUIRE(n_heavy >= 0 && n_heavy <= n_edges && n_edges < (1ll << 31),
                 "triplet_geometry_any_degree: %lld heavy edges of %lld", (long long)n_heavy, (long long)n_edges);
   DIG3D_REQUIRE(n_heavy == 0 || n_heavy == n_edges || heavy_ws,
@@ -687,9 +727,9 @@ int dig3d_triplet_geometry_any_degree(const float* pos, const int32_t* src, cons
   if (n_edges == 0) return DIG3D_OK;
   cudaStream_t st = (cudaStream_t)stream;
   if (n_heavy < n_edges) {
-    triplet_geometry_kernel<<<ceil_div(n_edges, GEO_WARPS), GEO_WARPS * 32, 0, st>>>(
+    triplet_geometry_kernel<ARG><<<ceil_div(n_edges, GEO_WARPS), GEO_WARPS * 32, 0, st>>>(
         pos, src, dst, row_ptr, trip_ptr, (int)n_edges, GEO_MAXDEG, use_torsion, angle, torsion, nullptr, nullptr,
-        idx_kj64, idx_ji64, nn1, nn2);
+        idx_kj64, idx_ji64, nn1, nn2, tors_arg);
     DIG3D_LAUNCH_CHECK();
   }
   if (n_heavy == 0) return DIG3D_OK;
@@ -700,10 +740,30 @@ int dig3d_triplet_geometry_any_degree(const float* pos, const int32_t* src, cons
     DIG3D_LAUNCH_CHECK();
     heavy = heavy_ws + 1;
   }
-  triplet_geometry_heavy_kernel<<<(unsigned)n_heavy, HEAVY_THREADS, 0, st>>>(
-      pos, src, dst, row_ptr, trip_ptr, heavy, use_torsion, angle, torsion, idx_kj64, idx_ji64, nn1, nn2);
+  triplet_geometry_heavy_kernel<ARG><<<(unsigned)n_heavy, HEAVY_THREADS, 0, st>>>(
+      pos, src, dst, row_ptr, trip_ptr, heavy, use_torsion, angle, torsion, idx_kj64, idx_ji64, nn1, nn2, tors_arg);
   DIG3D_LAUNCH_CHECK();
   return DIG3D_OK;
+}
+
+extern "C" {
+
+int dig3d_triplet_geometry_any_degree(const float* pos, const int32_t* src, const int32_t* dst,
+                                      const int32_t* row_ptr, const int32_t* trip_ptr, int64_t n_edges,
+                                      int64_t n_heavy, int32_t use_torsion, const int32_t* nn1, const int32_t* nn2,
+                                      int32_t* heavy_ws, float* angle, float* torsion, int64_t* idx_kj64,
+                                      int64_t* idx_ji64, void* stream) {
+  return triplet_geometry_any_degree_impl<false>(pos, src, dst, row_ptr, trip_ptr, n_edges, n_heavy, use_torsion, nn1,
+                                                 nn2, heavy_ws, angle, torsion, idx_kj64, idx_ji64, nullptr, stream);
+}
+
+int dig3d_triplet_geometry_any_degree_arg(const float* pos, const int32_t* src, const int32_t* dst,
+                                          const int32_t* row_ptr, const int32_t* trip_ptr, int64_t n_edges,
+                                          int64_t n_heavy, int32_t* heavy_ws, float* angle, float* torsion,
+                                          int64_t* idx_kj64, int64_t* idx_ji64, int32_t* tors_arg, void* stream) {
+  return triplet_geometry_any_degree_impl<true>(pos, src, dst, row_ptr, trip_ptr, n_edges, n_heavy, 1, nullptr,
+                                                nullptr, heavy_ws, angle, torsion, idx_kj64, idx_ji64, tors_arg,
+                                                stream);
 }
 
 int dig3d_knn2(const float* pos, const int64_t* batch, const int32_t* graph_ptr, int64_t n_nodes, int64_t n_graphs,

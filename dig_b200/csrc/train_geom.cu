@@ -376,11 +376,270 @@ triplet_torsion_jvp_kernel(const float* __restrict__ pos, const float* __restric
   }
 }
 
+// ------------------------------------------------------------------------------ xyz_to_dat's derivatives, any in-degree
+// The triplets of xyz_to_dat(..., use_torsion=True) with `tors_arg` (dig3d_triplet_geometry_any_degree_arg): the torsion
+// of triplet t = (k -> j -> i) is the candidate in slot tors_arg[t] of j's in-edges, c = src[row_ptr[j] + tors_arg[t]],
+// so no kernel below searches for it again.
+//
+// The per-triplet gradients are written once, templated on the scalar: float gives the gradient, `dual` (value and
+// tangent) evaluated with the tangent seeded by G gives, in the same pass, the gradient's value (<grad, G> is the JVP)
+// and its directional derivative along G (the Hessian-vector product H G).  Conventions (DESIGN.md §6): a collinear
+// angle (|ji x jk| = 0) keeps only the atan2 term in a = ji . jk, whose coefficient -b / (a^2 + b^2) is then 0, and the
+// tangent of |w| at w = 0 is taken as 0; a^2 + b^2 = 0 and |ji| = 0 pass nothing; the self candidate c = k is the
+// constant 2 pi or its rounding residue (plane1 x plane1) and passes nothing.  The derivative kernels of the models
+// (triplet_angle_bwd_kernel above, shared and unchanged) form cross products with ATen's fused rounding instead.
+struct dual {
+  float v, d;
+};
+__device__ __forceinline__ float val(float a) { return a; }
+__device__ __forceinline__ float val(dual a) { return a.v; }
+__device__ __forceinline__ dual operator+(dual a, dual b) { return {a.v + b.v, a.d + b.d}; }
+__device__ __forceinline__ dual operator-(dual a, dual b) { return {a.v - b.v, a.d - b.d}; }
+__device__ __forceinline__ dual operator-(dual a) { return {-a.v, -a.d}; }
+__device__ __forceinline__ dual operator*(dual a, dual b) { return {a.v * b.v, a.d * b.v + a.v * b.d}; }
+__device__ __forceinline__ dual operator/(dual a, dual b) {
+  const float q = a.v / b.v;
+  return {q, (a.d - q * b.d) / b.v};
+}
+__device__ __forceinline__ float sqrt_t(float a) { return sqrtf(a); }
+__device__ __forceinline__ dual sqrt_t(dual a) {
+  const float r = sqrtf(a.v);
+  return {r, r > 0.f ? a.d / (2.f * r) : 0.f};
+}
+
+template <typename T>
+struct v3 {
+  T x, y, z;
+};
+template <typename T>
+__device__ __forceinline__ v3<T> operator+(const v3<T> a, const v3<T> b) { return {a.x + b.x, a.y + b.y, a.z + b.z}; }
+template <typename T>
+__device__ __forceinline__ v3<T> operator*(const v3<T> a, const T s) { return {a.x * s, a.y * s, a.z * s}; }
+template <typename T>
+__device__ __forceinline__ T dot(const v3<T> a, const v3<T> b) { return a.x * b.x + a.y * b.y + a.z * b.z; }
+// The cross product's value from separately rounded products (no FMA contraction): exactly parallel copies of a vector
+// (an atom at the same position as another) then give exactly 0, so the conventions for a zero cross product apply.
+__device__ __forceinline__ float mul_rn(float a, float b) { return __fmul_rn(a, b); }
+__device__ __forceinline__ dual mul_rn(dual a, dual b) { return {__fmul_rn(a.v, b.v), a.d * b.v + a.v * b.d}; }
+template <typename T>
+__device__ __forceinline__ v3<T> cross(const v3<T> a, const v3<T> b) {
+  return {mul_rn(a.y, b.z) - mul_rn(a.z, b.y), mul_rn(a.z, b.x) - mul_rn(a.x, b.z), mul_rn(a.x, b.y) - mul_rn(a.y, b.x)};
+}
+
+// theta = atan2(b, a), a = u . v, w = u x v, b = |w|  ->  (d theta / du, d theta / dv); false: passes nothing.
+template <typename T>
+__device__ __forceinline__ bool angle_grad(const v3<T> u, const v3<T> v, v3<T>& g_u, v3<T>& g_v) {
+  const T a = dot(u, v);
+  const v3<T> w = cross(u, v);
+  const T b = sqrt_t(dot(w, w));
+  const T den = a * a + b * b;
+  if (val(den) == 0.f) return false;
+  const T ga = -b / den, gb = a / den;
+  g_u = v * ga;
+  g_v = u * ga;
+  if (val(b) > 0.f) {
+    const v3<T> wh = w * (T{1.f} / b);
+    g_u = g_u + cross(v, wh) * gb;
+    g_v = g_v + cross(wh, u) * gb;
+  }
+  return true;
+}
+
+// tau = atan2(tb, ta), p1 = u x vk, p2 = u x vc, ta = p1 . p2, tb = ((p1 x p2) . u) / |u|
+//   -> (d tau / du, d tau / dvk, d tau / dvc); false: passes nothing.
+template <typename T>
+__device__ __forceinline__ bool torsion_grad(const v3<T> u, const v3<T> vk, const v3<T> vc, v3<T>& g_u, v3<T>& g_vk,
+                                             v3<T>& g_vc) {
+  const T n = sqrt_t(dot(u, u));
+  if (val(n) == 0.f) return false;
+  const v3<T> p1 = cross(u, vk), p2 = cross(u, vc);
+  const T ta = dot(p1, p2);
+  const v3<T> q = cross(p1, p2);
+  const T tb = dot(q, u) / n;
+  const T den = ta * ta + tb * tb;
+  if (val(den) == 0.f) return false;
+  const T g_ta = -tb / den, g_tb = ta / den;
+  const T g_s = g_tb / n;                           // d tau / d (q . u)
+  const T g_n = -(g_tb * tb) / n;                   // d tau / d |u| (tb = (q . u) / |u|)
+  const v3<T> g_q = u * g_s;                        // (p1 x p2) . g_q = p1 . (p2 x g_q) = p2 . (g_q x p1)
+  const v3<T> g_p1 = p2 * g_ta + cross(p2, g_q);
+  const v3<T> g_p2 = p1 * g_ta + cross(g_q, p1);
+  g_u = q * g_s + u * (g_n / n) + cross(vk, g_p1) + cross(vc, g_p2);
+  g_vk = cross(g_p1, u);
+  g_vc = cross(g_p2, u);
+  return true;
+}
+
+__device__ __forceinline__ v3<float> to_v3(const f3 a) { return {a.x, a.y, a.z}; }
+__device__ __forceinline__ f3 to_f3(const v3<float> a) { return {a.x, a.y, a.z}; }
+__device__ __forceinline__ v3<dual> to_dual(const f3 a, const f3 da) {
+  return {{a.x, da.x}, {a.y, da.y}, {a.z, da.z}};
+}
+__device__ __forceinline__ f3 value3(const v3<dual> a) { return {a.x.v, a.y.v, a.z.v}; }
+__device__ __forceinline__ f3 tangent3(const v3<dual> a) { return {a.x.d, a.y.d, a.z.d}; }
+
+// Slot of i among j's in-edges (d if absent), one ballot per 32 slots: triplet tt of edge (j -> i) is slot
+// s = tt + (tt >= p_i) of j's in-edges.
+__device__ __forceinline__ int slot_of(const int32_t* __restrict__ src, int base, int d, int i, int lane) {
+  int p_i = d;
+  for (int s0 = 0; s0 < d; s0 += 32) {
+    const int sl = s0 + lane;
+    const unsigned hit = __ballot_sync(0xffffffffu, sl < d && src[base + sl] == i);
+    if (hit) { p_i = s0 + __ffs(hit) - 1; break; }
+  }
+  return p_i;
+}
+
+// dpos of sum_t dtorsion[t] torsion[t], any in-degree: one warp per edge e = (j -> i), lanes over its triplets.  The i
+// and j parts are summed over the warp (one atomic triple each per edge); k and c get atomics.
+__global__ void __launch_bounds__(256)
+triplet_torsion_bwd_arg_kernel(const float* __restrict__ pos, const int32_t* __restrict__ src,
+                               const int32_t* __restrict__ dst, const int32_t* __restrict__ row_ptr,
+                               const int32_t* __restrict__ trip_ptr, const int32_t* __restrict__ tors_arg,
+                               const float* __restrict__ dtorsion, int n_edges, float* __restrict__ dpos) {
+  const int lane = threadIdx.x & 31;
+  const int e = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (e >= n_edges) return;
+  const int j = src[e], i = dst[e];
+  const int base = row_ptr[j], d = row_ptr[j + 1] - base;
+  const int t0 = trip_ptr[e], nt = trip_ptr[e + 1] - t0;
+  if (nt == 0) return;
+  const int p_i = slot_of(src, base, d, i, lane);
+  const f3 pj = load3(pos, j);
+  const v3<float> u = to_v3(sub3(load3(pos, i), pj));
+  f3 gi = {0.f, 0.f, 0.f}, gj = {0.f, 0.f, 0.f};
+  for (int tt = lane; tt < nt; tt += 32) {
+    const int s = tt + (tt >= p_i ? 1 : 0), a = tors_arg[t0 + tt];
+    const float g = dtorsion[t0 + tt];
+    if (a < 0 || a == s || g == 0.f) continue;
+    const int k = src[base + s], c = src[base + a];
+    v3<float> g_u, g_vk, g_vc;
+    if (!torsion_grad(u, to_v3(sub3(load3(pos, k), pj)), to_v3(sub3(load3(pos, c), pj)), g_u, g_vk, g_vc)) continue;
+    const f3 hk = to_f3(g_vk * g), hc = to_f3(g_vc * g), hu = to_f3(g_u * g);
+    atomic_add3(dpos, k, hk);
+    atomic_add3(dpos, c, hc);
+    gi = add3(gi, hu);
+    gj = add3(gj, add3(hu, add3(hk, hc)));
+  }
+  gi = warp_sum3(gi);
+  gj = warp_sum3(gj);
+  if (lane == 0) {
+    atomic_add3(dpos, i, gi);
+    atomic_add3(dpos, j, scale3(gj, -1.f));
+  }
+}
+
+// Backward of (triplet_angle_bwd + triplet_torsion_bwd_arg), i.e. of dpos = sum_t dangle_t grad angle_t + dtorsion_t
+// grad torsion_t, given G = d(loss) / d(dpos) [N, 3]:
+//   d_dangle[t] = <grad angle_t, G>,  d_dtorsion[t] = <grad torsion_t, G>,
+//   d_pos += dangle_t H_angle_t G + dtorsion_t H_torsion_t G.
+// dangle / dtorsion null: that term is absent (its Hessian term is zero; d_dangle / d_dtorsion are still written when
+// given).  Same warp-per-edge layout as triplet_torsion_bwd_arg_kernel; d_dangle / d_dtorsion are written for every
+// triplet (0 where the conventions pass nothing).
+__global__ void __launch_bounds__(256)
+triplet_geometry_bwd2_kernel(const float* __restrict__ pos, const int32_t* __restrict__ src,
+                             const int32_t* __restrict__ dst, const int32_t* __restrict__ row_ptr,
+                             const int32_t* __restrict__ trip_ptr, const int32_t* __restrict__ tors_arg,
+                             const float* __restrict__ dangle, const float* __restrict__ dtorsion,
+                             const float* __restrict__ G, int n_edges, float* __restrict__ d_dangle,
+                             float* __restrict__ d_dtorsion, float* __restrict__ d_pos) {
+  const int lane = threadIdx.x & 31;
+  const int e = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (e >= n_edges) return;
+  const int j = src[e], i = dst[e];
+  const int base = row_ptr[j], d = row_ptr[j + 1] - base;
+  const int t0 = trip_ptr[e], nt = trip_ptr[e + 1] - t0;
+  if (nt == 0) return;
+  const int p_i = slot_of(src, base, d, i, lane);
+  const f3 pj = load3(pos, j), Gj = load3(G, j);
+  const f3 Gu = sub3(load3(G, i), Gj);
+  const v3<dual> u = to_dual(sub3(load3(pos, i), pj), Gu);
+  const bool want_angle = dangle || d_dangle, want_torsion = dtorsion || d_dtorsion;
+  f3 hi = {0.f, 0.f, 0.f}, hj = {0.f, 0.f, 0.f};
+  for (int tt = lane; tt < nt; tt += 32) {
+    const int t = t0 + tt, s = tt + (tt >= p_i ? 1 : 0);
+    const int k = src[base + s];
+    const f3 Gk = sub3(load3(G, k), Gj);
+    const v3<dual> vk = to_dual(sub3(load3(pos, k), pj), Gk);
+    if (want_angle) {
+      v3<dual> g_u, g_v;
+      float jvp = 0.f;
+      if (angle_grad(u, vk, g_u, g_v)) {
+        jvp = dot(to_v3(value3(g_u)), to_v3(Gu)) + dot(to_v3(value3(g_v)), to_v3(Gk));
+        const float w = dangle ? dangle[t] : 0.f;
+        if (w != 0.f) {
+          const f3 hu = scale3(tangent3(g_u), w), hk = scale3(tangent3(g_v), w);
+          atomic_add3(d_pos, k, hk);
+          hi = add3(hi, hu);
+          hj = add3(hj, add3(hu, hk));
+        }
+      }
+      if (d_dangle) d_dangle[t] = jvp;
+    }
+    if (want_torsion) {
+      const int a = tors_arg[t];
+      float jvp = 0.f;
+      if (a >= 0 && a != s) {
+        const int c = src[base + a];
+        const f3 Gc = sub3(load3(G, c), Gj);
+        v3<dual> g_u, g_vk, g_vc;
+        if (torsion_grad(u, vk, to_dual(sub3(load3(pos, c), pj), Gc), g_u, g_vk, g_vc)) {
+          jvp = dot(to_v3(value3(g_u)), to_v3(Gu)) + dot(to_v3(value3(g_vk)), to_v3(Gk)) +
+                dot(to_v3(value3(g_vc)), to_v3(Gc));
+          const float w = dtorsion ? dtorsion[t] : 0.f;
+          if (w != 0.f) {
+            const f3 hu = scale3(tangent3(g_u), w), hk = scale3(tangent3(g_vk), w), hc = scale3(tangent3(g_vc), w);
+            atomic_add3(d_pos, k, hk);
+            atomic_add3(d_pos, c, hc);
+            hi = add3(hi, hu);
+            hj = add3(hj, add3(hu, add3(hk, hc)));
+          }
+        }
+      }
+      if (d_dtorsion) d_dtorsion[t] = jvp;
+    }
+  }
+  hi = warp_sum3(hi);
+  hj = warp_sum3(hj);
+  if (lane == 0) {
+    atomic_add3(d_pos, i, hi);
+    atomic_add3(d_pos, j, scale3(hj, -1.f));
+  }
+}
+
 }  // namespace dig3d
 
 using namespace dig3d;
 
 extern "C" {
+
+int dig3d_triplet_torsion_bwd_arg(const float* pos, const int32_t* src, const int32_t* dst, const int32_t* row_ptr,
+                                  const int32_t* trip_ptr, const int32_t* tors_arg, const float* dtorsion,
+                                  int64_t n_edges, float* dpos, void* stream) {
+  DIG3D_REQUIRE(pos && src && dst && row_ptr && trip_ptr && tors_arg && dtorsion && dpos,
+                "triplet_torsion_bwd_arg: null pointer");
+  DIG3D_REQUIRE(n_edges >= 0 && n_edges < (1ll << 26), "triplet_torsion_bwd_arg: %lld edges", (long long)n_edges);
+  if (n_edges == 0) return DIG3D_OK;
+  triplet_torsion_bwd_arg_kernel<<<ceil_div(n_edges * 32, 256), 256, 0, (cudaStream_t)stream>>>(
+      pos, src, dst, row_ptr, trip_ptr, tors_arg, dtorsion, (int)n_edges, dpos);
+  DIG3D_LAUNCH_CHECK();
+  return DIG3D_OK;
+}
+
+int dig3d_triplet_geometry_bwd2(const float* pos, const int32_t* src, const int32_t* dst, const int32_t* row_ptr,
+                                const int32_t* trip_ptr, const int32_t* tors_arg, const float* dangle,
+                                const float* dtorsion, const float* g_dpos, int64_t n_edges, float* d_dangle,
+                                float* d_dtorsion, float* d_pos, void* stream) {
+  DIG3D_REQUIRE(pos && src && dst && row_ptr && trip_ptr && g_dpos && d_pos, "triplet_geometry_bwd2: null pointer");
+  DIG3D_REQUIRE(!(dtorsion || d_dtorsion) || tors_arg, "triplet_geometry_bwd2: the torsion terms need tors_arg");
+  DIG3D_REQUIRE(n_edges >= 0 && n_edges < (1ll << 26), "triplet_geometry_bwd2: %lld edges", (long long)n_edges);
+  if (n_edges == 0) return DIG3D_OK;
+  triplet_geometry_bwd2_kernel<<<ceil_div(n_edges * 32, 256), 256, 0, (cudaStream_t)stream>>>(
+      pos, src, dst, row_ptr, trip_ptr, tors_arg, dangle, dtorsion, g_dpos, (int)n_edges, d_dangle, d_dtorsion,
+      d_pos);
+  DIG3D_LAUNCH_CHECK();
+  return DIG3D_OK;
+}
 
 int dig3d_edge_dist_bwd(const float* pos, const int32_t* src, const int32_t* dst, const float* dist, const float* ddist,
                         int64_t n_edges, float* dpos, void* stream) {

@@ -57,7 +57,8 @@ class Graph3D:
                  "row_ptr", "src", "dst", "edge_index", "dist", "vec", "trip_ptr",
                  "angle", "torsion", "idx_kj", "idx_ji", "idx_kj64", "idx_ji64",
                  "out_ptr", "out_list", "pos_in",      # out-edge lists (CSR by source), None for graphs built without them
-                 "comenet_refs")                       # ComENet's reference atoms (comenet_geometry)
+                 "comenet_refs",                       # ComENet's reference atoms (comenet_geometry)
+                 "tors_arg")                           # winning torsion candidate slots (triplet_geometry_any_degree_arg)
 
     def __init__(self):
         for s in self.__slots__:
@@ -218,6 +219,26 @@ def triplet_geometry_any_degree(g, pos, use_torsion, n_heavy, nn=None):
              _p(g.row_ptr), _p(g.trip_ptr), e, int(n_heavy), int(use_torsion),
              _p(nn[0]) if nn is not None else None, _p(nn[1]) if nn is not None else None, _p(ws), _p(g.angle),
              _p(g.torsion) if use_torsion else None, _p(g.idx_kj64), _p(g.idx_ji64), _stream())
+    return g
+
+
+def triplet_geometry_any_degree_arg(g, pos, n_heavy):
+    """triplet_geometry_any_degree(g, pos, 1, n_heavy) -- the same angle / torsion / index bits -- that also sets
+    g.tors_arg [T] int32, the slot of each triplet's winning torsion candidate among j's in-edges (-1: none finite),
+    which the derivative kernels read (triplet_torsion_bwd_arg, triplet_geometry_bwd2)."""
+    dev = pos.device
+    t = g.n_triplets
+    g.angle = torch.empty(t, dtype=torch.float32, device=dev)
+    g.torsion = torch.empty(t, dtype=torch.float32, device=dev)
+    g.idx_kj64 = torch.empty(t, dtype=torch.int64, device=dev)
+    g.idx_ji64 = torch.empty(t, dtype=torch.int64, device=dev)
+    g.tors_arg = torch.empty(t, dtype=torch.int32, device=dev)
+    e = g.n_edges
+    if e and t:
+        ws = torch.empty(n_heavy + 1, dtype=torch.int32, device=dev) if 0 < n_heavy < e else None
+        call("dig3d_triplet_geometry_any_degree_arg", _p(pos.detach(), torch.float32, "pos"), _p(g.src), _p(g.dst),
+             _p(g.row_ptr), _p(g.trip_ptr), e, int(n_heavy), _p(ws), _p(g.angle), _p(g.torsion), _p(g.idx_kj64),
+             _p(g.idx_ji64), _p(g.tors_arg), _stream())
     return g
 
 
@@ -1259,6 +1280,14 @@ def triplet_torsion_bwd(pos, g, dtorsion, dpos):
          _p(dtorsion, F32, "dtorsion"), g.n_edges, _p(dpos), _stream())
 
 
+def triplet_torsion_bwd_arg(pos, g, dtorsion, dpos):
+    """dpos += d torsion through the candidates g.tors_arg (any in-degree, no search)."""
+    if g.n_edges == 0 or g.n_triplets == 0:
+        return
+    call("dig3d_triplet_torsion_bwd_arg", _p(pos, F32, "pos"), _p(g.src), _p(g.dst), _p(g.row_ptr), _p(g.trip_ptr),
+         _p(g.tors_arg, torch.int32, "tors_arg"), _p(dtorsion, F32, "dtorsion"), g.n_edges, _p(dpos), _stream())
+
+
 def triplet_basis_project_bwd_geom(g, bess, bess_dx, basis_id, d_sbf_p, d_t_p, w_sbf1_rows, w_t1_rows, cutoff):
     """-> (ddist_kj [E], dangle [T], dtorsion [T] | None); d_t_p / w_t1_rows None = no torsion branch."""
     dev = bess.device
@@ -1559,6 +1588,24 @@ def edge_dist_bwd2(pos, g, ddist, g_dpos):
         call("dig3d_edge_dist_bwd2", _p(pos, F32, "pos"), _p(g.src), _p(g.dst), _p(g.dist), _p(ddist, F32, "ddist"),
              _p(g_dpos, F32, "g_dpos"), g.n_edges, _p(d_ddist), _p(d_pos), _stream())
     return d_ddist, d_pos
+
+
+def triplet_geometry_bwd2(pos, g, dangle, dtorsion, g_dpos, d_pos, want_dangle=True, want_dtorsion=True):
+    """Backward of triplet_angle_bwd (dangle) + triplet_torsion_bwd_arg (dtorsion) given g_dpos = d(loss)/d(dpos):
+    accumulates dangle H_angle g_dpos + dtorsion H_torsion g_dpos into d_pos and returns (d_dangle [T] | None,
+    d_dtorsion [T] | None), the JVPs <grad angle_t, g_dpos> / <grad torsion_t, g_dpos>.  dangle / dtorsion None = 0;
+    the torsion terms need g.tors_arg."""
+    dev = pos.device
+    t = g.n_triplets
+    d_da = torch.zeros(t, device=dev, dtype=F32) if want_dangle else None
+    d_dt = torch.zeros(t, device=dev, dtype=F32) if want_dtorsion else None
+    if g.n_edges and t and (dangle is not None or dtorsion is not None or want_dangle or want_dtorsion):
+        tors = dtorsion is not None or want_dtorsion
+        call("dig3d_triplet_geometry_bwd2", _p(pos, F32, "pos"), _p(g.src), _p(g.dst), _p(g.row_ptr), _p(g.trip_ptr),
+             _p(g.tors_arg, torch.int32, "tors_arg") if tors else None, _p(dangle, F32, "dangle"),
+             _p(dtorsion, F32, "dtorsion"), _p(g_dpos, F32, "g_dpos"), g.n_edges, _p(d_da), _p(d_dt), _p(d_pos),
+             _stream())
+    return d_da, d_dt
 
 
 def schnet_edge_features_bwd2(dist, offset, coeff, cutoff, dgauss, dcut, g):

@@ -7,7 +7,7 @@ materialise idx_kj / idx_ji); they exist for users of the reference's utility AP
 """
 import torch
 
-from ... import ops
+from ... import autograd_dd, ops
 from ...ops import _p, _stream, call
 
 
@@ -28,9 +28,10 @@ def radius_graph(x, r, batch=None, loop=False, max_num_neighbors=32, flow='sourc
 _HEAVY_KERNEL_FOR_ALL_EDGES = False
 
 
-def _xyz_to_dat_sorted(pos, ei, n, use_torsion, knn_batch=None):
+def _xyz_to_dat_sorted(pos, ei, n, use_torsion, knn_batch=None, want_grad=False):
     """Kernel path for an edge_index sorted by (target, source); returns None when it is not sorted.
-    knn_batch: the `batch` vector -- selects G-SphereNet's single-reference torsion (nearest neighbour of j)."""
+    knn_batch: the `batch` vector -- selects G-SphereNet's single-reference torsion (nearest neighbour of j).
+    want_grad: with the torsion, record each triplet's winning candidate (g.tors_arg) for the derivative kernels."""
     dev = pos.device
     e = ei.size(1)
     g = ops.Graph3D()
@@ -52,6 +53,8 @@ def _xyz_to_dat_sorted(pos, ei, n, use_torsion, knn_batch=None):
     g.n_triplets = t
     n_heavy = e if _HEAVY_KERNEL_FOR_ALL_EDGES else fl[1]
     if knn_batch is None:
+        if want_grad and use_torsion:
+            return ops.triplet_geometry_any_degree_arg(g, pos, n_heavy)
         return ops.triplet_geometry_any_degree(g, pos, int(bool(use_torsion)), n_heavy)
     n_graphs = int(knn_batch[-1].item()) + 1 if n else 0
     graph_ptr = torch.empty(n_graphs + 1, dtype=torch.int32, device=dev)
@@ -76,7 +79,13 @@ def xyz_to_dat(pos, edge_index, num_nodes, use_torsion=False, _knn_batch=None):
 
     Any in-degree: a node of in-degree d and out-degree d' has about d * d' triplets, and the torsion takes the min
     over d candidates per triplet (the sets the reference materialises).  Raises ValueError for 2^31 edges or
-    triplets or more (int32 indices), before the triplet buffers are allocated."""
+    triplets or more (int32 indices), before the triplet buffers are allocated.
+
+    Derivatives: when `pos` requires grad and grad mode is on, `dist`, `angle` and `torsion` are differentiable in
+    `pos`, twice (forces with `torch.autograd.grad(E, pos, create_graph=True)`, then a backward through them), with
+    the same values bit for bit.  The torsion's gradient flows through the first minimal candidate; a zero-length edge,
+    a collinear triplet's cross-product term, atan2(0, 0) and the self candidate (plane1 x plane1) pass nothing
+    (DESIGN.md §6).  Otherwise the outputs do not require grad, as before."""
     if edge_index.dim() != 2 or edge_index.size(0) != 2:
         raise ValueError("edge_index must be [2, E]")
     e = edge_index.size(1)
@@ -86,16 +95,23 @@ def xyz_to_dat(pos, edge_index, num_nodes, use_torsion=False, _knn_batch=None):
     j, i = ei[0], ei[1]
     if e and (int(ei.min()) < 0 or int(ei.max()) >= n):
         raise ValueError("xyz_to_dat: edge_index holds node ids outside [0, num_nodes)")
-    g = _xyz_to_dat_sorted(pos, ei, n, use_torsion, _knn_batch)
-    if g is not None:
+    want_grad = _knn_batch is None and pos.requires_grad and torch.is_grad_enabled()
+    g = _xyz_to_dat_sorted(pos, ei, n, use_torsion, _knn_batch, want_grad)
+    sorted_in = g is not None
+    if not sorted_in:                                                   # arbitrary edge order
+        perm = torch.sort(i * n + j, stable=True).indices              # sorted position -> caller's edge id
+        g = _xyz_to_dat_sorted(pos, ei[:, perm].contiguous(), n, use_torsion, _knn_batch, want_grad)
+        if g is None:
+            raise RuntimeError("xyz_to_dat: internal error, sorted edge list rejected")
+    if want_grad:
+        geo = autograd_dd.geometry(pos, g, 3 if use_torsion else 2)
+        dist, angle, torsion = geo[0], geo[1], (geo[2] if use_torsion else None)
+    else:
+        dist, angle, torsion = g.dist, g.angle, g.torsion
+    if sorted_in:
         if use_torsion:
-            return g.dist, g.angle, g.torsion, i, j, g.idx_kj64, g.idx_ji64
-        return g.dist, g.angle, i, j, g.idx_kj64, g.idx_ji64
-    # arbitrary edge order
-    perm = torch.sort(i * n + j, stable=True).indices                  # sorted position -> caller's edge id
-    g = _xyz_to_dat_sorted(pos, ei[:, perm].contiguous(), n, use_torsion, _knn_batch)
-    if g is None:
-        raise RuntimeError("xyz_to_dat: internal error, sorted edge list rejected")
+            return dist, angle, torsion, i, j, g.idx_kj64, g.idx_ji64
+        return dist, angle, i, j, g.idx_kj64, g.idx_ji64
     inv = torch.empty_like(perm)
     inv[perm] = torch.arange(e, device=perm.device)                    # caller's edge id -> sorted position
     tp = g.trip_ptr.long()
@@ -104,10 +120,8 @@ def xyz_to_dat(pos, edge_index, num_nodes, use_torsion=False, _knn_batch=None):
     t = int(cnt.sum())
     first = torch.cumsum(cnt, 0) - cnt
     take = torch.repeat_interleave(start - first, cnt) + torch.arange(t, device=perm.device)
-    dist = g.dist[inv]
-    angle = g.angle[take]
     idx_kj = perm[g.idx_kj64[take]]
     idx_ji = torch.repeat_interleave(torch.arange(e, device=perm.device), cnt)
     if use_torsion:
-        return dist, angle, g.torsion[take], i, j, idx_kj, idx_ji
-    return dist, angle, i, j, idx_kj, idx_ji
+        return dist[inv], angle[take], torsion[take], i, j, idx_kj, idx_ji
+    return dist[inv], angle[take], i, j, idx_kj, idx_ji

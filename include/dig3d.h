@@ -145,6 +145,15 @@ int dig3d_triplet_geometry_any_degree(const float* pos, const int32_t* src, cons
                                       int32_t* heavy_ws, float* angle, float* torsion, int64_t* idx_kj64,
                                       int64_t* idx_ji64, void* stream);
 
+/* dig3d_triplet_geometry_any_degree with use_torsion 1 (same kernels, same angle / torsion / index bits) that also writes
+ * tors_arg[T]: the slot s of the winning torsion candidate among j's in-edges (c = src[row_ptr[j] + s]), the first slot
+ * among exactly equal minima, -1 when no candidate is finite.  The derivative kernels dig3d_triplet_torsion_bwd_arg and
+ * dig3d_triplet_geometry_bwd2 read it instead of searching again. */
+int dig3d_triplet_geometry_any_degree_arg(const float* pos, const int32_t* src, const int32_t* dst,
+                                          const int32_t* row_ptr, const int32_t* trip_ptr, int64_t n_edges,
+                                          int64_t n_heavy, int32_t* heavy_ws, float* angle, float* torsion,
+                                          int64_t* idx_kj64, int64_t* idx_ji64, int32_t* tors_arg, void* stream);
+
 /* ------------------------------------------------------------------ basis
  * dist_emb / angle_emb / torsion_emb      spherenet/features.py:167-263, dimenetpp/features.py:149-220
  * basis_id: 0 = dimenet flavour ns=7 nr=6, 1 = dimenet ns=3 nr=6, 2 = gemnet ns=2 nr=3 (ComENet).
@@ -707,6 +716,20 @@ int dig3d_edge_dist_bwd2(const float* pos, const int32_t* src, const int32_t* ds
 int dig3d_schnet_edge_features_bwd2(const float* dist, int64_t n_edges, const float* offset, int32_t n_gauss,
                                     double coeff, double cutoff, const float* dgauss, const float* dcut, const float* g,
                                     float* d_dgauss, float* d_dcut, float* d_dist, void* stream);
+/* ---- xyz_to_dat's derivatives at any in-degree (tors_arg from dig3d_triplet_geometry_any_degree_arg; n_edges < 2^26).
+ * triplet_torsion_bwd_arg: dpos += d torsion[t] through candidate tors_arg[t] (one warp per edge, no search, no shared
+ *   memory); the self candidate c = k, tors_arg = -1, |ji| = 0 and atan2(0, 0) pass nothing.
+ * triplet_geometry_bwd2: the backward of dig3d_triplet_angle_bwd + dig3d_triplet_torsion_bwd_arg given
+ *   g_dpos = d(loss)/d(dpos): d_dangle[t] = <grad angle_t, g_dpos>, d_dtorsion[t] = <grad torsion_t, g_dpos> (every row
+ *   written when non-NULL) and d_pos += dangle_t H_angle_t g_dpos + dtorsion_t H_torsion_t g_dpos (atomics into a
+ *   caller-initialised buffer).  dangle / dtorsion NULL = zero; tors_arg may be NULL when dtorsion and d_dtorsion are. */
+int dig3d_triplet_torsion_bwd_arg(const float* pos, const int32_t* src, const int32_t* dst, const int32_t* row_ptr,
+                                  const int32_t* trip_ptr, const int32_t* tors_arg, const float* dtorsion,
+                                  int64_t n_edges, float* dpos, void* stream);
+int dig3d_triplet_geometry_bwd2(const float* pos, const int32_t* src, const int32_t* dst, const int32_t* row_ptr,
+                                const int32_t* trip_ptr, const int32_t* tors_arg, const float* dangle,
+                                const float* dtorsion, const float* g_dpos, int64_t n_edges, float* d_dangle,
+                                float* d_dtorsion, float* d_pos, void* stream);
 /* ProNet (pronet.py:352-449, pronet/features.py:253-344): per-edge geometry from the C-alpha chain (sequence-neighbour
  * references), level 0 = aminoacid (feature1[E,12] from tau), level 1 = backbone / allatom (feature1[E,36] from the three
  * Euler angles of the N-CA-C frames; needs pos_n / pos_c); feature0[E,24] = d_theta_phi_emb, pos_emb[E,num_pos_emb];
