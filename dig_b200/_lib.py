@@ -178,6 +178,9 @@ SIGNATURES = {
     "dig3d_geometry_jvp": [P, P, P, P, P, P, P, c_int64, P, P, P, P],
     "dig3d_edge_basis_tangent": [P, P, c_int64, c_double, c_int32, P, c_int32, c_int32, P, P, P],
     "dig3d_rbf_freq_grad_tangent": [P, P, c_int64, c_double, c_int32, P, c_int32, P, P, P],
+    "dig3d_edge_basis_tangent_bwd": [P, P, c_int64, c_double, c_int32, P, c_int32, c_int32, P, P, P, P, P],
+    "dig3d_triplet_basis_tangent_bwd": [P, P, P, P, P, P, P, P, P, P, P, P, P, P, c_int64, c_int64, c_int32, P, P,
+                                        c_double, P, P, P, P, P, P, P],
     "dig3d_triplet_basis_tangent": [P, P, P, P, P, P, P, c_int64, c_int32, P, P, P],
     "dig3d_edge_dist_bwd2": [P, P, P, P, P, P, c_int64, P, P, P],
     "dig3d_schnet_edge_features_bwd2": [P, c_int64, P, c_int32, c_double, c_double, P, P, P, P, P, P, P],

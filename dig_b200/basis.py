@@ -269,25 +269,32 @@ def basis_sources(flavor, num_spherical, num_radial):
 
 @functools.lru_cache(maxsize=None)
 def basis_sources_second_order(flavor, num_spherical, num_radial):
-    """Second derivatives of the closed forms of `basis_sources` (bessel_dxx [ns*nr] in x; yl0_dtheta2 [ns] in theta):
-    what a second-order path through angle_emb needs (training ON forces for DimeNet++: d/dpos of the force goes through
-    d2(basis)/d(dist)2, d2/d(angle)2 and the mixed product of first derivatives, which `basis_sources` already has).
-    Not emitted into the generated headers yet -- no kernel consumes them in this round (DESIGN.md 7.1)."""
+    """Second derivatives of the closed forms of `basis_sources`: bessel_dxx [ns*nr] in x, yl0_dtheta2 [ns] in theta,
+    and ylm_dtheta2 / ylm_dtheta_dphi / ylm_dphi2 [ns*ns] in (theta, phi).  The Hessian path of DimeNet++ / SphereNet
+    reads them (csrc/generated/basis_<tag>_d2.cuh, the reverse mode of the tangent kernels in csrc/basis.cu)."""
     sym = _sym()
-    x, theta = sym.symbols("x"), sym.symbols("theta")
+    x, theta, phi = sym.symbols("x"), sym.symbols("theta"), sym.symbols("phi")
     if flavor == "dimenet":
         bess = bessel_expressions(_jn_dimenet, num_spherical, num_radial)
         y0 = harmonics_dimenet(num_spherical, zero_m_only=True)
+        yall = harmonics_dimenet(num_spherical, zero_m_only=False)
     elif flavor == "gemnet":
         bess = bessel_expressions(_jn_gemnet, num_spherical, num_radial)
         y0 = harmonics_gemnet(num_spherical, zero_m_only=True)
+        yall = harmonics_gemnet(num_spherical, zero_m_only=False)
     else:
         raise ValueError(flavor)
-    out = {"bessel_dxx": [], "yl0_dtheta2": []}
+    out = {"bessel_dxx": [], "yl0_dtheta2": [], "ylm_dtheta2": [], "ylm_dtheta_dphi": [], "ylm_dphi2": []}
     for l in range(num_spherical):
         for n in range(num_radial):
             out["bessel_dxx"].append(_src(sym.diff(bess[l][n], x, 2), [x]))
         out["yl0_dtheta2"].append("0.0" if l == 0 else _src(sym.diff(y0[l][0], theta, 2), [theta]))
+    for l in range(num_spherical):
+        for k in range(2 * l + 1 if l else 1):
+            for key, args in (("ylm_dtheta2", (theta, theta)), ("ylm_dtheta_dphi", (theta, phi)),
+                              ("ylm_dphi2", (phi, phi))):
+                d = 0 if l == 0 else sym.diff(yall[l][k], *args)
+                out[key].append("0.0" if d == 0 else _src(d, [theta, phi]))
     return out
 
 

@@ -187,6 +187,26 @@ def emit_header(tag, flavor, num_spherical, num_radial, sources):
     return "\n".join(parts)
 
 
+def emit_header_second_order(tag, flavor, num_spherical, num_radial, sources):
+    """Header of the second derivatives (basis.basis_sources_second_order) for one (flavor, ns, nr): the reverse mode of
+    the tangent kernels (Hessian-vector products) is their only reader, so they stay out of the first-order header."""
+    ns, nr = num_spherical, num_radial
+    parts = [
+        "// GENERATED by dig_b200/codegen.py -- do not edit.\n"
+        f"// flavor={flavor} num_spherical={ns} num_radial={nr}: second derivatives of the closed forms of\n"
+        f"// basis_{tag}.cuh (symbolic, same fp32 rounding rules); see dig_b200/basis.py.\n"
+        "#pragma once\n",
+        f"namespace basis_{tag} {{\n",
+        emit_function("bessel_dxx", ["x"], sources["bessel_dxx"], "d2/dx2 of bessel()"),
+        emit_function("yl0_dtheta2", ["theta"], sources["yl0_dtheta2"], "d2/dtheta2 of yl0()"),
+        emit_function("ylm_dtheta2", ["theta", "phi"], sources["ylm_dtheta2"], "d2/dtheta2 of ylm()"),
+        emit_function("ylm_dtheta_dphi", ["theta", "phi"], sources["ylm_dtheta_dphi"], "d2/dtheta dphi of ylm()"),
+        emit_function("ylm_dphi2", ["theta", "phi"], sources["ylm_dphi2"], "d2/dphi2 of ylm()"),
+        "}  // namespace\n",
+    ]
+    return "\n".join(parts)
+
+
 CONFIGS = {
     # tag: (flavor, num_spherical, num_radial)
     "dimenet_7_6": ("dimenet", 7, 6),      # SphereNet / DimeNet++ defaults
@@ -194,6 +214,8 @@ CONFIGS = {
     "gemnet_2_3": ("gemnet", 2, 3),        # ComENet defaults
     "gemnet_2_6": ("gemnet", 2, 6),        # ProNet defaults (pronet/features.py is comenet/features.py with nr = 6)
 }
+# configurations with a second-order header (DimeNet++ / SphereNet Hessians)
+SECOND_ORDER = ("dimenet_7_6", "dimenet_3_6")
 
 
 def generate_all(out_dir, force=False):
@@ -208,6 +230,14 @@ def generate_all(out_dir, force=False):
         src = basis.basis_sources(flavor, ns, nr)
         with open(path, "w") as fh:
             fh.write(emit_header(tag, flavor, ns, nr, src))
+        written.append(path)
+    for tag in SECOND_ORDER:
+        flavor, ns, nr = CONFIGS[tag]
+        path = os.path.join(out_dir, f"basis_{tag}_d2.cuh")
+        if os.path.exists(path) and not force:
+            continue
+        with open(path, "w") as fh:
+            fh.write(emit_header_second_order(tag, flavor, ns, nr, basis.basis_sources_second_order(flavor, ns, nr)))
         written.append(path)
     return written
 

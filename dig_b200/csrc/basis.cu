@@ -14,6 +14,8 @@
 #include "generated/basis_dimenet_7_6.cuh"
 #include "generated/basis_dimenet_3_6.cuh"
 #include "generated/basis_gemnet_2_3.cuh"
+#include "generated/basis_dimenet_7_6_d2.cuh"
+#include "generated/basis_dimenet_3_6_d2.cuh"
 
 namespace dig3d {
 
@@ -28,6 +30,11 @@ struct B76 {
   __device__ static void yl0_dtheta(float t, float (&o)[NS]) { basis_dimenet_7_6::yl0_dtheta(t, o); }
   __device__ static void ylm_dtheta(float t, float p, float (&o)[NY]) { basis_dimenet_7_6::ylm_dtheta(t, p, o); }
   __device__ static void ylm_dphi(float t, float p, float (&o)[NY]) { basis_dimenet_7_6::ylm_dphi(t, p, o); }
+  __device__ static void bessel_dxx(float x, float (&o)[NB]) { basis_dimenet_7_6::bessel_dxx(x, o); }
+  __device__ static void yl0_dtheta2(float t, float (&o)[NS]) { basis_dimenet_7_6::yl0_dtheta2(t, o); }
+  __device__ static void ylm_dtheta2(float t, float p, float (&o)[NY]) { basis_dimenet_7_6::ylm_dtheta2(t, p, o); }
+  __device__ static void ylm_dtheta_dphi(float t, float p, float (&o)[NY]) { basis_dimenet_7_6::ylm_dtheta_dphi(t, p, o); }
+  __device__ static void ylm_dphi2(float t, float p, float (&o)[NY]) { basis_dimenet_7_6::ylm_dphi2(t, p, o); }
 };
 struct B36 {
   static constexpr int NS = basis_dimenet_3_6::NS, NR = basis_dimenet_3_6::NR;
@@ -40,6 +47,11 @@ struct B36 {
   __device__ static void yl0_dtheta(float t, float (&o)[NS]) { basis_dimenet_3_6::yl0_dtheta(t, o); }
   __device__ static void ylm_dtheta(float t, float p, float (&o)[NY]) { basis_dimenet_3_6::ylm_dtheta(t, p, o); }
   __device__ static void ylm_dphi(float t, float p, float (&o)[NY]) { basis_dimenet_3_6::ylm_dphi(t, p, o); }
+  __device__ static void bessel_dxx(float x, float (&o)[NB]) { basis_dimenet_3_6::bessel_dxx(x, o); }
+  __device__ static void yl0_dtheta2(float t, float (&o)[NS]) { basis_dimenet_3_6::yl0_dtheta2(t, o); }
+  __device__ static void ylm_dtheta2(float t, float p, float (&o)[NY]) { basis_dimenet_3_6::ylm_dtheta2(t, p, o); }
+  __device__ static void ylm_dtheta_dphi(float t, float p, float (&o)[NY]) { basis_dimenet_3_6::ylm_dtheta_dphi(t, p, o); }
+  __device__ static void ylm_dphi2(float t, float p, float (&o)[NY]) { basis_dimenet_3_6::ylm_dphi2(t, p, o); }
 };
 struct G23 {
   static constexpr int NS = basis_gemnet_2_3::NS, NR = basis_gemnet_2_3::NR;
@@ -1001,6 +1013,221 @@ triplet_basis_bwd_kernel(const float* __restrict__ bess, const float* __restrict
   if (lane == 0) ddist[kj] = acc_x * inv_cutoff;
 }
 
+// ------------------------------------------------------------------ reverse mode of the tangent kernels (Hessians)
+// The tangents above are first derivatives of the bases times the geometry tangents.  Their reverse mode in the VALUE
+// inputs (dist, angle, torsion) needs the second derivatives: the closed forms of generated/basis_<tag>_d2.cuh and
+//   env''(x) = 2/x^3 + a (p-1)(p-2) x^(p-3) + b p (p-1) x^(p-2) + c (p+1) p x^(p-1).
+// Their reverse mode in the tangent inputs is a first-order backward.  d(H v) = one reverse pass over the tangent
+// network along v (autograd_jvp.py), so these kernels are what reaches the positions from a force's gradient.
+__device__ __forceinline__ float envelope_dxx(float x, int p, float a, float b, float c) {
+  const float xp3 = powf(x, (float)(p - 3));
+  const float xp2 = xp3 * x, xp1 = xp2 * x;
+  return 2.0f / (x * x * x) + a * (float)((p - 1) * (p - 2)) * xp3 + b * (float)(p * (p - 1)) * xp2 +
+         c * (float)((p + 1) * p) * xp1;
+}
+
+// Reverse of rbf0_dot[e][n] = f_n'(x) xd  (f_n = env(x) sin(freq_n x), x = dist / cutoff, xd = dist_dot / cutoff)
+// given G = d(loss)/d(rbf0_dot):
+//   d_dist[e]     = sum_n G[e][n] f_n''(x) xd / cutoff,   d_dist_dot[e] = sum_n G[e][n] f_n'(x) / cutoff
+// and, when bess_dxx is given, d2(bess)/dx2 of the edge (enveloped as the forward's bess when env_on_bessel), which
+// triplet_basis_tangent_bwd reads.  One thread per edge, each output written once.
+template <class BS>
+__global__ void edge_basis_tangent_bwd_kernel(const float* __restrict__ dist, const float* __restrict__ dist_dot,
+                                              int n_edges, float inv_cutoff, int p, float ea, float eb, float ec,
+                                              const float* __restrict__ freq, int env_on_bessel,
+                                              const float* __restrict__ g_rbf0_dot, float* __restrict__ d_dist,
+                                              float* __restrict__ d_dist_dot, float* __restrict__ bess_dxx) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= n_edges) return;
+  const float x = __fmul_rn(dist[e], inv_cutoff);
+  const float env = envelope(x, p, ea, eb, ec), envd = envelope_dx(x, p, ea, eb, ec);
+  const float envdd = envelope_dxx(x, p, ea, eb, ec);
+  if (g_rbf0_dot) {
+    const float xd = dist_dot[e] * inv_cutoff;
+    float a1 = 0.f, a2 = 0.f;
+#pragma unroll
+    for (int n = 0; n < BS::NR; ++n) {
+      const float f = __ldg(freq + n);
+      float sn, cs;
+      sincosf(f * x, &sn, &cs);
+      const float gn = g_rbf0_dot[(size_t)e * BS::NR + n];
+      a1 = fmaf(gn, envd * sn + env * f * cs, a1);
+      a2 = fmaf(gn, envdd * sn + 2.0f * envd * f * cs - env * f * f * sn, a2);
+    }
+    d_dist[e] = a2 * xd * inv_cutoff;
+    d_dist_dot[e] = a1 * inv_cutoff;
+  }
+  if (bess_dxx) {
+    float b2[BS::NB];
+    BS::bessel_dxx(x, b2);
+    if (env_on_bessel) {
+      float b[BS::NB], b1[BS::NB];
+      BS::bessel(x, b);
+      BS::bessel_dx(x, b1);
+#pragma unroll
+      for (int c = 0; c < BS::NB; ++c) b2[c] = envdd * b[c] + 2.0f * envd * b1[c] + env * b2[c];
+    }
+#pragma unroll
+    for (int c = 0; c < BS::NB; ++c) bess_dxx[(size_t)e * BS::NB + c] = b2[c];
+  }
+}
+
+// Reverse of triplet_basis_tangent_kernel (with bess_dot = B'(x) xd folded in) in all of its inputs, given
+// Gs = d(loss)/d(sbf_dot) and Gt = d(loss)/d(tbf_dot).  Per triplet, with H_k[l] = sum_n Gs[l,n] B^(k)[kj][l,n]
+// (B, B', B'' the edge's Bessel values and x-derivatives) and Y = Y_l0(th):
+//   d_angle      = sum_l Y'' thd H0 + Y' xd H1         d_angle_dot = sum_l Y' H0
+//   d_x (kj)     = sum_l Y' thd H1 + Y xd H2           d_xd (kj)   = sum_l Y H1
+// and for the torsion branch, with Y = Y_ab(th, ph), Yd = Y_th thd + Y_ph phd and H_k[ab] = sum_r Gt[ab,r] B^(k)[b,r]:
+//   d_angle     += sum_ab (Y_thth thd + Y_thph phd) H0 + Y_th xd H1     d_angle_dot   += sum_ab Y_th H0
+//   d_torsion    = sum_ab (Y_thph thd + Y_phph phd) H0 + Y_ph xd H1     d_torsion_dot  = sum_ab Y_ph H0
+//   d_x         += sum_ab Yd H1 + Y xd H2                                d_xd          += sum_ab Y H1
+// (x-derivatives of the Bessel part: H1 / H2 with B', B'').
+// d_dist[kj] = sum d_x / cutoff and d_dist_dot[kj] = sum d_xd / cutoff over the triplets whose k->j edge is kj.  The
+// triplets of an edge are found as in triplet_basis_bwd_kernel (one warp per k->j edge, the out-edge lists of j), so
+// the edge sums are owned by one warp: no float atomics, the same bits on every run.
+template <class BS>
+__global__ void __launch_bounds__(TBB_WARPS * 32)
+triplet_basis_tangent_bwd_kernel(const float* __restrict__ bess, const float* __restrict__ bess_dx,
+                                 const float* __restrict__ bess_dxx, const float* __restrict__ dist_dot,
+                                 const float* __restrict__ angle, const float* __restrict__ angle_dot,
+                                 const float* __restrict__ torsion, const float* __restrict__ torsion_dot,
+                                 const int32_t* __restrict__ dst, const int32_t* __restrict__ row_ptr,
+                                 const int32_t* __restrict__ trip_ptr, const int32_t* __restrict__ out_ptr,
+                                 const int32_t* __restrict__ out_list, const int32_t* __restrict__ pos_in, int n_edges,
+                                 const float* __restrict__ g_sbf, const float* __restrict__ g_tbf, float inv_cutoff,
+                                 float* __restrict__ d_dist, float* __restrict__ d_dist_dot,
+                                 float* __restrict__ d_angle, float* __restrict__ d_angle_dot,
+                                 float* __restrict__ d_torsion, float* __restrict__ d_torsion_dot) {
+  constexpr int NS = BS::NS, NR = BS::NR, NB = BS::NB, NY = BS::NY;
+  __shared__ float sb[TBB_WARPS][3][NB];
+  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int kj = blockIdx.x * TBB_WARPS + w;
+  if (kj >= n_edges) return;                                   // uniform per warp
+  for (int c = lane; c < NB; c += 32) {
+    sb[w][0][c] = bess[(size_t)kj * NB + c];
+    sb[w][1][c] = bess_dx[(size_t)kj * NB + c];
+    sb[w][2][c] = bess_dxx[(size_t)kj * NB + c];
+  }
+  __syncwarp();
+  const float xd = dist_dot[kj] * inv_cutoff;
+  const int j = dst[kj], rank_k = kj - row_ptr[j];
+  const int o_lo = out_ptr[j], o_hi = out_ptr[j + 1];
+  float acc_x = 0.f, acc_xd = 0.f;
+  for (int o0 = o_lo; o0 < o_hi; o0 += 32) {
+    const int o = o0 + lane;
+    if (o >= o_hi) continue;
+    const int ji = out_list[o], rank_i = pos_in[ji];
+    if (rank_i == rank_k) continue;                            // i == k: no triplet
+    const int t = trip_ptr[ji] + rank_k - (rank_i < rank_k ? 1 : 0);
+    const float th = angle[t], thd = angle_dot[t];
+    float dth = 0.f, dthd = 0.f, dph = 0.f, dphd = 0.f, dx = 0.f, dxd = 0.f;
+    if (g_sbf) {
+      const float* gs = g_sbf + (size_t)t * NB;
+      float y0[NS], y1[NS], y2[NS];
+      BS::yl0(th, y0);
+      BS::yl0_dtheta(th, y1);
+      BS::yl0_dtheta2(th, y2);
+#pragma unroll
+      for (int l = 0; l < NS; ++l) {
+        float h0 = 0.f, h1 = 0.f, h2 = 0.f;
+#pragma unroll
+        for (int n = 0; n < NR; ++n) {
+          const float gr = gs[l * NR + n];
+          h0 = fmaf(gr, sb[w][0][l * NR + n], h0);
+          h1 = fmaf(gr, sb[w][1][l * NR + n], h1);
+          h2 = fmaf(gr, sb[w][2][l * NR + n], h2);
+        }
+        dth = fmaf(y2[l] * thd, h0, fmaf(y1[l] * xd, h1, dth));
+        dthd = fmaf(y1[l], h0, dthd);
+        dx = fmaf(y1[l] * thd, h1, fmaf(y0[l] * xd, h2, dx));
+        dxd = fmaf(y0[l], h1, dxd);
+      }
+    }
+    if (g_tbf) {
+      const float ph = torsion[t], phd = torsion_dot[t];
+      const float* gt = g_tbf + (size_t)t * (NY * NR);
+      // H0 is kept per (a, b); H1 / H2 are recomputed where they are read (registers: the harmonics take NY each)
+      auto hk = [&](int ab, int k) {
+        const int b = ab % NS;
+        float h = 0.f;
+#pragma unroll
+        for (int r = 0; r < NR; ++r) h = fmaf(gt[ab * NR + r], sb[w][k][b * NR + r], h);
+        return h;
+      };
+      float H0[NY];
+#pragma unroll
+      for (int ab = 0; ab < NY; ++ab) H0[ab] = hk(ab, 0);
+      {
+        float y[NY];
+        BS::ylm(th, ph, y);
+#pragma unroll
+        for (int ab = 0; ab < NY; ++ab) {
+          dx = fmaf(y[ab] * xd, hk(ab, 2), dx);
+          dxd = fmaf(y[ab], hk(ab, 1), dxd);
+        }
+      }
+      {
+        float y[NY];
+        BS::ylm_dtheta(th, ph, y);
+#pragma unroll
+        for (int ab = 0; ab < NY; ++ab) {
+          const float h1 = hk(ab, 1);
+          dth = fmaf(y[ab] * xd, h1, dth);
+          dthd = fmaf(y[ab], H0[ab], dthd);
+          dx = fmaf(y[ab] * thd, h1, dx);
+        }
+      }
+      {
+        float y[NY];
+        BS::ylm_dphi(th, ph, y);
+#pragma unroll
+        for (int ab = 0; ab < NY; ++ab) {
+          const float h1 = hk(ab, 1);
+          dph = fmaf(y[ab] * xd, h1, dph);
+          dphd = fmaf(y[ab], H0[ab], dphd);
+          dx = fmaf(y[ab] * phd, h1, dx);
+        }
+      }
+      {
+        float y[NY];
+        BS::ylm_dtheta2(th, ph, y);
+#pragma unroll
+        for (int ab = 0; ab < NY; ++ab) dth = fmaf(y[ab] * thd, H0[ab], dth);
+      }
+      {
+        float y[NY];
+        BS::ylm_dtheta_dphi(th, ph, y);
+#pragma unroll
+        for (int ab = 0; ab < NY; ++ab) {
+          dth = fmaf(y[ab] * phd, H0[ab], dth);
+          dph = fmaf(y[ab] * thd, H0[ab], dph);
+        }
+      }
+      {
+        float y[NY];
+        BS::ylm_dphi2(th, ph, y);
+#pragma unroll
+        for (int ab = 0; ab < NY; ++ab) dph = fmaf(y[ab] * phd, H0[ab], dph);
+      }
+    }
+    d_angle[t] = dth;
+    d_angle_dot[t] = dthd;
+    if (d_torsion) d_torsion[t] = dph;
+    if (d_torsion_dot) d_torsion_dot[t] = dphd;
+    acc_x += dx;
+    acc_xd += dxd;
+  }
+#pragma unroll
+  for (int off = 16; off; off >>= 1) {
+    acc_x += __shfl_xor_sync(0xffffffffu, acc_x, off);
+    acc_xd += __shfl_xor_sync(0xffffffffu, acc_xd, off);
+  }
+  if (lane == 0) {
+    d_dist[kj] = acc_x * inv_cutoff;
+    d_dist_dot[kj] = acc_xd * inv_cutoff;
+  }
+}
+
 // Backward of the fused projection w.r.t. the geometry (forces):
 //   sbf_p[q][t] = sum_l  Y_l0(angle_t)            Rs[q][l],   Rs[q][l]  = sum_r bess[kj][l,r]  w_sbf1[q][l,r]
 //   t_p[q][t]   = sum_ab Y_ab(angle_t, torsion_t) R[q][ab],   R[q][ab]  = sum_r bess[kj][b,r]  w_t1[q][ab,r]
@@ -1337,6 +1564,58 @@ int dig3d_triplet_basis_bwd(const float* bess, const float* bess_dx, const float
     case 0: triplet_basis_bwd_kernel<B76><<<grid, TBB_WARPS * 32, 0, st>>>(bess, bess_dx, angle, torsion, dst, row_ptr, trip_ptr, out_ptr, out_list, pos_in, (int)n_edges, d_sbf, d_tbf, inv, ddist, dangle, dtorsion); break;
     case 1: triplet_basis_bwd_kernel<B36><<<grid, TBB_WARPS * 32, 0, st>>>(bess, bess_dx, angle, torsion, dst, row_ptr, trip_ptr, out_ptr, out_list, pos_in, (int)n_edges, d_sbf, d_tbf, inv, ddist, dangle, dtorsion); break;
     default: set_error("triplet_basis_bwd: unsupported basis_id %d", basis_id); return DIG3D_EUNSUPPORTED;
+  }
+  DIG3D_LAUNCH_CHECK();
+  return DIG3D_OK;
+}
+
+int dig3d_edge_basis_tangent_bwd(const float* dist, const float* dist_dot, int64_t n_edges, double cutoff,
+                                 int32_t envelope_exponent, const float* freq, int32_t basis_id,
+                                 int32_t envelope_on_bessel, const float* g_rbf0_dot, float* d_dist, float* d_dist_dot,
+                                 float* bess_dxx, void* stream) {
+  DIG3D_REQUIRE(dist && (g_rbf0_dot || bess_dxx), "edge_basis_tangent_bwd: null pointer");
+  DIG3D_REQUIRE(!g_rbf0_dot || (dist_dot && freq && d_dist && d_dist_dot),
+                "edge_basis_tangent_bwd: g_rbf0_dot needs dist_dot, freq, d_dist and d_dist_dot");
+  DIG3D_REQUIRE(cutoff > 0.0, "edge_basis_tangent_bwd: cutoff must be positive");
+  if (n_edges == 0) return DIG3D_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int p = envelope_exponent + 1;
+  const float a = -(float)((p + 1) * (p + 2)) / 2.f, b = (float)(p * (p + 2)), c = -(float)(p * (p + 1)) / 2.f;
+  const float inv = 1.0f / (float)cutoff;
+  const int grid = ceil_div(n_edges, 128);
+  switch (basis_id) {
+    case 0: edge_basis_tangent_bwd_kernel<B76><<<grid, 128, 0, st>>>(dist, dist_dot, (int)n_edges, inv, p, a, b, c, freq, envelope_on_bessel, g_rbf0_dot, d_dist, d_dist_dot, bess_dxx); break;
+    case 1: edge_basis_tangent_bwd_kernel<B36><<<grid, 128, 0, st>>>(dist, dist_dot, (int)n_edges, inv, p, a, b, c, freq, envelope_on_bessel, g_rbf0_dot, d_dist, d_dist_dot, bess_dxx); break;
+    default: set_error("edge_basis_tangent_bwd: unsupported basis_id %d", basis_id); return DIG3D_EUNSUPPORTED;
+  }
+  DIG3D_LAUNCH_CHECK();
+  return DIG3D_OK;
+}
+
+int dig3d_triplet_basis_tangent_bwd(const float* bess, const float* bess_dx, const float* bess_dxx,
+                                    const float* dist_dot, const float* angle, const float* angle_dot,
+                                    const float* torsion, const float* torsion_dot, const int32_t* dst,
+                                    const int32_t* row_ptr, const int32_t* trip_ptr, const int32_t* out_ptr,
+                                    const int32_t* out_list, const int32_t* pos_in, int64_t n_edges,
+                                    int64_t n_triplets, int32_t basis_id, const float* g_sbf, const float* g_tbf,
+                                    double cutoff, float* d_dist, float* d_dist_dot, float* d_angle,
+                                    float* d_angle_dot, float* d_torsion, float* d_torsion_dot, void* stream) {
+  DIG3D_REQUIRE(cutoff > 0.0, "triplet_basis_tangent_bwd: cutoff must be positive");
+  if (n_edges == 0) return DIG3D_OK;
+  // without triplets every per-triplet buffer is empty (possibly NULL): only the edge outputs (zeros) are written
+  DIG3D_REQUIRE(bess && bess_dx && bess_dxx && dist_dot && dst && row_ptr && trip_ptr && out_ptr && out_list &&
+                    pos_in && d_dist && d_dist_dot && (n_triplets == 0 || (angle && angle_dot && d_angle && d_angle_dot)),
+                "triplet_basis_tangent_bwd: null pointer");
+  DIG3D_REQUIRE(n_triplets == 0 || !(g_tbf || d_torsion || d_torsion_dot) || (torsion && torsion_dot),
+                "triplet_basis_tangent_bwd: the torsion branch needs torsion and torsion_dot");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int grid = ceil_div(n_edges, TBB_WARPS);
+  const float inv = 1.0f / (float)cutoff;
+  if (n_triplets == 0) { g_sbf = nullptr; g_tbf = nullptr; d_torsion = nullptr; d_torsion_dot = nullptr; }
+  switch (basis_id) {
+    case 0: triplet_basis_tangent_bwd_kernel<B76><<<grid, TBB_WARPS * 32, 0, st>>>(bess, bess_dx, bess_dxx, dist_dot, angle, angle_dot, torsion, torsion_dot, dst, row_ptr, trip_ptr, out_ptr, out_list, pos_in, (int)n_edges, g_sbf, g_tbf, inv, d_dist, d_dist_dot, d_angle, d_angle_dot, d_torsion, d_torsion_dot); break;
+    case 1: triplet_basis_tangent_bwd_kernel<B36><<<grid, TBB_WARPS * 32, 0, st>>>(bess, bess_dx, bess_dxx, dist_dot, angle, angle_dot, torsion, torsion_dot, dst, row_ptr, trip_ptr, out_ptr, out_list, pos_in, (int)n_edges, g_sbf, g_tbf, inv, d_dist, d_dist_dot, d_angle, d_angle_dot, d_torsion, d_torsion_dot); break;
+    default: set_error("triplet_basis_tangent_bwd: unsupported basis_id %d", basis_id); return DIG3D_EUNSUPPORTED;
   }
   DIG3D_LAUNCH_CHECK();
   return DIG3D_OK;

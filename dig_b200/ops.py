@@ -1580,6 +1580,46 @@ def triplet_basis_tangent(bess, bess_dot, angle, angle_dot, torsion, torsion_dot
     return s_dot, t_dot
 
 
+def edge_basis_tangent_bwd(dist, dist_dot, cutoff, envelope_exponent, freq, basis_id, envelope_on_bessel, g_rbf0_dot,
+                           n_bessel=0, want_bess_dxx=False):
+    """Reverse of `edge_basis_tangent`'s rbf0_dot in its inputs: -> (d_dist [E], d_dist_dot [E]) given g_rbf0_dot (None:
+    both None), and bess_dxx [E, n_bessel] = d2(bess)/dx2 when want_bess_dxx (for `triplet_basis_tangent_bwd`)."""
+    e = dist.numel()
+    dev = dist.device
+    want_r = g_rbf0_dot is not None
+    d_d = torch.empty(e, device=dev, dtype=F32) if want_r else None
+    d_dd = torch.empty(e, device=dev, dtype=F32) if want_r else None
+    bdxx = torch.empty(e, n_bessel, device=dev, dtype=F32) if want_bess_dxx else None
+    if e and (want_r or want_bess_dxx):
+        call("dig3d_edge_basis_tangent_bwd", _p(dist, F32, "dist"), _p(dist_dot, F32, "dist_dot") if want_r else None,
+             e, float(cutoff), int(envelope_exponent), _p(freq.detach(), F32, "freq") if want_r else None,
+             int(basis_id), int(bool(envelope_on_bessel)), _p(g_rbf0_dot, F32, "g_rbf0_dot") if want_r else None,
+             _p(d_d), _p(d_dd), _p(bdxx), _stream())
+    return d_d, d_dd, bdxx
+
+
+def triplet_basis_tangent_bwd(g, bess, bess_dx, bess_dxx, dist_dot, angle, angle_dot, torsion, torsion_dot, basis_id,
+                              g_sbf, g_tbf, cutoff):
+    """Reverse of `triplet_basis_tangent` (bess_dot = bess_dx * dist_dot / cutoff) given g_sbf / g_tbf (either None) ->
+    (d_dist, d_dist_dot [E]; d_angle, d_angle_dot [T]; d_torsion, d_torsion_dot [T] | None when torsion is None).
+    Needs the graph's out-edge lists (`build_graph` makes them)."""
+    dev = bess.device
+    e, t = g.n_edges, angle.numel()
+    if g.out_ptr is None or g.out_list is None or g.pos_in is None:
+        raise ValueError("triplet_basis_tangent_bwd: the graph carries no out-edge lists (build it with ops.build_graph)")
+    tors = torsion is not None
+    outs = [torch.empty(n, device=dev, dtype=F32) for n in (e, e, t, t)]
+    outs += [torch.empty(t, device=dev, dtype=F32) for _ in range(2)] if tors else [None, None]
+    if e:
+        call("dig3d_triplet_basis_tangent_bwd", _p(bess, F32, "bess"), _p(bess_dx, F32, "bess_dx"),
+             _p(bess_dxx, F32, "bess_dxx"), _p(dist_dot, F32, "dist_dot"), _p(angle, F32, "angle"),
+             _p(angle_dot, F32, "angle_dot"), _p(torsion, F32, "torsion") if tors else None,
+             _p(torsion_dot, F32, "torsion_dot") if tors else None, _p(g.dst), _p(g.row_ptr), _p(g.trip_ptr),
+             _p(g.out_ptr), _p(g.out_list), _p(g.pos_in), e, t, int(basis_id), _p(g_sbf, F32, "g_sbf"),
+             _p(g_tbf, F32, "g_tbf"), float(cutoff), *[_p(o) for o in outs], _stream())
+    return tuple(outs)
+
+
 def edge_dist_bwd2(pos, g, ddist, g_dpos):
     """-> (d_ddist [E], d_pos [N,3]) of edge_dist_bwd given g_dpos = d(loss)/d(dpos)."""
     d_ddist = torch.zeros(g.n_edges, device=pos.device, dtype=F32)

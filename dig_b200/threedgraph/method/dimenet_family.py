@@ -267,13 +267,13 @@ class _DimeNetFamily(nn.Module):
                             z=z if with_emb else None, z_rows=self.init_e.emb.num_embeddings if with_emb else 0)
         if wants_grad(self) or self._generic:
             nf = getattr(batch_data, "node_feature", None)
-            if (self.training and torch.is_grad_enabled() and pos.requires_grad
-                    and any(p.requires_grad for p in self.parameters())):
-                # training ON forces (run.py:110-123): grad(out, pos, create_graph=True) must stay differentiable in the
-                # parameters -- reverse over forward mode, dig_b200/autograd_jvp.py
+            if torch.is_grad_enabled() and pos.requires_grad:
+                # forces: grad(out, pos, create_graph=True) stays differentiable in the parameters (training ON forces,
+                # run.py:110-123) and in pos (Hessian-vector products), in training and eval mode alike -- reverse over
+                # forward mode, dig_b200/autograd_jvp.py.  Energies and first-order forces are those of _forward_train.
                 return jv.energy_with_force(lambda p: self._exact(self._forward_train, z, p, g, nf),
                                             lambda p, c: self._exact(self._forward_dual, z, p, c, g, nf),
-                                            pos, tuple(self.parameters()))
+                                            pos, tuple(self.parameters()), second_order=True)
             return self._exact(self._forward_train, z, pos, g, nf, exact=bool(pos.requires_grad))
         # dense edge-MLP chain: "h16" (default) = register-accumulator engine, 3xFP16 operands (csrc/spherenet_h16.cu),
         # run from the cached plan below; "tc" = first-generation 3xTF32 chain with fp32 operand range
@@ -550,26 +550,37 @@ class _DimeNetFamily(nn.Module):
     def _forward_dual(self, z, pos, cvec, g, node_feature=None):
         """(E, E_dot): the forward of _forward_train carried together with its directional derivative along the per-atom
         displacement `cvec` [N, 3] (same reference lines, op for op), built on the first-order primitives so that
-        E_dot is differentiable in the parameters.  Positions are data here: geometry, its tangents and the angular
-        bases are constants; the radial basis is differentiable in dist_emb.freq.  See dig_b200/autograd_jvp.py."""
+        E_dot is differentiable in the parameters.  When pos requires grad (Hessian-vector products), the geometry, its
+        tangents and the bases are differentiable functions of pos as well: the reverse pass over E_dot then reaches pos
+        through the second derivatives of the geometry (csrc/train_geom.cu) and of the bases (csrc/basis.cu).
+        Otherwise positions are data: geometry, its tangents and the angular bases are constants and the radial basis is
+        differentiable in dist_emb.freq.  See dig_b200/autograd_jvp.py."""
         ns, nr = self.num_spherical, self.num_radial
         tors = self._torsion
-        pos = pos.detach()
+        hess = pos.requires_grad
         ops.triplet_geometry(g, pos, use_torsion=tors, want_idx=True)
-        d_dot, a_dot, t_dot = ops.geometry_jvp(pos, cvec, g, want_angle=True, want_torsion=tors)
-        dist, angle, tors_angle = g.dist.view(-1), g.angle.view(-1), (g.torsion.view(-1) if tors else None)
+        if hess and tors:
+            # the torsion's second derivatives follow the winning candidate of each triplet (g.tors_arg); the _arg
+            # variant rewrites angle / torsion with the same bits (the capped graph has in-degree <= 32: no heavy edge)
+            ops.triplet_geometry_any_degree_arg(g, pos, 0)
+        d_dot, a_dot, t_dot = jv.geometry_jvp(pos, cvec, g, tors)
+        if hess:
+            dist, angle, *rest = ag.geometry(pos, g, 3 if tors else 2)
+            tors_angle = rest[0] if tors else None
+        else:
+            dist, angle, tors_angle = g.dist.view(-1), g.angle.view(-1), (g.torsion.view(-1) if tors else None)
         freq = self.emb.dist_emb.freq
         cfg = (self.cutoff, self.envelope_exponent, self._basis_id, not tors, nr, ns * nr)
         rbf0, bess = ag.edge_basis(freq, dist, *cfg)
         rbf0_d = jv.edge_basis_tangent(freq, dist, d_dot, *cfg)
-        _, bess_d = ops.edge_basis_tangent(dist, d_dot, self.cutoff, self.envelope_exponent, None, self._basis_id,
-                                           not tors, nr, ns * nr, want_rbf0=False, want_bess=True)
-        sbf_d, tbf_d = ops.triplet_basis_tangent(bess, bess_d, angle, a_dot, tors_angle, t_dot, g.idx_kj,
-                                                 self._basis_id, ns, nr, want_tbf=tors)
+        sbf_d, tbf_d = jv.triplet_basis_tangent(dist, d_dot, angle, a_dot, tors_angle, t_dot, bess, g,
+                                                (self.cutoff, self.envelope_exponent, self._basis_id, not tors, ns, nr))
         geo_cfg = (self.cutoff, self.envelope_exponent, not tors, dist)
         L = self.num_layers
         sbf_ps, t_ps = [], []
-        if self._triplet_generic:          # materialised bases (constants here, with the tangents above)
+        if self._triplet_generic and hess:  # materialised bases, functions of the geometry
+            sbf, tbf = ag.triplet_basis(bess, dist, angle, tors_angle, g, geo_cfg[:3], self._basis_id, ns, nr, tors)
+        elif self._triplet_generic:         # materialised bases (constants here, with the tangents above)
             sbf, tbf = ops.triplet_basis(bess, angle, tors_angle, g.idx_kj, self._basis_id, ns, nr, tors)
         else:
             for first in range(0, L, 4):

@@ -143,7 +143,12 @@ class run():
                 loss = e_loss + p * f_loss
             else:
                 loss = loss_func(out, batch_data.y.unsqueeze(1))
-            loss.backward()
+            if energy_and_force:
+                # the force term also reaches batch_data.pos (its Hessian-vector product, autograd_jvp._ForceOp); the
+                # step only needs the parameters, so the position term is not computed
+                loss.backward(inputs=[q for q in model.parameters() if q.requires_grad])
+            else:
+                loss.backward()
             # data-parallel launch (one process per GPU, torch.distributed initialised): average the gradients of
             # the per-rank molecule shards; a no-op in the reference's single-process use
             parallel.allreduce_gradients(model.parameters())

@@ -141,9 +141,10 @@ class SchNet(nn.Module):
     def _forward_train(self, z, pos, g):
         """Differentiable forward (reference schnet.py:149-168 op for op) over dig_b200.autograd's primitives;
         used whenever autograd is recording, i.e. by run.train."""
-        # forces (run.py:126,165: autograd.grad(out, pos)): dist carries the position gradient.  Training ON forces
-        # differentiates that backward once more: use the twice-differentiable Functions (autograd_dd) then.
-        P = autograd_dd if (pos.requires_grad and any(p.requires_grad for p in self.parameters())) else ag
+        # forces (run.py:126,165: autograd.grad(out, pos)): dist carries the position gradient.  Training ON forces and
+        # second derivatives in pos (Hessians, also with every parameter frozen) differentiate that backward once more:
+        # the twice-differentiable Functions (autograd_dd) whenever pos requires grad.
+        P = autograd_dd if pos.requires_grad else ag
         dist = P.geometry(pos, g, 1) if pos.requires_grad else g.dist
         gauss, cut = P.schnet_edge_features(dist, self.dist_emb.offset, self.dist_emb.coeff, self.cutoff)
         v = P.gather_rows(self.init_v.weight, z)

@@ -693,6 +693,27 @@ int dig3d_rbf_freq_grad_tangent(const float* dist, const float* dist_dot, int64_
 int dig3d_triplet_basis_tangent(const float* bess, const float* bess_dot, const float* angle, const float* angle_dot,
                                 const float* torsion, const float* torsion_dot, const int32_t* idx_kj,
                                 int64_t n_triplets, int32_t basis_id, float* sbf_dot, float* tbf_dot, void* stream);
+/* Reverse mode of the tangents in their value inputs (Hessian-vector products of DimeNet++ / SphereNet):
+ * edge_basis_tangent_bwd: given g_rbf0_dot = d(loss)/d(rbf0_dot) [E,nr] (nullable), d_dist [E] (through d2 rbf0/dx2)
+ *   and d_dist_dot [E] (through d rbf0/dx); and, when bess_dxx is non-NULL, bess_dxx [E,ns*nr] = d2(bess)/dx2 (x = dist /
+ *   cutoff, enveloped like the forward's bess when envelope_on_bessel).  Every output is written, none accumulated.
+ * triplet_basis_tangent_bwd: reverse of triplet_basis_tangent with bess_dot = bess_dx * dist_dot / cutoff folded in,
+ *   given g_sbf [T, ns*nr] / g_tbf [T, ns*ns*nr] (either NULL = zero): d_dist / d_dist_dot [E] (the k->j edge's share,
+ *   summed by one warp per edge, no atomics) and d_angle / d_angle_dot / d_torsion / d_torsion_dot [T] (the torsion
+ *   pair nullable).  bess_dx from dig3d_edge_basis_bwd, bess_dxx from dig3d_edge_basis_tangent_bwd; needs the graph's
+ *   out-edge lists, like dig3d_triplet_basis_bwd. */
+int dig3d_edge_basis_tangent_bwd(const float* dist, const float* dist_dot, int64_t n_edges, double cutoff,
+                                 int32_t envelope_exponent, const float* freq, int32_t basis_id,
+                                 int32_t envelope_on_bessel, const float* g_rbf0_dot, float* d_dist, float* d_dist_dot,
+                                 float* bess_dxx, void* stream);
+int dig3d_triplet_basis_tangent_bwd(const float* bess, const float* bess_dx, const float* bess_dxx,
+                                    const float* dist_dot, const float* angle, const float* angle_dot,
+                                    const float* torsion, const float* torsion_dot, const int32_t* dst,
+                                    const int32_t* row_ptr, const int32_t* trip_ptr, const int32_t* out_ptr,
+                                    const int32_t* out_list, const int32_t* pos_in, int64_t n_edges,
+                                    int64_t n_triplets, int32_t basis_id, const float* g_sbf, const float* g_tbf,
+                                    double cutoff, float* d_dist, float* d_dist_dot, float* d_angle,
+                                    float* d_angle_dot, float* d_torsion, float* d_torsion_dot, void* stream);
 int dig3d_schnet_edge_features_bwd(const float* dist, int64_t n_edges, const float* offset, int32_t n_gauss,
                                    double coeff, double cutoff, const float* dgauss, const float* dcut, float* ddist,
                                    void* stream);
