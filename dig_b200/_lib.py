@@ -130,11 +130,13 @@ SIGNATURES = {
     "dig3d_comenet_geometry": [P, P, P, P, P, P, P, c_int64, c_int64, c_double, P, P, P, P, P],
     "dig3d_comenet_features_bwd": [P, P, P, P, P, P, P, P, c_int64, c_int64, c_double, P, P, P, P, P],
     "dig3d_comenet_features_tangent": [P, P, P, P, P, c_int64, c_int64, c_double, P, P, P, P],
+    "dig3d_comenet_features_tangent_bwd": [P, P, P, P, P, P, P, P, c_int64, c_int64, c_double, P, P, P, P, P, P],
     "dig3d_comenet_embed": [P, P, c_int64, P, P],
     "dig3d_pbc_edge_vectors": [P, P, P, P, P, c_int64, P, P, P],
     "dig3d_comenet_geometry_edges": [P, P, P, P, P, c_int64, c_int64, c_double, P, P, P, P, P, P],
     "dig3d_comenet_features_bwd_vec": [P, P, P, P, P, P, P, P, c_int64, c_int64, c_double, P, P, P, P, P],
     "dig3d_comenet_features_tangent_vec": [P, P, P, P, P, c_int64, c_int64, c_double, P, P, P, P],
+    "dig3d_comenet_features_tangent_bwd_vec": [P, P, P, P, P, P, P, P, c_int64, c_int64, c_double, P, P, P, P, P, P],
     "dig3d_pbc_cell_bwd": [P, P, P, P, c_int64, P, P],
     "dig3d_radius_graph_pbc_count": [P, P, P, c_int64, c_int64, c_double, c_int32, P, P, P, P, P, P, P],
     "dig3d_radius_graph_pbc_fill": [P, P, c_int64, c_int64, c_double, P, P, P, P, c_int64, P, P, P, P],

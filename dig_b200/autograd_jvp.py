@@ -22,6 +22,9 @@ grad_fn (`_ForceOp`), and a backward through it reaches the parameters and, when
   _EdgeBasisTangent     d(rbf0)/d(dist) * dist_dot, differentiable in dist_emb.freq, dist and dist_dot
   _TripletBasisTangent  the tangents of the materialised angular bases, differentiable in the geometry and its tangents
   _GeometryJVP          the geometry tangents J(pos) c, differentiable in pos and c
+  _ComenetFeaturesTangent / _ComenetOcpFeaturesTangent
+                        ComENet's feature tangents J(pos) c, differentiable in pos (csrc/comenet.cu
+                        `features_tangent_bwd`)
   graphnorm_dual        GraphNorm and its tangent (ComENet), differentiable in h, h_dot, weight and mean_scale
   energy_with_force     wraps a model's first-order forward + dual forward
 """
@@ -245,6 +248,63 @@ class _GeometryJVP(torch.autograd.Function):
 
 def geometry_jvp(pos, cvec, g, want_torsion):
     return _GeometryJVP.apply(pos, cvec, g, want_torsion)
+
+
+class _ComenetFeaturesTangent(torch.autograd.Function):
+    """ComENet's (feature1_dot [E,12], feature2_dot [E,6]) = J(pos) cvec (ops.comenet_features_tangent), differentiable
+    in pos: backward = ops.comenet_features_tangent_bwd, the features' second derivatives along cvec.  cvec is a
+    constant (the force's cotangent in _ForceOp)."""
+
+    @staticmethod
+    def forward(ctx, pos, g, cutoff, cvec):
+        pos, cvec = _c(pos.detach()), _c(cvec.detach())
+        ctx.g, ctx.cutoff = g, cutoff
+        ctx.save_for_backward(pos, cvec)
+        ctx.set_materialize_grads(False)
+        return ops.comenet_features_tangent(g, pos, cutoff, cvec)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g1, g2):
+        pos, cvec = ctx.saved_tensors
+        if g1 is None and g2 is None:
+            return (None,) * 4
+        e = ctx.g.n_edges
+        g1 = torch.zeros(e, 12, dtype=torch.float32, device=pos.device) if g1 is None else _c(g1)
+        g2 = torch.zeros(e, 6, dtype=torch.float32, device=pos.device) if g2 is None else _c(g2)
+        return ops.comenet_features_tangent_bwd(ctx.g, pos, ctx.cutoff, cvec, g1, g2), None, None, None
+
+
+def comenet_features_tangent(pos, g, cutoff, cvec):
+    return _ComenetFeaturesTangent.apply(pos, g, cutoff, cvec)
+
+
+class _ComenetOcpFeaturesTangent(torch.autograd.Function):
+    """ComENet-OCP's feature tangents along cvec, the cell held fixed (ops.comenet_ocp_features_tangent), differentiable
+    in pos: backward = ops.comenet_ocp_features_tangent_bwd.  The edge vectors are those of the graph view gv."""
+
+    @staticmethod
+    def forward(ctx, pos, gv, cutoff, cvec):
+        cvec = _c(cvec.detach())
+        ctx.gv, ctx.cutoff = gv, cutoff
+        ctx.save_for_backward(cvec)
+        ctx.set_materialize_grads(False)
+        return ops.comenet_ocp_features_tangent(gv, cutoff, cvec)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g1, g2):
+        (cvec,) = ctx.saved_tensors
+        if g1 is None and g2 is None:
+            return (None,) * 4
+        e, dev = ctx.gv.n_edges, cvec.device
+        g1 = torch.zeros(e, 12, dtype=torch.float32, device=dev) if g1 is None else _c(g1)
+        g2 = torch.zeros(e, 6, dtype=torch.float32, device=dev) if g2 is None else _c(g2)
+        return ops.comenet_ocp_features_tangent_bwd(ctx.gv, ctx.cutoff, cvec, g1, g2), None, None, None
+
+
+def comenet_ocp_features_tangent(pos, gv, cutoff, cvec):
+    return _ComenetOcpFeaturesTangent.apply(pos, gv, cutoff, cvec)
 
 
 # ----------------------------------------------------------------------------- energy with a twice-usable force

@@ -214,8 +214,8 @@ CONFIGS = {
     "gemnet_2_3": ("gemnet", 2, 3),        # ComENet defaults
     "gemnet_2_6": ("gemnet", 2, 6),        # ProNet defaults (pronet/features.py is comenet/features.py with nr = 6)
 }
-# configurations with a second-order header (DimeNet++ / SphereNet Hessians)
-SECOND_ORDER = ("dimenet_7_6", "dimenet_3_6")
+# configurations with a second-order header (DimeNet++ / SphereNet / ComENet Hessians)
+SECOND_ORDER = ("dimenet_7_6", "dimenet_3_6", "gemnet_2_3")
 
 
 def generate_all(out_dir, force=False):

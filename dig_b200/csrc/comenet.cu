@@ -11,7 +11,9 @@
 // kernels 32 nodes; the [E, 256] edge filters and messages of the two convolutions never reach HBM
 // (the reference materialises both, 31 MB each per 16 structures).
 #include "dense.cuh"
+#include "dual.cuh"
 #include "generated/basis_gemnet_2_3.cuh"
+#include "generated/basis_gemnet_2_3_d2.cuh"
 
 namespace dig3d {
 
@@ -484,6 +486,185 @@ __global__ void comenet_features_tangent_kernel(const float* __restrict__ pos, c
     }
 }
 
+// ------------------------------------------------------------------ Hessian-vector products: reverse of the tangent
+// dpos = sum_e sum_k g_k (d2 f_k / dpos2) cvec with g1 / g2 = d loss / d f1_dot / f2_dot: the reverse of the tangent
+// kernel above in the positions (its reverse in cvec is features_bwd itself).  It is d/de of J(pos + e cvec)^T g, so
+// this is pass 1 of the backward evaluated on dual numbers (value, tangent along cvec) seeded with df1 = g1,
+// df2 = g2; the tangent part of the five edge-vector gradients then goes through the backward's gather and node passes,
+// which are linear and do not depend on pos.  The values, partials and aliasing flags are those of the first-order
+// kernels and the intermediate tangents those of the tangent kernel, so the conventions carry over: the reference atoms
+// are constant, an aliased cross product is a constant (its value the residue, its tangent 0, its gradient terms 0),
+// and a zero norm or atan2(0, 0) passes nothing in either part.
+struct df3 {
+  dual x, y, z;
+};
+__device__ __forceinline__ df3 make_df3(const f3 v, const f3 t) { return {{v.x, t.x}, {v.y, t.y}, {v.z, t.z}}; }
+__device__ __forceinline__ f3 tangent3(const df3 a) { return {a.x.d, a.y.d, a.z.d}; }
+__device__ __forceinline__ dual scale(const dual a, float s) { return {a.v * s, a.d * s}; }
+__device__ __forceinline__ dual fmad(const dual a, const dual b, const dual c) {
+  return {fmaf(a.v, b.v, c.v), fmaf(a.d, b.v, fmaf(a.v, b.d, c.d))};
+}
+__device__ __forceinline__ df3 neg3(const df3 a) { return {-a.x, -a.y, -a.z}; }
+__device__ __forceinline__ df3 add3(const df3 a, const df3 b) { return {a.x + b.x, a.y + b.y, a.z + b.z}; }
+__device__ __forceinline__ df3 sub3(const df3 a, const df3 b) { return {a.x - b.x, a.y - b.y, a.z - b.z}; }
+__device__ __forceinline__ df3 scale3(const df3 a, const dual s) { return {a.x * s, a.y * s, a.z * s}; }
+__device__ __forceinline__ df3 axpy3(const dual s, const df3 a, const df3 b) {
+  return {fmad(s, a.x, b.x), fmad(s, a.y, b.y), fmad(s, a.z, b.z)};
+}
+__device__ __forceinline__ df3 cross3(const df3 a, const df3 b) {
+  return {a.y * b.z - a.z * b.y, a.z * b.x - a.x * b.z, a.x * b.y - a.y * b.x};
+}
+// atan2_partials with their tangents; py / px are atan2_partials' values at (y.v, x.v)
+__device__ __forceinline__ void atan2_partials_dual(const dual y, const dual x, float py, float px, dual& Py, dual& Px) {
+  const float den = fmaf(x.v, x.v, y.v * y.v);
+  if (den == 0.f) { Py = {0.f, 0.f}; Px = {0.f, 0.f}; return; }
+  const float dden = 2.f * fmaf(x.v, x.d, y.v * y.d);
+  Py = {py, (x.d - py * dden) / den};
+  Px = {px, (-y.d - px * dden) / den};
+}
+
+// Pass 1 on duals: work[e][role][3] = the tangent of pass 1's five edge-vector gradients (same roles)
+template <bool FROM_VEC>
+__global__ void comenet_features_tangent_bwd_edge_kernel(const float* __restrict__ pos, const float* __restrict__ dist,
+                                                         const int32_t* __restrict__ src, const int32_t* __restrict__ dst,
+                                                         const int32_t* __restrict__ a0_in,
+                                                         const int32_t* __restrict__ a1_in,
+                                                         const int32_t* __restrict__ a0_out,
+                                                         const int32_t* __restrict__ a1_out, int n_edges,
+                                                         float inv_cutoff, const float* __restrict__ cvec,
+                                                         const float* __restrict__ g1, const float* __restrict__ g2,
+                                                         float* __restrict__ work) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= n_edges) return;
+  const ComenetEdgeRefs r = comenet_edge_refs(src, dst, a0_in, a1_in, a0_out, a1_out, e);
+  const ComenetEdgeGeom G = comenet_edge_geom<FROM_VEC>(pos, src, dst, e, r);
+  const ComenetEdgePartials P = comenet_edge_partials<FROM_VEC>(G, r, e, src, dst);
+  ComenetEdgeBasis B;
+  const float x = __fmul_rn(dist[e], inv_cutoff);
+  comenet_edge_basis(x, G, B);
+  // the tangents along cvec, as comenet_features_tangent_kernel computes them
+  const f3 zero = {0.f, 0.f, 0.f};
+  const f3 dP = edge_vec<false>(cvec, src, dst, e), dA = edge_vec<false>(cvec, src, dst, r.e0i);
+  const f3 dB = edge_vec<false>(cvec, src, dst, r.e1i), dR = edge_vec<false>(cvec, src, dst, r.iref);
+  const f3 dS = edge_vec<false>(cvec, src, dst, r.jref);
+  const f3 Mv = neg3(G.pji), dM = neg3(dP);
+  const float ddist = dot3(G.pji, dP) * P.inv_d;
+  const f3 dpl1 = P.pl1_0 ? zero : add3(cross3(dM, G.in0), cross3(Mv, dA));
+  const float da1 = dot3(dM, G.in0) + dot3(Mv, dA);
+  const float db1 = dot3(G.pl1, dpl1) * P.inv_b1;
+  const float dth = fmaf(P.th_b1, db1, P.th_a1 * da1);
+  const float dd = dot3(G.pji, dP) / G.d;
+  const f3 dpl2 = P.pl2_0 ? zero : add3(cross3(dM, G.in1), cross3(Mv, dB));
+  const float da2 = dot3(dpl1, G.pl2) + dot3(G.pl1, dpl2);
+  const f3 dc2 = P.c2_0 ? zero : add3(cross3(dpl1, G.pl2), cross3(G.pl1, dpl2));
+  const float ds2 = dot3(dc2, G.pji) + dot3(G.c2, dP);
+  const float db2 = ds2 / G.d - G.s2 * dd / (G.d * G.d);
+  const float dph = fmaf(P.ph_b2, db2, P.ph_a2 * da2);
+  const f3 dq1 = P.q1_0 ? zero : add3(cross3(dP, G.jref), cross3(G.pji, dS));
+  const f3 dq2 = P.q2_0 ? zero : add3(cross3(dP, G.iref), cross3(G.pji, dR));
+  const float da3 = dot3(dq1, G.q2) + dot3(G.q1, dq2);
+  const f3 dc3 = P.c3_0 ? zero : add3(cross3(dq1, G.q2), cross3(G.q1, dq2));
+  const float ds3 = dot3(dc3, G.pji) + dot3(G.c3, dP);
+  const float db3 = ds3 / G.d - G.s3 * dd / (G.d * G.d);
+  const float dta = fmaf(P.ta_b3, db3, P.ta_a3 * da3);
+  // the basis and its first derivatives as duals (tangents from the generated second derivatives)
+  float rbdd[6], y0dd[2], ytt[4], ytp[4], ypp[4];
+  basis_gemnet_2_3::bessel_dxx(x, rbdd);
+  basis_gemnet_2_3::yl0_dtheta2(G.tau, y0dd);
+  basis_gemnet_2_3::ylm_dtheta2(G.theta, G.phi, ytt);
+  basis_gemnet_2_3::ylm_dtheta_dphi(G.theta, G.phi, ytp);
+  basis_gemnet_2_3::ylm_dphi2(G.theta, G.phi, ypp);
+  const float dx = ddist * inv_cutoff;
+  dual rb[6], rbd[6], y0[2], y0d[2], ylm[4], ylmt[4], ylmp[4];
+#pragma unroll
+  for (int k = 0; k < 6; ++k) { rb[k] = {B.rb[k], B.rbd[k] * dx}; rbd[k] = {B.rbd[k], rbdd[k] * dx}; }
+#pragma unroll
+  for (int l = 0; l < 2; ++l) { y0[l] = {B.y0[l], B.y0d[l] * dta}; y0d[l] = {B.y0d[l], y0dd[l] * dta}; }
+#pragma unroll
+  for (int h = 0; h < 4; ++h) {
+    ylm[h] = {B.ylm[h], fmaf(B.ylmt[h], dth, B.ylmp[h] * dph)};
+    ylmt[h] = {B.ylmt[h], fmaf(ytt[h], dth, ytp[h] * dph)};
+    ylmp[h] = {B.ylmp[h], fmaf(ytp[h], dth, ypp[h] * dph)};
+  }
+  // features -> d(rbf), d theta, d phi, d tau (pass 1, on duals)
+  const dual dz = {0.f, 0.f};
+  dual grb[6] = {dz, dz, dz, dz, dz, dz};
+  dual gth = dz, gph = dz, gta = dz;
+#pragma unroll
+  for (int l = 0; l < 2; ++l)
+#pragma unroll
+    for (int q = 0; q < 3; ++q) {
+      const float g = __ldg(g2 + (size_t)e * NF2 + l * 3 + q);
+      grb[l * 3 + q] = fmad(dual{g, 0.f}, y0[l], grb[l * 3 + q]);
+      gta = fmad(scale(rb[l * 3 + q], g), y0d[l], gta);
+    }
+#pragma unroll
+  for (int h = 0; h < 4; ++h)
+#pragma unroll
+    for (int q = 0; q < 3; ++q) {
+      const int k = (h == 0 ? 0 : 1) * 3 + q;
+      const float g = __ldg(g1 + (size_t)e * NF1 + h * 3 + q);
+      grb[k] = fmad(dual{g, 0.f}, ylm[h], grb[k]);
+      gth = fmad(scale(rb[k], g), ylmt[h], gth);
+      gph = fmad(scale(rb[k], g), ylmp[h], gph);
+    }
+  dual gx = dz;
+#pragma unroll
+  for (int k = 0; k < 6; ++k) gx = fmad(grb[k], rbd[k], gx);
+  const dual gdist = scale(gx, inv_cutoff);
+  // angles -> vectors
+  const df3 pji = make_df3(G.pji, dP), M = make_df3(Mv, dM), in0 = make_df3(G.in0, dA), in1 = make_df3(G.in1, dB);
+  const df3 iref = make_df3(G.iref, dR), jref = make_df3(G.jref, dS);
+  const df3 pl1 = make_df3(G.pl1, dpl1), pl2 = make_df3(G.pl2, dpl2), c2 = make_df3(G.c2, dc2);
+  const df3 q1 = make_df3(G.q1, dq1), q2 = make_df3(G.q2, dq2), c3 = make_df3(G.c3, dc3);
+  const df3 zd = {dz, dz, dz};
+  const dual d = {G.d, dd}, s2 = {G.s2, ds2}, s3 = {G.s3, ds3};
+  const dual inv_d = {P.inv_d, -P.inv_d * P.inv_d * dd}, inv_b1 = {P.inv_b1, -P.inv_b1 * P.inv_b1 * db1};
+  dual th_b1, th_a1, ph_b2, ph_a2, ta_b3, ta_a3;
+  atan2_partials_dual({G.b1, db1}, {G.a1, da1}, P.th_b1, P.th_a1, th_b1, th_a1);
+  atan2_partials_dual({__fdiv_rn(G.s2, G.d), db2}, {G.a2, da2}, P.ph_b2, P.ph_a2, ph_b2, ph_a2);
+  atan2_partials_dual({__fdiv_rn(G.s3, G.d), db3}, {G.a3, da3}, P.ta_b3, P.ta_a3, ta_b3, ta_a3);
+  df3 gP = scale3(pji, gdist * inv_d), gM = zd, gA = zd;
+  // theta = atan2(|pl1|, M . in0)
+  const dual g_a1 = gth * th_a1;
+  df3 gpl1 = scale3(pl1, gth * th_b1 * inv_b1);
+  gM = axpy3(g_a1, in0, gM);
+  gA = axpy3(g_a1, M, gA);
+  // phi = atan2(s2 / d, pl1 . pl2), s2 = (pl1 x pl2) . pji
+  const dual g_b2 = gph * ph_b2, g_a2 = gph * ph_a2;
+  const dual g_s2 = g_b2 / d;
+  dual g_d = -g_b2 * s2 / (d * d);
+  const df3 gc2 = P.c2_0 ? zd : scale3(pji, g_s2);
+  gP = axpy3(g_s2, c2, gP);
+  gpl1 = add3(gpl1, axpy3(g_a2, pl2, cross3(pl2, gc2)));
+  df3 gpl2 = axpy3(g_a2, pl1, cross3(gc2, pl1));
+  if (P.pl1_0) gpl1 = zd;
+  if (P.pl2_0) gpl2 = zd;
+  // tau = atan2(s3 / d, q1 . q2), s3 = (q1 x q2) . pji, q1 = pji x jref, q2 = pji x iref
+  const dual g_b3 = gta * ta_b3, g_a3 = gta * ta_a3;
+  const dual g_s3 = g_b3 / d;
+  g_d = g_d - g_b3 * s3 / (d * d);
+  const df3 gc3 = P.c3_0 ? zd : scale3(pji, g_s3);
+  gP = axpy3(g_s3, c3, gP);
+  df3 gq1 = axpy3(g_a3, q2, cross3(q2, gc3));
+  df3 gq2 = axpy3(g_a3, q1, cross3(gc3, q1));
+  if (P.q1_0) gq1 = zd;
+  if (P.q2_0) gq2 = zd;
+  gP = add3(gP, add3(cross3(jref, gq1), cross3(iref, gq2)));
+  const df3 gS = cross3(gq1, pji), gR = cross3(gq2, pji);
+  // d = sqrt(sum(pji^2)) of phi / tau
+  gP = axpy3(g_d / d, pji, gP);
+  // pl1 = M x in0, pl2 = M x in1
+  gM = add3(gM, add3(cross3(in0, gpl1), cross3(in1, gpl2)));
+  gA = add3(gA, cross3(gpl1, M));
+  const df3 gB = cross3(gpl2, M);
+  gP = sub3(gP, gM);
+  float* w = work + (size_t)e * 15;
+  const f3 out[5] = {tangent3(gP), tangent3(gA), tangent3(gB), tangent3(gR), tangent3(gS)};
+#pragma unroll
+  for (int k = 0; k < 5; ++k) { w[3 * k] = out[k].x; w[3 * k + 1] = out[k].y; w[3 * k + 2] = out[k].z; }
+}
+
 // ------------------------------------------------------------------ OCP variant: arbitrary edge lists, periodic images
 // distance_vec = pos[row] - pos[col] + cell_offsets . cell[graph of the edge]      (ocpmodels get_pbc_distances, called
 // at comenet-ocp.py:352-359; row = edge_index[0] = source j, col = edge_index[1] = target i)
@@ -932,6 +1113,24 @@ int dig3d_comenet_geometry(const float* pos, const float* dist, const int32_t* s
 
 }  // extern "C"
 
+// Passes 2 and 3 of the features backward: work[0, 15E) (the five edge-vector gradients of every edge) -> dvec =
+// work[15E, 18E) -> dpos
+static int comenet_vec_grads_to_dpos(const int32_t* src, const int32_t* dst, const int32_t* row_ptr,
+                                     const int32_t* out_ptr, const int32_t* out_list, const int32_t* refs,
+                                     int64_t n_nodes, int64_t n_edges, float* work, float* dpos, cudaStream_t st) {
+  float* dvec = work + 15 * n_edges;
+  if (n_edges) {
+    comenet_features_bwd_gather_kernel<<<ceil_div(n_edges, 128), 128, 0, st>>>(
+        src, dst, row_ptr, out_ptr, out_list, refs, refs + n_nodes, refs + 2 * n_nodes, refs + 3 * n_nodes,
+        (int)n_edges, work, dvec);
+    DIG3D_LAUNCH_CHECK();
+  }
+  comenet_features_bwd_node_kernel<<<ceil_div(n_nodes, 128), 128, 0, st>>>(row_ptr, out_ptr, out_list, (int)n_nodes,
+                                                                           dvec, dpos);
+  DIG3D_LAUNCH_CHECK();
+  return DIG3D_OK;
+}
+
 // The three passes of the features backward (pos [N,3], or FROM_VEC: vec [E,3]) and the tangent kernel's launch
 template <bool FROM_VEC>
 static int comenet_features_bwd_launch(const float* pos, const float* dist, const int32_t* src, const int32_t* dst,
@@ -943,19 +1142,12 @@ static int comenet_features_bwd_launch(const float* pos, const float* dist, cons
   cudaStream_t st = (cudaStream_t)stream;
   const int32_t* a0i = refs; const int32_t* a1i = refs + n_nodes;
   const int32_t* a0o = refs + 2 * n_nodes; const int32_t* a1o = refs + 3 * n_nodes;
-  float* dvec = work + 15 * n_edges;
   if (n_edges) {
     comenet_features_bwd_edge_kernel<FROM_VEC><<<ceil_div(n_edges, 128), 128, 0, st>>>(
         pos, dist, src, dst, a0i, a1i, a0o, a1o, (int)n_edges, 1.0f / (float)cutoff, dfeature1, dfeature2, work);
     DIG3D_LAUNCH_CHECK();
-    comenet_features_bwd_gather_kernel<<<ceil_div(n_edges, 128), 128, 0, st>>>(
-        src, dst, row_ptr, out_ptr, out_list, a0i, a1i, a0o, a1o, (int)n_edges, work, dvec);
-    DIG3D_LAUNCH_CHECK();
   }
-  comenet_features_bwd_node_kernel<<<ceil_div(n_nodes, 128), 128, 0, st>>>(row_ptr, out_ptr, out_list, (int)n_nodes,
-                                                                           dvec, dpos);
-  DIG3D_LAUNCH_CHECK();
-  return DIG3D_OK;
+  return comenet_vec_grads_to_dpos(src, dst, row_ptr, out_ptr, out_list, refs, n_nodes, n_edges, work, dpos, st);
 }
 
 template <bool FROM_VEC>
@@ -968,6 +1160,24 @@ static int comenet_features_tangent_launch(const float* pos, const float* dist, 
       1.0f / (float)cutoff, cvec, feature1_dot, feature2_dot);
   DIG3D_LAUNCH_CHECK();
   return DIG3D_OK;
+}
+
+// The reverse of the tangent in the positions: pass 1 on duals, then passes 2 and 3 of the backward
+template <bool FROM_VEC>
+static int comenet_features_tangent_bwd_launch(const float* pos, const float* dist, const int32_t* src,
+                                               const int32_t* dst, const int32_t* row_ptr, const int32_t* out_ptr,
+                                               const int32_t* out_list, const int32_t* refs, int64_t n_nodes,
+                                               int64_t n_edges, double cutoff, const float* cvec, const float* g1,
+                                               const float* g2, float* work, float* dpos, void* stream) {
+  if (n_nodes == 0) return DIG3D_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (n_edges) {
+    comenet_features_tangent_bwd_edge_kernel<FROM_VEC><<<ceil_div(n_edges, 128), 128, 0, st>>>(
+        pos, dist, src, dst, refs, refs + n_nodes, refs + 2 * n_nodes, refs + 3 * n_nodes, (int)n_edges,
+        1.0f / (float)cutoff, cvec, g1, g2, work);
+    DIG3D_LAUNCH_CHECK();
+  }
+  return comenet_vec_grads_to_dpos(src, dst, row_ptr, out_ptr, out_list, refs, n_nodes, n_edges, work, dpos, st);
 }
 
 extern "C" {
@@ -1010,6 +1220,28 @@ int dig3d_comenet_features_tangent_vec(const float* vec, const float* dist, cons
                 "comenet_features_tangent_vec: null pointer");
   return comenet_features_tangent_launch<true>(vec, dist, src, dst, refs, n_nodes, n_edges, cutoff, cvec,
                                                feature1_dot, feature2_dot, stream);
+}
+
+int dig3d_comenet_features_tangent_bwd(const float* pos, const float* dist, const int32_t* src, const int32_t* dst,
+                                       const int32_t* row_ptr, const int32_t* out_ptr, const int32_t* out_list,
+                                       const int32_t* refs, int64_t n_nodes, int64_t n_edges, double cutoff,
+                                       const float* cvec, const float* g1, const float* g2, float* work, float* dpos,
+                                       void* stream) {
+  DIG3D_REQUIRE(pos && dist && src && dst && row_ptr && out_ptr && out_list && refs && cvec && g1 && g2 && work &&
+                    dpos, "comenet_features_tangent_bwd: null pointer");
+  return comenet_features_tangent_bwd_launch<false>(pos, dist, src, dst, row_ptr, out_ptr, out_list, refs, n_nodes,
+                                                    n_edges, cutoff, cvec, g1, g2, work, dpos, stream);
+}
+
+int dig3d_comenet_features_tangent_bwd_vec(const float* vec, const float* dist, const int32_t* src,
+                                           const int32_t* dst, const int32_t* row_ptr, const int32_t* out_ptr,
+                                           const int32_t* out_list, const int32_t* refs, int64_t n_nodes,
+                                           int64_t n_edges, double cutoff, const float* cvec, const float* g1,
+                                           const float* g2, float* work, float* dpos, void* stream) {
+  DIG3D_REQUIRE(vec && dist && src && dst && row_ptr && out_ptr && out_list && refs && cvec && g1 && g2 && work &&
+                    dpos, "comenet_features_tangent_bwd_vec: null pointer");
+  return comenet_features_tangent_bwd_launch<true>(vec, dist, src, dst, row_ptr, out_ptr, out_list, refs, n_nodes,
+                                                   n_edges, cutoff, cvec, g1, g2, work, dpos, stream);
 }
 
 int dig3d_pbc_cell_bwd(const float* dvec, const float* cell_offsets, const int32_t* row_ptr, const int32_t* graph_ptr,

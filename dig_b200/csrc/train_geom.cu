@@ -7,6 +7,7 @@
 //
 //   triplet_torsion_bwd  torsion[t] = min_c dihedral(k, j->i, c)              geometric_computing.py:53-75
 #include "common.cuh"
+#include "dual.cuh"
 
 namespace dig3d {
 
@@ -388,25 +389,7 @@ triplet_torsion_jvp_kernel(const float* __restrict__ pos, const float* __restric
 // tangent of |w| at w = 0 is taken as 0; a^2 + b^2 = 0 and |ji| = 0 pass nothing; the self candidate c = k is the
 // constant 2 pi or its rounding residue (plane1 x plane1) and passes nothing.  The derivative kernels of the models
 // (triplet_angle_bwd_kernel above, shared and unchanged) form cross products with ATen's fused rounding instead.
-struct dual {
-  float v, d;
-};
-__device__ __forceinline__ float val(float a) { return a; }
-__device__ __forceinline__ float val(dual a) { return a.v; }
-__device__ __forceinline__ dual operator+(dual a, dual b) { return {a.v + b.v, a.d + b.d}; }
-__device__ __forceinline__ dual operator-(dual a, dual b) { return {a.v - b.v, a.d - b.d}; }
-__device__ __forceinline__ dual operator-(dual a) { return {-a.v, -a.d}; }
-__device__ __forceinline__ dual operator*(dual a, dual b) { return {a.v * b.v, a.d * b.v + a.v * b.d}; }
-__device__ __forceinline__ dual operator/(dual a, dual b) {
-  const float q = a.v / b.v;
-  return {q, (a.d - q * b.d) / b.v};
-}
-__device__ __forceinline__ float sqrt_t(float a) { return sqrtf(a); }
-__device__ __forceinline__ dual sqrt_t(dual a) {
-  const float r = sqrtf(a.v);
-  return {r, r > 0.f ? a.d / (2.f * r) : 0.f};
-}
-
+// `dual` and its arithmetic: dual.cuh.
 template <typename T>
 struct v3 {
   T x, y, z;

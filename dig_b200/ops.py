@@ -586,6 +586,21 @@ def comenet_features_tangent(g, pos, cutoff, cvec):
     return f1d, f2d
 
 
+def comenet_features_tangent_bwd(g, pos, cutoff, cvec, g1, g2):
+    """dpos [N, 3] = d/dpos of sum(g1 * feature1_dot + g2 * feature2_dot) with cvec held constant: the Hessian-vector
+    products sum_k g_k (d2 f_k / dpos2) cvec of comenet_features_tangent's features.  Deterministic (no float
+    atomics)."""
+    p = _comenet_force_inputs(g, pos)
+    e, n = g.n_edges, g.n_nodes
+    dpos = torch.empty(n, 3, dtype=F32, device=pos.device)
+    work = torch.empty(max(18 * e, 1), dtype=F32, device=pos.device)
+    if n:
+        call("dig3d_comenet_features_tangent_bwd", p, _p(g.dist), _p(g.src), _p(g.dst), _p(g.row_ptr), _p(g.out_ptr),
+             _p(g.out_list), _p(g.comenet_refs), n, e, float(cutoff), _p(cvec, F32, "cvec"), _p(g1, F32, "g1"),
+             _p(g2, F32, "g2"), _p(work), _p(dpos), _stream())
+    return dpos
+
+
 def comenet_ocp_features_bwd(gv, cutoff, df1, df2):
     """ComENet-OCP: (dpos [N, 3], dvec [E, 3]) = d loss / d pos and d loss / d(distance vector) through the features of
     dig3d_comenet_geometry_edges, given their gradients df1 [E,12] / df2 [E,6] in the target-sorted edge order of the
@@ -615,6 +630,21 @@ def comenet_ocp_features_tangent(gv, cutoff, cvec):
         call("dig3d_comenet_features_tangent_vec", _p(gv.vec, F32, "vec"), _p(gv.dist), _p(gv.src), _p(gv.dst),
              _p(gv.refs), n, e, float(cutoff), _p(cvec, F32, "cvec"), _p(f1d), _p(f2d), _stream())
     return f1d, f2d
+
+
+def comenet_ocp_features_tangent_bwd(gv, cutoff, cvec, g1, g2):
+    """ComENet-OCP: dpos [N, 3] = d/dpos of sum(g1 * feature1_dot + g2 * feature2_dot) along cvec [N, 3], the cell held
+    fixed, in the graph view's target-sorted edge order (see comenet_ocp_features_bwd).  Deterministic."""
+    e, n = gv.n_edges, gv.n_nodes
+    dev = gv.vec.device
+    if e == 0:
+        return torch.zeros(n, 3, dtype=F32, device=dev)
+    dpos = torch.empty(n, 3, dtype=F32, device=dev)
+    work = torch.empty(18 * e, dtype=F32, device=dev)
+    call("dig3d_comenet_features_tangent_bwd_vec", _p(gv.vec, F32, "vec"), _p(gv.dist), _p(gv.src), _p(gv.dst),
+         _p(gv.row_ptr), _p(gv.out_ptr), _p(gv.out_list), _p(gv.refs), n, e, float(cutoff),
+         _p(cvec, F32, "cvec"), _p(g1, F32, "g1"), _p(g2, F32, "g2"), _p(work), _p(dpos), _stream())
+    return dpos
 
 
 def pbc_cell_bwd(dvec, cell_offsets, row_ptr, graph_ptr, n_graphs):

@@ -209,8 +209,9 @@ class ComENet(nn.Module):
 
     `energy_and_force=True` (an extension at the end of the argument list, as SchNet / DimeNetPP / SphereNet have it in
     the reference): forward calls `pos.requires_grad_()`.  Whenever pos requires grad -- set by this flag or by the caller
-    -- the energy is differentiable in pos (forces = -grad(E, pos)), and in training mode twice, for training on forces
-    (run.train(..., energy_and_force=True))."""
+    -- the energy is differentiable in pos (forces = -grad(E, pos)), and twice: in the parameters, for training on
+    forces (run.train(..., energy_and_force=True)), and in pos (Hessian-vector products,
+    threedgraph.utils.molecular_hessians), in training and eval mode alike."""
 
     def __init__(self, cutoff=8.0, num_layers=4, hidden_channels=256, middle_channels=64, out_channels=1,
                  num_radial=3, num_spherical=2, num_output_layers=3, energy_and_force=False):
@@ -277,14 +278,14 @@ class ComENet(nn.Module):
                             want_edge_index=False, z=z, z_rows=self.emb.emb.num_embeddings)
         f1, f2, _ = ops.comenet_geometry(g, pos, self.cutoff)
         if torch.is_grad_enabled() and pos.requires_grad:
-            # forces: f1 / f2 carry the position gradient (csrc/comenet.cu); the graph's input-gradient GEMMs stay exact
-            if self.training and any(p.requires_grad for p in self.parameters()):
-                # training ON forces (run.py:110-123): reverse over forward mode, dig_b200/autograd_jvp.py
-                return jv.energy_with_force(
-                    lambda p: self._exact(self._forward_train, z, g, *ag.comenet_features(p, g, self.cutoff, f1, f2)),
-                    lambda p, c: self._exact(self._forward_dual, z, g, p, c, f1, f2),
-                    pos, tuple(self.parameters()))
-            return self._exact(self._forward_train, z, g, *ag.comenet_features(pos, g, self.cutoff, f1, f2))
+            # forces: f1 / f2 carry the position gradient (csrc/comenet.cu); the graph's input-gradient GEMMs stay exact.
+            # grad(out, pos, create_graph=True) stays differentiable in the parameters (training ON forces,
+            # run.py:110-123) and in pos (Hessian-vector products), in training and eval mode alike -- reverse over
+            # forward mode, dig_b200/autograd_jvp.py.  Energies and first-order forces are those of _forward_train.
+            return jv.energy_with_force(
+                lambda p: self._exact(self._forward_train, z, g, *ag.comenet_features(p, g, self.cutoff, f1, f2)),
+                lambda p, c: self._exact(self._forward_dual, z, g, p, c, f1, f2),
+                pos, tuple(self.parameters()), second_order=True)
         if wants_grad(self) or self._generic:
             return self._forward_train(z, g, f1, f2)
         dense = os.environ.get("DIG3D_COMENET_DENSE", "h16")
@@ -441,7 +442,11 @@ class ComENet(nn.Module):
 
     def _forward_dual(self, z, g, pos, cvec, f1, f2):
         """(E, E_dot) along the per-atom displacement cvec [N, 3] (comenet_energy_dual); the feature tangents come from
-        ops.comenet_features_tangent."""
+        ops.comenet_features_tangent.  When pos requires grad (Hessian-vector products), the features and their tangents
+        are differentiable functions of pos (ag.comenet_features, jv.comenet_features_tangent); otherwise constants."""
+        if pos.requires_grad:
+            return comenet_energy_dual(self, z, g, *ag.comenet_features(pos, g, self.cutoff, f1, f2),
+                                       *jv.comenet_features_tangent(pos, g, self.cutoff, cvec))
         return comenet_energy_dual(self, z, g, f1, f2, *ops.comenet_features_tangent(g, pos.detach(), self.cutoff, cvec))
 
     def forward(self, batch_data):

@@ -92,7 +92,9 @@ class ComENet(nn.Module):
     `F = -torch.autograd.grad(E.sum(), data.pos)[0]`; with `data.cell.requires_grad_()`, `grad(E.sum(), data.cell)` is
     dE/dcell [G, 3, 3] (from which a stress is built).  The energy is bit for bit the energy-only forward's; the geometry
     and cell kernels have no float atomics.  In training mode, `grad(E, pos, create_graph=True)` is differentiable in
-    the parameters (training on forces); that path refuses a cell that requires grad (no second order in the cell).
+    the parameters (training on forces) and, in training and eval mode alike, in pos with the cell held fixed
+    (Hessian-vector products).  Training on forces refuses a cell that requires grad (no second order in the cell); with
+    a cell that requires grad, the gradients are first order only.
     `regress_forces=True` stays refused: the reference returns no forces with it either."""
 
     def __init__(self, num_atoms, bond_feat_dim, num_targets=1, otf_graph=False, use_pbc=True, regress_forces=False,
@@ -234,16 +236,27 @@ class ComENet(nn.Module):
         if wants_cell and gv.n_edges and not torch.equal(gv.edge_graph.long(), batch[gv.dst.long()]):
             raise ValueError("ComENet-OCP: the cell gradient needs every edge in the structure of its target atom "
                              "(neighbors must count the edges of each structure in batch order)")
-        if self.training and wants_pos and any(p.requires_grad for p in self.parameters()):
-            # training on forces: reverse over forward mode (dig_b200/autograd_jvp.py); no second order in the cell
-            if wants_cell:
-                raise NotImplementedError("ComENet-OCP: training on forces with cell.requires_grad (the cell gradient "
-                                          "differentiated again) is not implemented; detach the cell")
+        if wants_cell and self.training and wants_pos and any(p.requires_grad for p in self.parameters()):
+            raise NotImplementedError("ComENet-OCP: training on forces with cell.requires_grad (the cell gradient "
+                                      "differentiated again) is not implemented; detach the cell")
+        if wants_pos and not wants_cell:
+            # grad(E, pos, create_graph=True) stays differentiable in the parameters (training on forces) and in pos
+            # (Hessian-vector products, the cell held fixed), in training and eval mode alike: reverse over forward
+            # mode, dig_b200/autograd_jvp.py.  Energies and first-order forces are those of the first-order path.
             cell_c = cell.detach()
             return jv.energy_with_force(
                 lambda p: exact_backward(comenet_energy, self, z, gv,
                                          *ag.comenet_ocp_features(p, cell_c, gv, self.cutoff, f1, f2)),
-                lambda p, c: exact_backward(comenet_energy_dual, self, z, gv, f1, f2,
-                                            *ops.comenet_ocp_features_tangent(gv, self.cutoff, c)),
-                pos, tuple(self.parameters()))
+                lambda p, c: exact_backward(self._energy_dual, z, gv, p, c, cell_c, f1, f2),
+                pos, tuple(self.parameters()), second_order=True)
+        # a cell that requires grad: first order only (a second backward through these gradients raises)
         return exact_backward(comenet_energy, self, z, gv, *ag.comenet_ocp_features(pos, cell, gv, self.cutoff, f1, f2))
+
+    def _energy_dual(self, z, gv, pos, cvec, cell, f1, f2):
+        """(E, E_dot) along the per-atom displacement cvec [N, 3], the cell held fixed (comenet_energy_dual).  When pos
+        requires grad (Hessian-vector products), the features and their tangents are differentiable in pos; otherwise
+        constants."""
+        if pos.requires_grad:
+            return comenet_energy_dual(self, z, gv, *ag.comenet_ocp_features(pos, cell, gv, self.cutoff, f1, f2),
+                                       *jv.comenet_ocp_features_tangent(pos, gv, self.cutoff, cvec))
+        return comenet_energy_dual(self, z, gv, f1, f2, *ops.comenet_ocp_features_tangent(gv, self.cutoff, cvec))

@@ -11,7 +11,11 @@ def molecular_hessians(model, batch):
     E_b is the model's output for molecule b (summed over output channels).  Molecules do not interact, so the batch's
     Hessian is block diagonal and 3 * max_b n_b Hessian-vector products give every block: product (k, d) moves
     coordinate d of the k-th atom of EVERY molecule at once.  Each product is one `torch.autograd.grad` of the force.
-    `batch` is not modified; the model is evaluated in whatever mode (train / eval) it is in."""
+    `batch` is not modified; the model is evaluated in whatever mode (train / eval) it is in.
+
+    Models: SchNet, DimeNet++, SphereNet and ComENet.  With ComENet-OCP, the blocks are per structure in the positions
+    with the cell held fixed (the cell must not require grad; periodic images of a structure's own atoms stay inside
+    its block)."""
     b = copy.copy(batch)
     pos = batch.pos.detach().clone().requires_grad_(True)
     b.pos = pos

@@ -460,6 +460,16 @@ int dig3d_comenet_features_bwd(const float* pos, const float* dist, const int32_
 int dig3d_comenet_features_tangent(const float* pos, const float* dist, const int32_t* src, const int32_t* dst,
                                    const int32_t* refs, int64_t n_nodes, int64_t n_edges, double cutoff,
                                    const float* cvec, float* feature1_dot, float* feature2_dot, void* stream);
+/* Hessian-vector products through the geometry above.  features_tangent_bwd: dpos[N,3] (every row written) =
+ * d/dpos of sum(g1 * feature1_dot + g2 * feature2_dot), feature*_dot = features_tangent(cvec) with cvec held constant,
+ * i.e. sum over edges and features of g_k (d2 feature_k / dpos2) cvec.  g1 [E,12], g2 [E,6]; work: [18 * E] floats, the
+ * three passes of features_bwd with the first evaluated on dual numbers along cvec.  Same conventions (an aliased
+ * cross product is constant, a zero norm or atan2(0, 0) passes nothing) and no float atomics. */
+int dig3d_comenet_features_tangent_bwd(const float* pos, const float* dist, const int32_t* src, const int32_t* dst,
+                                       const int32_t* row_ptr, const int32_t* out_ptr, const int32_t* out_list,
+                                       const int32_t* refs, int64_t n_nodes, int64_t n_edges, double cutoff,
+                                       const float* cvec, const float* g1, const float* g2, float* work, float* dpos,
+                                       void* stream);
 
 /* ComENet-OCP (reference dig/threedgraph/method/comenet/ocp/comenet-ocp.py:343-474): the graph arrives as an arbitrary
  * edge list with periodic images.  dig3d_pbc_edge_vectors = ocpmodels' get_pbc_distances (distance_vec = pos[row] -
@@ -495,6 +505,13 @@ int dig3d_comenet_features_bwd_vec(const float* vec, const float* dist, const in
 int dig3d_comenet_features_tangent_vec(const float* vec, const float* dist, const int32_t* src, const int32_t* dst,
                                        const int32_t* refs, int64_t n_nodes, int64_t n_edges, double cutoff,
                                        const float* cvec, float* feature1_dot, float* feature2_dot, void* stream);
+/* features_tangent_bwd_vec: dig3d_comenet_features_tangent_bwd on the sorted edges with the edge vectors read from vec
+ * and their tangent cvec[src] - cvec[dst] (the cell held fixed): the Hessian-vector products in pos. */
+int dig3d_comenet_features_tangent_bwd_vec(const float* vec, const float* dist, const int32_t* src,
+                                           const int32_t* dst, const int32_t* row_ptr, const int32_t* out_ptr,
+                                           const int32_t* out_list, const int32_t* refs, int64_t n_nodes,
+                                           int64_t n_edges, double cutoff, const float* cvec, const float* g1,
+                                           const float* g2, float* work, float* dpos, void* stream);
 int dig3d_pbc_cell_bwd(const float* dvec, const float* cell_offsets, const int32_t* row_ptr, const int32_t* graph_ptr,
                        int64_t n_graphs, float* dcell, void* stream);
 
