@@ -7,9 +7,7 @@ with int_emb_size != 64 or basis_emb_size_* != 8: materialised bases, ordinary l
       per triplet   NR fmas per (l) / (ab) row, then one fma per harmonic (NS, and NY with torsion):  NR + NS + NY + 1
       ddist[kj]     the triplet sums of its n(kj) triplets added in one lane per 32 (n(kj) adds at most), a 5-level
                     butterfly, the product with fl(1 / cutoff) (2 roundings)
-  HARMONIC_TOL: the fp32 closed forms (one correctly rounded op per node, CUDA sinf / cosf within 2 ulp) lie within
-  7e-6 of their fp64 values for num_spherical = 7 and 5e-7 for 3 over theta in [0, pi], phi in [-pi, pi] (values and
-  both derivatives, measured with the same strings on the CPU); 2e-5 leaves room for the device's sin / cos.
+  HARMONIC_TOL: CLOSED_FORM_TOL of tests/triplet_backward_ref.py, which also holds the fp64 reference.
 * the adjoint identity with dig3d_triplet_basis_tangent, determinism, T = 0, edges that are no triplet's k->j edge.
 * model forces against the reference fixture (DimeNet++) and torch.autograd over the restatement on the same GPU
   (SphereNet: the torsion's self-candidate tie-breaks differ between devices), and parameter gradients of force training.
@@ -28,17 +26,10 @@ from helpers import GOLDEN, formula_state_dict, rel_err
 
 pytestmark = pytest.mark.gpu
 FTOL = 1e-5
-HARMONIC_TOL = 2e-5
+HARMONIC_TOL = ref.CLOSED_FORM_TOL
 NR = 6
 BASES = [(0, False), (0, True), (1, False), (1, True)]          # (basis_id, torsion)
 _CACHE = {}
-
-
-def _collinear_batch():
-    """(pos, batch, cutoff): a straight chain of four atoms (angles exactly 0 and pi) next to a bent triple."""
-    pos = torch.tensor([[0, 0, 0], [1.2, 0, 0], [2.4, 0, 0], [3.6, 0, 0],
-                        [0, 0, 0], [1.1, 0, 0], [0.3, 1.0, 0.2]], dtype=torch.float32)
-    return pos, torch.tensor([0, 0, 0, 0, 1, 1, 1]), 5.0
 
 
 def _no_triplet_batch():
@@ -62,7 +53,7 @@ def _graph(name):
     elif name == "ragged":
         pos, batch, cutoff, num_graphs = ref.ragged_batch()
     elif name == "collinear":
-        pos, batch, cutoff = _collinear_batch()
+        pos, batch, cutoff = ref.collinear_batch()
     else:
         pos, batch, cutoff = _no_triplet_batch()
     pos, batch = pos.float().contiguous().to(dev), batch.long().to(dev)
@@ -91,49 +82,6 @@ def _inputs(name, basis_id, tors, seed):
     return g, cutoff, ns, bess, bess_dx, d_sbf, d_tbf
 
 
-def _harmonics(ns, angle, torsion):
-    """fp64 closed forms of the generated headers: yl0, yl0', ylm, dylm/dtheta, dylm/dphi, each [T, K]."""
-    from dig_b200.basis import basis_sources
-    src = basis_sources("dimenet", ns, NR)
-    th = angle.double()
-    ph = torsion.double() if torsion is not None else torch.zeros_like(th)
-    env = {"sin": torch.sin, "cos": torch.cos, "sqrt": torch.sqrt, "pi": math.pi, "theta": th, "phi": ph}
-
-    def table(key):
-        cols = [eval(s, env) for s in src[key]]
-        return torch.stack([c if torch.is_tensor(c) else torch.full_like(th, float(c)) for c in cols], 1)
-    return {k: table(k) for k in ("yl0", "yl0_dtheta", "ylm", "ylm_dtheta", "ylm_dphi")}
-
-
-def _reference(g, cutoff, ns, bess, bess_dx, angle, torsion, d_sbf, d_tbf):
-    """fp64 (ddist, dangle, dtorsion), their magnitudes M (every factor by its absolute value) and Mh (the harmonic
-    factor dropped)."""
-    Y = _harmonics(ns, angle, torsion)
-    kj = g.idx_kj.long()
-    B = bess.double()[kj].view(-1, ns, NR)
-    Bd = bess_dx.double()[kj].view(-1, ns, NR)
-    ds = d_sbf.double().view(-1, ns, NR)
-    out = {}
-    for mode in ("v", "m", "h"):
-        f = (lambda x: x) if mode == "v" else torch.abs
-        y = {k: (torch.ones_like(v) if mode == "h" else f(v)) for k, v in Y.items()}
-        s_b, s_bd = (f(ds) * f(B)).sum(2), (f(ds) * f(Bd)).sum(2)           # [T, ns]
-        dang = (y["yl0_dtheta"] * s_b).sum(1)
-        dx = (y["yl0"] * s_bd).sum(1)
-        dtor = None
-        if d_tbf is not None:
-            dt = d_tbf.double().view(-1, ns, ns, NR)                          # [T, a, b, r]
-            h = (f(dt) * f(B)[:, None]).sum(3).reshape(-1, ns * ns)          # [T, ab]
-            hd = (f(dt) * f(Bd)[:, None]).sum(3).reshape(-1, ns * ns)
-            dang = dang + (y["ylm_dtheta"] * h).sum(1)
-            dtor = (y["ylm_dphi"] * h).sum(1)
-            dx = dx + (y["ylm"] * hd).sum(1)
-        inv = 1.0 / cutoff
-        ddist = torch.zeros(g.n_edges, dtype=torch.float64, device=bess.device).index_add_(0, kj, dx) * inv
-        out[mode] = (ddist, dang, dtor)
-    return out
-
-
 def _run(g, cutoff, basis_id, bess, bess_dx, d_sbf, d_tbf, tors):
     from dig_b200 import ops
     return ops.triplet_basis_bwd(g, bess, bess_dx, g.angle, g.torsion if tors else None, basis_id, d_sbf, d_tbf,
@@ -154,7 +102,7 @@ def test_triplet_basis_bwd_matches_fp64(graph, basis_id, tors):
     if graph == "collinear":
         a = g.angle.double()
         assert bool((a == 0).any()) and bool((a - math.pi).abs().lt(1e-6).any())
-    r = _reference(g, cutoff, ns, bess, bess_dx, g.angle, g.torsion if tors else None, d_sbf, d_tbf)
+    r = ref.basis_bwd_reference(g, cutoff, ns, bess, bess_dx, g.angle, g.torsion if tors else None, d_sbf, d_tbf)
     counts = torch.bincount(g.idx_kj.long(), minlength=g.n_edges)
     ny = ns * ns if tors else 0
     c_t = NR + ns + ny + 1
@@ -189,7 +137,7 @@ def test_triplet_basis_bwd_is_the_adjoint_of_the_tangent(basis_id, tors):
     dot = lambda a, b: float((a.double() * b.double()).sum())
     lhs = dot(d_sbf, sbf_d) + (dot(d_tbf, tbf_d) if tors else 0.0)
     rhs = dot(ddist, d_dot) + dot(dangle, a_dot) + (dot(dtors, t_dot) if tors else 0.0)
-    r = _reference(g, cutoff, ns, bess, bess_dx, g.angle, g.torsion if tors else None, d_sbf, d_tbf)["m"]
+    r = ref.basis_bwd_reference(g, cutoff, ns, bess, bess_dx, g.angle, g.torsion if tors else None, d_sbf, d_tbf)["m"]
     mag = dot(r[0], d_dot.abs()) + dot(r[1], a_dot.abs()) + (dot(r[2], t_dot.abs()) if tors else 0.0)
     assert abs(lhs - rhs) <= 1e-5 * mag, (lhs, rhs, mag)
 

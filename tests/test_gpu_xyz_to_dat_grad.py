@@ -102,23 +102,6 @@ def _bits(a, b):
     return torch.equal(a.contiguous().view(torch.int32), b.contiguous().view(torch.int32))
 
 
-def _degenerate(pos, ei, tors_c):
-    """(edge mask, angle mask, torsion mask) of the elements under the degenerate conventions: zero-length edges,
-    collinear or zero-length angle arms, torsions with |ji| = 0, atan2(0, 0), no candidate or the self candidate."""
-    p = pos.double()
-    n = p.size(0)
-    j, i = ei
-    e_bad = (p[i] - p[j]).norm(dim=1) == 0
-    idx_i, idx_j, idx_k, _, _ = R.triplets(ei, n)
-    u, v = p[idx_i] - p[idx_j], p[idx_k] - p[idx_j]
-    w = torch.linalg.cross(u, v, dim=-1)
-    a_bad = w.norm(dim=1) == 0
-    c = torch.where(tors_c >= 0, tors_c, idx_k)
-    p2 = torch.linalg.cross(u, p[c] - p[idx_j], dim=-1)
-    t_bad = (tors_c < 0) | (tors_c == idx_k) | (u.norm(dim=1) == 0) | a_bad | (p2.norm(dim=1) == 0)
-    return e_bad, a_bad, t_bad
-
-
 def _weights(ne, nt, seed):
     gen = torch.Generator().manual_seed(seed)
     return [torch.randn(m, generator=gen).to(DEV) for m in (ne, nt, nt)]
@@ -169,7 +152,7 @@ def test_first_order_against_aten_and_fp64(name):
     n = pos.size(0)
     g = _kernel_graph(pos, ei)
     tors_c = R.candidate_atoms(ei, n, g.tors_arg)
-    e_bad, a_bad, t_bad = _degenerate(pos, ei, tors_c)
+    e_bad, a_bad, t_bad = R.degenerate(pos, ei, tors_c)
     w = _weights(ei.size(1), g.n_triplets, 5)
     w = [w[0] * ~e_bad, w[1] * ~a_bad, w[2] * ~t_bad]
     got = _dpos(_api().xyz_to_dat, pos, ei, w)
@@ -207,7 +190,7 @@ def test_degenerate_elements_pass_convention_conformant_gradients():
     n = pos.size(0)
     g = _kernel_graph(pos, ei)
     tors_c = R.candidate_atoms(ei, n, g.tors_arg)
-    e_bad, a_bad, t_bad = _degenerate(pos, ei, tors_c)
+    e_bad, a_bad, t_bad = R.degenerate(pos, ei, tors_c)
     assert bool(e_bad.any()) and bool(a_bad.any()) and bool(t_bad.any())
     w = [torch.ones(ei.size(1), device=DEV), torch.ones(g.n_triplets, device=DEV), torch.ones(g.n_triplets, device=DEV)]
     assert bool(torch.isfinite(_dpos(_api().xyz_to_dat, pos, ei, w)).all())
@@ -266,7 +249,7 @@ def test_identities(name):
     n = pos.size(0)
     g = _kernel_graph(pos, ei)
     tors_c = R.candidate_atoms(ei, n, g.tors_arg)
-    e_bad, a_bad, t_bad = _degenerate(pos, ei, tors_c)
+    e_bad, a_bad, t_bad = R.degenerate(pos, ei, tors_c)
     w = _weights(ei.size(1), g.n_triplets, 9)
     w = [w[0] * 0, w[1] * ~a_bad, w[2] * ~t_bad]
     gen = torch.Generator().manual_seed(10)
@@ -326,7 +309,7 @@ def test_second_order_against_fp64_double_backward(name):
     n = pos.size(0)
     g = _kernel_graph(pos, ei)
     tors_c = R.candidate_atoms(ei, n, g.tors_arg)
-    e_bad, a_bad, t_bad = _degenerate(pos, ei, tors_c)
+    e_bad, a_bad, t_bad = R.degenerate(pos, ei, tors_c)
     w = _weights(ei.size(1), g.n_triplets, 21)
     w = [w[0] * ~e_bad, w[1] * ~a_bad, w[2] * ~t_bad]
     G = torch.randn(n, 3, generator=torch.Generator().manual_seed(22)).to(DEV)

@@ -50,12 +50,61 @@ rbf_freq_grad (grid-stride over the edges, 8 partial sums per thread, warp shuff
     per term: C_ENV + 2 (x as a factor) + 1 (env x) + 4 (cosf, 2 ulp) + 1 (times cos) ; accumulation: one fma per
     grid-stride iteration, 5 shuffle levels, one atomic per warp that holds an edge:
                 c1 = C_ENV + 8 + iterations + 5 + warps,   c2 = 3
+
+The first-order force path of the fused widths (tests/test_gpu_force_path_fp64.py):
+edge_basis_bwd ddist (one thread per edge, csrc/basis.cu):
+    ddist[e] = fl(1/cutoff) sum_n drbf0[e, n] (env'(x) sin(f_n x) + env(x) f_n cos(f_n x)),  x = fl(dist fl(1 / cutoff)).
+    The reference is evaluated at the kernel's own fp32 x (`edge_bwd_reference`), so x carries no error of its own.
+    env and env' are cancelling sums (env(1) = env'(1) = 0): their magnitudes take every coefficient and power by
+    absolute value, env_abs as above and envd_abs = 1/x^2 + |a| (p-1) x^(p-2) + |b| p x^(p-1) + |c| (p+1) x^p.
+        M1 = sum_n |drbf0| (envd_abs |sin| + env_abs f |cos|) / cutoff
+        M2 = sum_n |drbf0| (envd_abs |cos| + env_abs f |sin|) (f x) / cutoff      the argument f x, counted as 3 u
+    Every arithmetic node is counted as one rounding even where nvcc contracts it into an fma (that only removes
+    roundings).  env: rcp 1, x^(p-1) 8 (powf, or fewer), two more powers 2, coefficients 1, three adds 3 -> 15.
+    env': powf(x, p-2) 8, two powers 2, coefficient times constant and times power 2, x x and the division 2 (the
+    shorter branch), three adds 3 -> 15.  Per order: the product with sinf / cosf (4 u each, 2 ulp) 1 + 4, f env 1,
+    the add 1, the fma into acc 1 per order; the product with fl(1 / cutoff) 2:
+                c1 = 15 + 1 + 4 + 1 + 1 + NR + 2,   c2 = 3
+edge_basis_bwd bess_dx (BS::bessel / BS::bessel_dx, the generated closed forms, one fp32 rounding per node):
+    the reference is the fp64 evaluation of basis_sources(...)["bessel_dx"] at the kernel's x; folded with the envelope
+    (DimeNet++) bess_dx = fma(env', bessel, env bessel_dx).  A closed form is a sum of products with at most one sin /
+    cos each; its magnitude (`source_magnitude`) is the same string evaluated in fp64 with every constant and
+    subtraction made positive and sin / cos by |sin| / |cos|, plus the first-order sensitivity of each term to a relative
+    error in its sin / cos argument (sin(a) -> |a| |cos a|, cos(a) -> |a| |sin a|) -- an fp32 argument z x carries the
+    rounding of z and of the product, and near a zero of sin(z x) that is the whole error.  BESSEL_DX_TOL is not derived
+    node by node: tests/test_force_path_ref_cpu.py evaluates every string node by node in fp32 on the CPU and asserts
+    the worst |fp32 - fp64| / magnitude over x in [X_MIN, 1) is at most BESSEL_DX_TOL / 4; the factor 4 leaves room for
+    the device's 2-ulp sinf / cosf and its reciprocal-times-constant divisions.  With the envelope the bound adds
+    gamma(15 + 2) (envd_abs |bessel| + env_abs |bessel_dx|) for the envelope's own roundings and the fma.
+triplet_basis_project_bwd_geom (one warp per (k -> j) edge, lane = candidate i of the molecule, csrc/basis.cu):
+    per edge and lane q = (layer, row): R[q] = sum_r bess[kj, (l, r)] w[q, (l, r)], NR fmas (and R' with bess_dx); per
+    triplet h_l = sum_q d[t, q] R[q], 32 fmas (dot32); then one fma per harmonic into d angle / d x / d torsion: NS
+    (yl0, yl0'), plus NY (ylm, d ylm / d theta, d ylm / d phi) with torsion:
+                c_t = NR + 32 + NS + NY
+    ddist[kj]: a lane adds the d x of every triplet it owns (one candidate i per 32-atom chunk of the molecule:
+    ceil(atoms / 32) adds at most), a 5-level butterfly, the product with fl(1 / cutoff) (2):
+                c_e = c_t + ceil(atoms / 32) + 5 + 2
+    The harmonics are the generated closed forms, held to CLOSED_FORM_TOL on every Y (the Mh term, as for
+    triplet_basis_bwd).  The reference is `basis_bwd_reference` with d_sbf = sum_l d_s[l] W_s[l] (fp64), and its
+    magnitudes with |d_s| |W_s| in place of d_sbf.
 """
+import ast
+import math
+
 import torch
 
 U = 2.0 ** -24
 ETA = 2.0 ** -150
 HARMONIC_TOL = 8e-6
+# fp32 closed-form harmonics (one correctly rounded op per node, CUDA sinf / cosf within 2 ulp) lie within 7e-6 of their
+# fp64 values for num_spherical = 7 and 5e-7 for 3 over theta in [0, pi], phi in [-pi, pi] (values and both derivatives,
+# measured with the same strings on the CPU); 2e-5 leaves room for the device's sin / cos.
+CLOSED_FORM_TOL = 2e-5
+BESSEL_DX_TOL = 16 * U
+# smallest x at which the fp32 closed forms of both bases were measured within BESSEL_DX_TOL / 4 of fp64 (relative to
+# `source_magnitude`, see test_force_path_ref_cpu.py); below it, 1 / x^k of the high orders leaves the fp32 range
+X_MIN = {0: 1e-5, 1: 1e-6}
+C_ENV_BWD = 15                   # roundings of env and of env' in edge_basis_bwd (module docstring)
 GATHER_BWD_MAX_GRID = 296        # csrc/train_sphere.cu
 FREQ_MAX_GRID = 592              # csrc/basis.cu
 
@@ -197,6 +246,150 @@ def freq_counts(n_edges, exponent):
     return float(c_env + 8 + iters + 5 + warps), 3.0
 
 
+# ---------------------------------------------------------------------------------------------------- force path (fp64)
+def envelope_terms(x, exponent):
+    """(env, env', env_abs, envd_abs) at x (fp64) -- see the module docstring."""
+    p, a, b, c = envelope_coefficients(exponent)
+    env = 1.0 / x + a * x ** (p - 1) + b * x ** p + c * x ** (p + 1)
+    envd = -1.0 / x ** 2 + a * (p - 1) * x ** (p - 2) + b * p * x ** (p - 1) + c * (p + 1) * x ** p
+    env_abs = 1.0 / x + abs(a) * x ** (p - 1) + abs(b) * x ** p + abs(c) * x ** (p + 1)
+    envd_abs = 1.0 / x ** 2 + abs(a) * (p - 1) * x ** (p - 2) + abs(b) * p * x ** (p - 1) + abs(c) * (p + 1) * x ** p
+    return env, envd, env_abs, envd_abs
+
+
+def kernel_x(dist, cutoff):
+    """x = fl(dist fl(1 / cutoff)) as the edge kernels form it, returned in fp64."""
+    inv = torch.tensor(1.0 / cutoff, dtype=torch.float32)
+    return (dist.detach().float() * inv.to(dist.device)).double()
+
+
+def edge_bwd_reference(x, freq, cutoff, exponent, drbf0):
+    """(exact ddist [E], M1, M2) of edge_basis_bwd at the kernel's x (fp64) -- see the module docstring."""
+    env, envd, env_abs, envd_abs = envelope_terms(x.unsqueeze(-1), exponent)
+    f, d = freq.detach().double(), drbf0.detach().double()
+    arg = f * x.unsqueeze(-1)
+    exact = (d * (envd * arg.sin() + env * f * arg.cos())).sum(1) / cutoff
+    m1 = (d.abs() * (envd_abs * arg.sin().abs() + env_abs * f.abs() * arg.cos().abs())).sum(1) / cutoff
+    m2 = (d.abs() * (envd_abs * arg.cos().abs() + env_abs * f.abs() * arg.sin().abs()) * arg.abs()).sum(1) / cutoff
+    return exact, m1, m2
+
+
+def edge_bwd_count(nr):
+    return float(C_ENV_BWD + 1 + 4 + 1 + 1 + nr + 2), 3.0
+
+
+class _Magnitude(ast.NodeTransformer):
+    """Every constant positive, every subtraction an addition, sin / cos -> |sin| / |cos| (`arg`: -> the sensitivity to
+    a relative error in the argument, |a| |cos a| / |a| |sin a|)."""
+
+    def __init__(self, arg):
+        self.arg = arg
+
+    def visit_BinOp(self, node):
+        self.generic_visit(node)
+        if isinstance(node.op, ast.Sub):
+            node.op = ast.Add()
+        return node
+
+    def visit_UnaryOp(self, node):
+        self.generic_visit(node)
+        return node.operand if isinstance(node.op, (ast.USub, ast.UAdd)) else node
+
+    def visit_Constant(self, node):
+        return ast.Constant(abs(node.value))
+
+    def visit_Call(self, node):
+        self.generic_visit(node)
+        if node.func.id not in ("sin", "cos"):
+            return node
+        call = lambda fn, args: ast.Call(ast.Name(fn, ast.Load()), args, [])
+        if not self.arg:
+            return call("abs", [node])
+        other = call("cos" if node.func.id == "sin" else "sin", node.args)
+        return ast.BinOp(call("abs", node.args), ast.Mult(), call("abs", [other]))
+
+
+def magnitude_source(src, arg=False):
+    """The closed form `src` with every term made non-negative (see _Magnitude), as a string."""
+    return ast.unparse(_Magnitude(arg).visit(ast.parse(src, mode="eval")))
+
+
+def eval_source(src, x):
+    """A basis_sources string evaluated on the tensor x: one rounding per node in x's dtype."""
+    env = {"sin": torch.sin, "cos": torch.cos, "sqrt": torch.sqrt, "abs": torch.abs, "pi": math.pi, "x": x}
+    v = eval(src, env)
+    return v if torch.is_tensor(v) else torch.full_like(x, float(v))
+
+
+def source_magnitude(src, x):
+    """fp64 magnitude of the closed form `src` at x: the abs-transform plus the argument sensitivity."""
+    return eval_source(magnitude_source(src), x) + eval_source(magnitude_source(src, arg=True), x)
+
+
+def bessel_tables(ns, nr, x):
+    """{key: (fp64 values [E, ns nr], magnitudes)} of the closed forms "bessel" and "bessel_dx" at x (fp64)."""
+    from dig_b200.basis import basis_sources
+    src = basis_sources("dimenet", ns, nr)
+    return {k: (torch.stack([eval_source(s, x) for s in src[k]], 1),
+                torch.stack([source_magnitude(s, x) for s in src[k]], 1)) for k in ("bessel", "bessel_dx")}
+
+
+def bess_dx_reference(x, ns, nr, exponent, env_on_bessel):
+    """(exact bess_dx [E, ns nr], bound) of edge_basis_bwd's second output at the kernel's x (fp64)."""
+    t = bessel_tables(ns, nr, x)
+    (b, mb), (bd, mbd) = t["bessel"], t["bessel_dx"]
+    if not env_on_bessel:
+        return bd, BESSEL_DX_TOL * mbd
+    env, envd, env_abs, envd_abs = (v.unsqueeze(-1) for v in envelope_terms(x, exponent))
+    exact = envd * b + env * bd
+    return exact, (BESSEL_DX_TOL * (envd_abs * mb + env_abs * mbd)
+                   + gamma(C_ENV_BWD + 2) * (envd_abs * b.abs() + env_abs * bd.abs()) + (C_ENV_BWD + 2) * ETA)
+
+
+def harmonics(ns, angle, torsion, nr=6):
+    """fp64 closed forms of the generated headers: yl0, yl0', ylm, dylm/dtheta, dylm/dphi, each [T, K]."""
+    from dig_b200.basis import basis_sources
+    src = basis_sources("dimenet", ns, nr)
+    th = angle.double()
+    ph = torsion.double() if torsion is not None else torch.zeros_like(th)
+    env = {"sin": torch.sin, "cos": torch.cos, "sqrt": torch.sqrt, "pi": math.pi, "theta": th, "phi": ph}
+
+    def table(key):
+        cols = [eval(s, env) for s in src[key]]
+        return torch.stack([c if torch.is_tensor(c) else torch.full_like(th, float(c)) for c in cols], 1)
+    return {k: table(k) for k in ("yl0", "yl0_dtheta", "ylm", "ylm_dtheta", "ylm_dphi")}
+
+
+def basis_bwd_reference(g, cutoff, ns, bess, bess_dx, angle, torsion, d_sbf, d_tbf):
+    """fp64 (ddist, dangle, dtorsion) of the triplet bases' reverse mode (g needs idx_kj and n_edges), under "v", their
+    magnitudes M (every factor by its absolute value) under "m" and Mh (the harmonic factor dropped) under "h"."""
+    nr = bess.size(1) // ns
+    Y = harmonics(ns, angle, torsion, nr)
+    kj = g.idx_kj.long()
+    B = bess.double()[kj].view(-1, ns, nr)
+    Bd = bess_dx.double()[kj].view(-1, ns, nr)
+    ds = d_sbf.double().view(-1, ns, nr)
+    out = {}
+    for mode in ("v", "m", "h"):
+        f = (lambda x: x) if mode == "v" else torch.abs
+        y = {k: (torch.ones_like(v) if mode == "h" else f(v)) for k, v in Y.items()}
+        s_b, s_bd = (f(ds) * f(B)).sum(2), (f(ds) * f(Bd)).sum(2)           # [T, ns]
+        dang = (y["yl0_dtheta"] * s_b).sum(1)
+        dx = (y["yl0"] * s_bd).sum(1)
+        dtor = None
+        if d_tbf is not None:
+            dt = d_tbf.double().view(-1, ns, ns, nr)                          # [T, a, b, r]
+            h = (f(dt) * f(B)[:, None]).sum(3).reshape(-1, ns * ns)          # [T, ab]
+            hd = (f(dt) * f(Bd)[:, None]).sum(3).reshape(-1, ns * ns)
+            dang = dang + (y["ylm_dtheta"] * h).sum(1)
+            dtor = (y["ylm_dphi"] * h).sum(1)
+            dx = dx + (y["ylm"] * hd).sum(1)
+        inv = 1.0 / cutoff
+        ddist = torch.zeros(g.n_edges, dtype=torch.float64, device=bess.device).index_add_(0, kj, dx) * inv
+        out[mode] = (ddist, dang, dtor)
+    return out
+
+
 # ---------------------------------------------------------------------------------------------------- the check
 def bound(mag, c):
     return gamma(c) * mag + c * ETA
@@ -246,3 +439,10 @@ def tiny_batch():
     """(pos, batch, cutoff): one bonded triple -- 6 edges, 6 triplets: fewer edges than the 8 warps of the only CTA."""
     pos = torch.tensor([[0, 0, 0], [1, 0, 0], [0, 1.2, 0]], dtype=torch.float32)
     return pos, torch.zeros(3, dtype=torch.long), 5.0
+
+
+def collinear_batch():
+    """(pos, batch, cutoff): a straight chain of four atoms (angles exactly 0 and pi) next to a bent triple."""
+    pos = torch.tensor([[0, 0, 0], [1.2, 0, 0], [2.4, 0, 0], [3.6, 0, 0],
+                        [0, 0, 0], [1.1, 0, 0], [0.3, 1.0, 0.2]], dtype=torch.float32)
+    return pos, torch.tensor([0, 0, 0, 0, 1, 1, 1]), 5.0

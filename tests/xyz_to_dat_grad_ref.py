@@ -128,6 +128,23 @@ def geometry_at(pos, edge_index, num_nodes, tors_c=None):
     return dist, angle, torch.where(live, tor, 0.0)
 
 
+def degenerate(pos, ei, tors_c):
+    """(edge mask, angle mask, torsion mask) of the elements under the degenerate conventions: zero-length edges,
+    collinear or zero-length angle arms, torsions with |ji| = 0, atan2(0, 0), no candidate or the self candidate."""
+    p = pos.double()
+    n = p.size(0)
+    j, i = ei
+    e_bad = (p[i] - p[j]).norm(dim=1) == 0
+    idx_i, idx_j, idx_k, _, _ = triplets(ei, n)
+    u, v = p[idx_i] - p[idx_j], p[idx_k] - p[idx_j]
+    w = torch.linalg.cross(u, v, dim=-1)
+    a_bad = w.norm(dim=1) == 0
+    c = torch.where(tors_c >= 0, tors_c, idx_k)
+    p2 = torch.linalg.cross(u, p[c] - p[idx_j], dim=-1)
+    t_bad = (tors_c < 0) | (tors_c == idx_k) | (u.norm(dim=1) == 0) | a_bad | (p2.norm(dim=1) == 0)
+    return e_bad, a_bad, t_bad
+
+
 # ------------------------------------------------------------------------------------------------- the derivation
 class Dual:
     """Value and tangent, both tensors (the kernels' `dual`)."""
