@@ -61,12 +61,9 @@ SIGNATURES = {
     "dig3d_validate_nodes": [P, P, c_int64, c_int64, c_int32, P, P],
     "dig3d_knn2": [P, P, P, c_int64, c_int64, P, P, P],
     "dig3d_triplet_geometry_knn": [P, P, P, P, P, c_int64, P, P, P, P, P, P, P],
-    "dig3d_triplet_count": [P, P, c_int64, c_int32, P, P],
     "dig3d_triplet_count_out": [P, P, c_int64, c_int32, P, P, P],
     "dig3d_scan_counts3": [P, P, P, c_int64, P, P, P, P, P],
     "dig3d_edge_fill_out": [P, P, P, P, P, c_int64, c_int32, c_int64, P, P, P, P, P, P, P, P, P, P, P, P],
-    "dig3d_scan_counts": [P, P, c_int64, P, P, P, P],
-    "dig3d_edge_fill": [P, P, P, P, P, c_int64, c_int32, c_int64, P, P, P, P, P, P, P],
     "dig3d_edges_to_csr": [P, P, c_int64, c_int64, P, P, P, P, P, P, P, P],
     "dig3d_triplet_geometry": [P, P, P, P, P, c_int64, c_int32, P, P, P, P, P, P, P],
     "dig3d_triplet_geometry_any_degree": [P, P, P, P, P, c_int64, c_int64, c_int32, P, P, P, P, P, P, P, P],
@@ -76,15 +73,9 @@ SIGNATURES = {
     "dig3d_radius_graph_dense_count": [P, P, P, c_int64, c_int64, c_double, c_int64, P, P, P, P, P],
     "dig3d_radius_graph_dense_fill": [P, P, P, c_int64, c_int64, c_double, c_int64, P, c_int64, P, P, P, P],
     "dig3d_edge_basis": [P, c_int64, c_double, c_int32, P, c_int32, c_int32, P, P, P],
-    "dig3d_edge_basis_set_split": [c_int32],
-    "dig3d_triplet_basis_project_set_mode": [c_int32],
     "dig3d_triplet_basis": [P, P, P, P, c_int64, c_int32, P, P, P],
-    "dig3d_triplet_basis_project": [P, P, P, P, P, P, P, P, P, c_int64, c_int64, c_int32, c_int32,
-                                    c_int32, P, P, P, P, P],
     "dig3d_triplet_basis_project_lists": [P, P, P, P, P, P, P, P, P, c_int64, c_int64, c_int32, c_int32,
                                     c_int32, P, P, P, P, P, P, P, P],
-    "dig3d_triplet_basis_project_node": [P, P, P, P, P, P, P, P, c_int64, c_int64, c_int32, c_int32, c_int32, c_int32,
-                                         P, P, P, P, P],
     "dig3d_segment_sum": [P, P, c_int64, c_int64, P, P],
     "dig3d_sphere_init_e": [P, P, P, P, c_int64, POINTER(InitEWeights), P, P, P],
     "dig3d_sphere_update_e_a": [P, P, c_int64, POINTER(UpdateEWeights), P, P, P],
@@ -93,19 +84,15 @@ SIGNATURES = {
     "dig3d_sphere_update_v": [P, c_int64, c_int32, POINTER(UpdateVWeights), P, P],
     "dig3d_sphere_update_v_batched": [P, c_int64, c_int32, c_int32, P, P, P],
     "dig3d_graph_readout": [P, P, c_int64, c_int64, c_int32, c_int32, P, P],
-    "dig3d_tc_packed_floats": [c_int32, c_int32],
     "dig3d_tc_pack": [P, P, P, P, c_int32, P],
     "dig3d_tc_timeouts": [],
     "dig3d_sphere_init_e_tc": [P, P, P, P, c_int64, POINTER(InitEWeights), P, P, P, P],
     "dig3d_sphere_update_e_a_tc": [P, P, c_int64, POINTER(TcUpdateE), P, P, P],
     "dig3d_sphere_triplet_gather": [P, P, P, c_int32, P, P, P, P, c_int64, P, P, P, P],
-    "dig3d_sphere_triplet_gather_node": [P, P, P, c_int32, P, P, P, P, P, c_int64, c_int32, P, P, P, P],
     "dig3d_sphere_triplet_gather_warp": [P, P, P, c_int32, P, P, P, P, P, c_int64, c_int32, c_int32, P, P, P, P, P,
                                          P, P],
-    "dig3d_sphere_triplet_gather_tc": [P, P, P, c_int32, P, P, P, P, P, c_int64, c_int32, P, P, P, P],
     "dig3d_sphere_update_e_b_tc": [P, P, P, P, P, c_int64, POINTER(TcUpdateE), P, P, P],
     "dig3d_tc_set_fast_swish": [c_int32],
-    "dig3d_h16_packed_bytes": [c_int32, c_int32],
     "dig3d_h16_pack": [P, P, P, P, c_int32, P],
     "dig3d_sphere_init_e_h16": [P, P, P, P, c_int64, POINTER(InitEWeights), P, P, P, P],
     "dig3d_sphere_init_e_h16_tab": [P, P, P, P, c_int64, POINTER(InitEWeights), P, P, P, P, P, P],
@@ -215,7 +202,7 @@ SIGNATURES = {
     "dig3d_xyz2mol": [P, P, c_int64, c_int32, P, P, P],
     "dig3d_gen_traj": [P, P, P, P, c_int64, P, P, P, P, P, P, P, P, P, P, P, P, P],
 }
-_RESTYPES = {"dig3d_last_error": c_char_p, "dig3d_h16_packed_bytes": c_int64}
+_RESTYPES = {"dig3d_last_error": c_char_p}
 
 _lib = None
 

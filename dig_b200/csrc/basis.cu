@@ -7,7 +7,7 @@
 //
 // The closed forms are the generated headers (dig_b200/codegen.py): one correctly rounded fp32
 // op per node of the reference's lambdified expression.  The fused model path never materialises
-// sbf / tbf: dig3d_triplet_basis_project contracts them with lin_sbf1 / lin_t1 of ALL layers at
+// sbf / tbf: dig3d_triplet_basis_project_lists contracts them with lin_sbf1 / lin_t1 of ALL layers at
 // once, grouped by the (k->j) edge so the radial half of the contraction is done once per edge.
 #include "common.cuh"
 #include "harmonics.cuh"
@@ -84,34 +84,11 @@ __device__ __forceinline__ float envelope(float x, int p, float a, float b, floa
   return r;
 }
 
-template <class BS>
-__global__ void edge_basis_kernel(const float* __restrict__ dist, int n_edges, float inv_cutoff, int p,
-                                  float ea, float eb, float ec, const float* __restrict__ freq,
-                                  int env_on_bessel, float* __restrict__ rbf0, float* __restrict__ bess) {
-  const int e = blockIdx.x * blockDim.x + threadIdx.x;
-  if (e >= n_edges) return;
-  // dist / cutoff  ->  dist * (1.0f / cutoff)   (ATen CUDA div-by-scalar)
-  const float x = __fmul_rn(dist[e], inv_cutoff);
-  const float env = envelope(x, p, ea, eb, ec);
-  if (rbf0) {
-#pragma unroll
-    for (int n = 0; n < BS::NR; ++n)
-      rbf0[(size_t)e * BS::NR + n] = __fmul_rn(env, sinf(__fmul_rn(__ldg(freq + n), x)));
-  }
-  if (bess) {
-    float b[BS::NB];
-    BS::bessel(x, b);
-#pragma unroll
-    for (int c = 0; c < BS::NB; ++c)
-      bess[(size_t)e * BS::NB + c] = env_on_bessel ? __fmul_rn(env, b[c]) : b[c];
-  }
-}
-
-
-// The same outputs with one edge's work spread over NS + 1 threads: blockIdx.y = Bessel order l (its NR entries, the
-// same expression trees and roundings as bessel(): codegen.emit_bessel_orders) or NS for the six rbf0 sines.  One thread per
-// edge walks ~80 sinf / cosf calls back to back on ~7 resident warps per SM (latency bound: 50 us for 34 k edges); split by
-// order the launch has 8x the warps and the critical path is the longest single order.  Bit-identical to edge_basis_kernel.
+// rbf0 [E, NR] and the Bessel values [E, NB] of every edge, one edge's work spread over NS + 1 threads: blockIdx.y =
+// Bessel order l (its NR entries, the same expression trees and roundings as bessel(): codegen.emit_bessel_orders) or NS
+// for the six rbf0 sines.  One thread per edge would walk ~80 sinf / cosf calls back to back on ~7 resident warps per SM
+// (latency bound: 50 us for 34 k edges); split by order the launch has 8x the warps and the critical path is the longest
+// single order.  dist / cutoff is dist * (1.0f / cutoff), as ATen CUDA divides by a scalar.
 template <class BS>
 __global__ void __launch_bounds__(128)
 edge_basis_split_kernel(const float* __restrict__ dist, int n_edges, float inv_cutoff, int p, float ea, float eb, float ec,
@@ -196,6 +173,8 @@ __global__ void triplet_basis_kernel(const float* __restrict__ bess, const float
 //   sbf_p[t][q] = sum_l' Y_l'0(angle_t) * Rs[l']
 // The harmonics of up to 32 triplets are evaluated with lane == triplet, parked in shared
 // memory, then consumed with lane == (l, m).
+// The library launches it without the torsion factor (DimeNet++); the torsion models run
+// triplet_basis_project_packed_kernel below.
 constexpr int PRJ_WARPS = 8;
 constexpr int PRJ_LD = 33;  // lane stride of the transposed weight tables (conflict-free both ways)
 
@@ -325,9 +304,9 @@ triplet_basis_project_kernel(const float* __restrict__ bess, const float* __rest
   }
 }
 
-// ------------------------------------------------------------------ fused projection, packed (round 2, default)
-// Same traversal and outputs as triplet_basis_project_kernel (torsion models), rebuilt around the FP32 issue rate
-// (that kernel is bound by its FP32 instruction count):
+// ------------------------------------------------------------------ fused projection, packed (torsion models)
+// Same traversal and outputs as triplet_basis_project_kernel with the torsion factor, rebuilt around the FP32 issue
+// rate (that organisation is bound by its FP32 instruction count):
 //   * per-edge radial contraction: for a Bessel order b the NS + 1 outputs Rs[b], R[a*NS + b] share their NR Bessel
 //     values, so they run as (NS + 1) / 2 paired FFMA chains on pairs of OUTPUTS -- the weights of a pair sit side by side in
 //     shared memory (one LDS.64 per pair of FFMAs), the Bessel values are staged duplicated;
@@ -336,9 +315,9 @@ triplet_basis_project_kernel(const float* __restrict__ bess, const float* __rest
 //     stride 60 floats: the 16-byte stores of eight lanes fall into eight different bank groups), so the per-triplet
 //     contraction is NS * (NS+1) / 2 paired FFMAs on natural register pairs; sbf_p keeps the scalar kernel's summation order,
 //     t_p is summed as (NS+1)/2 interleaved partial sums;
-//   * RECURRENCE: the harmonics come from the recurrences of harmonics.cuh (two sincosf + ~250 multiply-adds) instead
-//     of the node-by-node closed forms (~1200 instructions); the radial contraction runs AFTER the harmonics so that
-//     its 56 result registers are not live while they are evaluated.
+//   * the harmonics come from the recurrences of harmonics.cuh (two sincosf + ~250 multiply-adds) instead of the
+//     node-by-node closed forms (~1200 instructions); the radial contraction runs AFTER the harmonics so that its 56
+//     result registers are not live while they are evaluated.
 template <class BS>
 struct PrjPackSmem {
   static constexpr int NP = (BS::NS + 1) / 2;                       // output pairs per Bessel order
@@ -350,7 +329,7 @@ struct PrjPackSmem {
   int32_t trip[PRJ_WARPS][32];
 };
 
-template <class BS, bool RECURRENCE>
+template <class BS>
 __global__ void __launch_bounds__(PRJ_WARPS * 32, 2)
 triplet_basis_project_packed_kernel(const float* __restrict__ bess, const float* __restrict__ angle,
                                     const float* __restrict__ torsion, const int32_t* __restrict__ src,
@@ -422,12 +401,7 @@ triplet_basis_project_packed_kernel(const float* __restrict__ bess, const float*
         const int slot = __popc(m & ((1u << lane) - 1));
         sm.trip[w][slot] = t;
         float y[NY], y0[NS];
-        if (RECURRENCE) {
-          ylm_recurrence<NS>(angle[t], torsion[t], y, y0);
-        } else {
-          BS::yl0(angle[t], y0);
-          BS::ylm(angle[t], torsion[t], y);
-        }
+        ylm_recurrence<NS>(angle[t], torsion[t], y, y0);
         float yp[ROW];
 #pragma unroll
         for (int b = 0; b < NS; ++b)
@@ -475,161 +449,6 @@ triplet_basis_project_packed_kernel(const float* __restrict__ bess, const float*
         t_p[o] = (acc[0].y + rest.x) + rest.y;
       }
       __syncwarp();
-    }
-  }
-}
-
-// ------------------------------------------------------------------ fused projection, node-centred (round 2)
-// Same outputs as triplet_basis_project_kernel, organised around the MIDDLE node j of the triplets (k -> j -> i): all
-// in-edges (k -> j) of j meet the same out-edges (j -> i), so a CTA owns one node at a time and
-//   * discovers the out-edges of j ONCE (the edge-centred kernel repeats the binary searches for every in-edge),
-//   * evaluates the harmonics of up to PN_TRIP triplets with ALL 256 threads (one triplet per thread; with one warp
-//     per (k -> j) edge only ~14 of 32 lanes had a triplet at QM9 sizes, and the ~1200 instructions of the 49 + 7
-//     closed forms are half of this kernel's work),
-//   * then contracts with lane = output column q exactly like the edge-centred kernel (same FMA order: the results
-//     are bit-identical).
-constexpr int PN_THREADS = 256;
-constexpr int PN_TRIP = 256;     // triplets whose harmonics are staged per pass
-constexpr int PN_MAXIN = 64;     // in-degree bound (cap + 1 <= 64)
-constexpr int PN_OUT = 256;      // out-edges handled per sweep over the molecule
-
-template <class BS, bool TORSION>
-struct PrjNodeSmem {
-  static constexpr int NYT = TORSION ? BS::NY : 1;
-  float wt[TORSION ? BS::NY * BS::NR * PRJ_LD : 1];
-  float ws[BS::NB * PRJ_LD];
-  float bess[PN_THREADS / 32][BS::NB];
-  static constexpr int YLD = ((NYT + BS::NS + 3) / 4) * 4;
-  alignas(16) float y[PN_TRIP][YLD];
-  int32_t trip[PN_TRIP];
-  int32_t in_src[PN_MAXIN];
-  int32_t out_e[PN_OUT], out_pos[PN_OUT];
-  int32_t n_out;
-};
-
-template <class BS, bool TORSION>
-__global__ void __launch_bounds__(PN_THREADS)
-triplet_basis_project_node_kernel(const float* __restrict__ bess, const float* __restrict__ angle,
-                                  const float* __restrict__ torsion, const int32_t* __restrict__ src,
-                                  const int32_t* __restrict__ row_ptr, const int32_t* __restrict__ trip_ptr,
-                                  const int32_t* __restrict__ graph_ptr, const int64_t* __restrict__ batch,
-                                  int n_nodes, int n_triplets, const float* __restrict__ w_sbf1,
-                                  const float* __restrict__ w_t1, float* __restrict__ sbf_p, float* __restrict__ t_p) {
-  constexpr int NS = BS::NS, NR = BS::NR, NB = BS::NB, NY = BS::NY;
-  constexpr int NYT = TORSION ? NY : 1;
-  using SM = PrjNodeSmem<BS, TORSION>;
-  extern __shared__ __align__(16) unsigned char prj_smem_raw[];
-  SM& sm = *reinterpret_cast<SM*>(prj_smem_raw);
-  const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
-  if (TORSION)
-    for (int id = tid; id < 32 * NY * NR; id += PN_THREADS)
-      sm.wt[(id % (NY * NR)) * PRJ_LD + id / (NY * NR)] = __ldg(w_t1 + id);
-  for (int id = tid; id < 32 * NB; id += PN_THREADS) sm.ws[(id % NB) * PRJ_LD + id / NB] = __ldg(w_sbf1 + id);
-  for (int j = blockIdx.x; j < n_nodes; j += gridDim.x) {
-    const int base = row_ptr[j], d = row_ptr[j + 1] - base;
-    if (d == 0) continue;                      // no in-edge, no triplet through j          (uniform over the CTA)
-    const int g = (int)batch[j], lo = graph_ptr[g], hi = graph_ptr[g + 1];
-    __syncthreads();                           // previous node fully consumed; weight tables staged
-    for (int s = tid; s < d; s += PN_THREADS) sm.in_src[s] = src[base + s];
-    for (int c0 = lo; c0 < hi; c0 += PN_OUT) {
-      if (tid == 0) sm.n_out = 0;
-      __syncthreads();
-      // out-edges (j -> i), i in [c0, c0 + PN_OUT): edge id and the position of i among j's in-neighbours (d: absent)
-      {
-        const int i = c0 + tid;
-        if (i < hi && i != j) {
-          const int ib = row_ptr[i], di = row_ptr[i + 1] - ib;
-          int a = 0, b = di;
-          while (a < b) { const int mid = (a + b) >> 1; if (src[ib + mid] < j) a = mid + 1; else b = mid; }
-          if (a < di && src[ib + a] == j) {
-            int pa = 0, pb = d;
-            while (pa < pb) { const int mid = (pa + pb) >> 1; if (sm.in_src[mid] < i) pa = mid + 1; else pb = mid; }
-            const int slot = atomicAdd(&sm.n_out, 1);
-            sm.out_e[slot] = ib + a;
-            sm.out_pos[slot] = (pa < d && sm.in_src[pa] == i) ? pa : d;
-          }
-        }
-      }
-      __syncthreads();
-      const int o = sm.n_out;
-      if (o == 0) continue;                    // uniform
-      const int grp = max(1, PN_TRIP / o);     // in-edges per pass (o <= PN_OUT = PN_TRIP, so grp * o <= PN_TRIP)
-      for (int s0 = 0; s0 < d; s0 += grp) {
-        const int ng = min(grp, d - s0);
-        // harmonics of the (in-edge s, out-edge u) pairs of this pass, one triplet per thread
-        for (int p = tid; p < ng * o; p += PN_THREADS) {
-          const int s = s0 + p / o, u = p % o;
-          const int pos_i = sm.out_pos[u];
-          int t = -1;
-          if (pos_i != s) {                    // k == i is not a triplet
-            t = trip_ptr[sm.out_e[u]] + s - ((pos_i < s) ? 1 : 0);
-            const float th = angle[t];
-            float y0[NS];
-            BS::yl0(th, y0);
-#pragma unroll
-            for (int l = 0; l < NS; ++l) sm.y[p][NYT + l] = y0[l];
-            if (TORSION) {
-              float y[NY];
-              BS::ylm(th, torsion[t], y);
-#pragma unroll
-              for (int ab = 0; ab < NY; ++ab) sm.y[p][ab] = y[ab];
-            }
-          }
-          sm.trip[p] = t;
-        }
-        __syncthreads();
-        // contraction: one warp per in-edge, lane = output column q
-        for (int sg = w; sg < ng; sg += PN_THREADS / 32) {
-          const int kj = base + s0 + sg;
-          __syncwarp();
-          for (int c = lane; c < NB; c += 32) sm.bess[w][c] = __ldg(bess + (size_t)kj * NB + c);
-          __syncwarp();
-          float R[NYT], Rs[NS];
-#pragma unroll
-          for (int b = 0; b < NS; ++b) {
-            float rb[NR];
-#pragma unroll
-            for (int r = 0; r < NR; ++r) rb[r] = sm.bess[w][b * NR + r];
-            float acc = 0.f;
-#pragma unroll
-            for (int r = 0; r < NR; ++r) acc = fmaf(rb[r], sm.ws[(b * NR + r) * PRJ_LD + lane], acc);
-            Rs[b] = acc;
-            if (TORSION) {
-#pragma unroll
-              for (int a = 0; a < NS; ++a) {
-                const int ab = a * NS + b;
-                float acc_t = 0.f;
-#pragma unroll
-                for (int r = 0; r < NR; ++r) acc_t = fmaf(rb[r], sm.wt[(ab * NR + r) * PRJ_LD + lane], acc_t);
-                R[ab] = acc_t;
-              }
-            }
-          }
-          for (int u = 0; u < o; ++u) {
-            const int p = sg * o + u;
-            const int tt = sm.trip[p];
-            if (tt < 0) continue;
-            float yv[SM::YLD];
-#pragma unroll
-            for (int i = 0; i < SM::YLD; i += 4) {
-              const float4 q = *reinterpret_cast<const float4*>(&sm.y[p][i]);
-              yv[i] = q.x; yv[i + 1] = q.y; yv[i + 2] = q.z; yv[i + 3] = q.w;
-            }
-            float acc_s = 0.f;
-#pragma unroll
-            for (int l = 0; l < NS; ++l) acc_s = fmaf(yv[NYT + l], Rs[l], acc_s);
-            const size_t oo = ((size_t)(lane >> 3) * n_triplets + tt) * 8 + (lane & 7);
-            sbf_p[oo] = acc_s;
-            if (TORSION) {
-              float acc_t = 0.f;
-#pragma unroll
-              for (int ab = 0; ab < NY; ++ab) acc_t = fmaf(yv[ab], R[ab], acc_t);
-              t_p[oo] = acc_t;
-            }
-          }
-        }
-        __syncthreads();
-      }
     }
   }
 }
@@ -1414,11 +1233,6 @@ triplet_basis_project_bwd_geom_kernel(const float* __restrict__ bess, const floa
   }
 }
 
-// fused projection of the torsion models: 0 = scalar kernel (round 1), 1 = packed kernel with the closed-form
-// harmonics, 2 = packed kernel with the recurrence harmonics (default)
-static int h_project_mode = 2;
-static int h_edge_basis_split = 1;   // 1: one thread per (edge, Bessel order); 0: one thread per edge (round 1)
-
 template <class BS>
 static int launch_edge_basis(const float* dist, int64_t n_edges, double cutoff, int exponent,
                              const float* freq, int env_on_bessel, float* rbf0, float* bess,
@@ -1426,12 +1240,8 @@ static int launch_edge_basis(const float* dist, int64_t n_edges, double cutoff, 
   const int p = exponent + 1;
   const float a = (float)(-(p + 1) * (p + 2) / 2.0), b = (float)(p * (p + 2)), c = (float)(-p * (p + 1) / 2.0);
   const float inv = 1.0f / (float)cutoff;
-  if (h_edge_basis_split)
-    edge_basis_split_kernel<BS><<<dim3(ceil_div(n_edges, 128), BS::NS + 1), 128, 0, st>>>(
-        dist, (int)n_edges, inv, p, a, b, c, freq, env_on_bessel, rbf0, bess);
-  else
-    edge_basis_kernel<BS><<<ceil_div(n_edges, 128), 128, 0, st>>>(dist, (int)n_edges, inv, p, a, b, c, freq,
-                                                               env_on_bessel, rbf0, bess);
+  edge_basis_split_kernel<BS><<<dim3(ceil_div(n_edges, 128), BS::NS + 1), 128, 0, st>>>(
+      dist, (int)n_edges, inv, p, a, b, c, freq, env_on_bessel, rbf0, bess);
   return 0;
 }
 
@@ -1455,11 +1265,6 @@ int dig3d_edge_basis(const float* dist, int64_t n_edges, double cutoff, int32_t 
     default: set_error("edge_basis: unknown basis_id %d", basis_id); return DIG3D_EUNSUPPORTED;
   }
   DIG3D_LAUNCH_CHECK();
-  return DIG3D_OK;
-}
-
-int dig3d_edge_basis_set_split(int32_t on) {
-  h_edge_basis_split = on ? 1 : 0;
   return DIG3D_OK;
 }
 
@@ -1621,17 +1426,6 @@ int dig3d_triplet_basis_tangent_bwd(const float* bess, const float* bess_dx, con
   return DIG3D_OK;
 }
 
-int dig3d_triplet_basis_project(const float* bess, const float* angle, const float* torsion,
-                                const int32_t* src, const int32_t* dst, const int32_t* row_ptr,
-                                const int32_t* trip_ptr, const int32_t* graph_ptr, const int64_t* batch,
-                                int64_t n_edges, int64_t n_triplets, int32_t basis_id, int32_t n_layers,
-                                int32_t basis_emb, const float* w_sbf1, const float* w_t1, float* sbf_p,
-                                float* t_p, void* stream) {
-  return dig3d_triplet_basis_project_lists(bess, angle, torsion, src, dst, row_ptr, trip_ptr, graph_ptr, batch, n_edges,
-                                           n_triplets, basis_id, n_layers, basis_emb, w_sbf1, w_t1, sbf_p, t_p, nullptr,
-                                           nullptr, nullptr, stream);
-}
-
 int dig3d_triplet_basis_project_lists(const float* bess, const float* angle, const float* torsion,
                                       const int32_t* src, const int32_t* dst, const int32_t* row_ptr,
                                       const int32_t* trip_ptr, const int32_t* graph_ptr, const int64_t* batch,
@@ -1654,10 +1448,10 @@ int dig3d_triplet_basis_project_lists(const float* bess, const float* angle, con
   cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
   const int grid = (int)((n_edges + PRJ_WARPS - 1) / PRJ_WARPS < 2 * n_sm ? (n_edges + PRJ_WARPS - 1) / PRJ_WARPS
                                                                           : 2 * n_sm);
-#define DIG3D_PRJ_ONE(BS, TORS)                                                                             \
+#define DIG3D_PRJ_ONE(BS)                                                                                   \
   {                                                                                                         \
-    auto kfn = triplet_basis_project_kernel<BS, TORS>;                                                      \
-    const size_t smem = sizeof(PrjSmem<BS, TORS>);                                                          \
+    auto kfn = triplet_basis_project_kernel<BS, false>;                                                     \
+    const size_t smem = sizeof(PrjSmem<BS, false>);                                                         \
     if (cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) { \
       set_error("triplet_basis_project: cannot reserve %zu bytes of shared memory", smem);                  \
       return DIG3D_ECUDA;                                                                                   \
@@ -1665,9 +1459,9 @@ int dig3d_triplet_basis_project_lists(const float* bess, const float* angle, con
     kfn<<<grid, PRJ_WARPS * 32, smem, st>>>(bess, angle, torsion, src, dst, row_ptr, trip_ptr, graph_ptr,   \
                                             batch, (int)n_edges, (int)n_triplets, w_sbf1, w_t1, sbf_p, t_p);\
   }
-#define DIG3D_PRJP_ONE(BS, REC)                                                                            \
+#define DIG3D_PRJP_ONE(BS)                                                                                  \
   {                                                                                                         \
-    auto kfn = triplet_basis_project_packed_kernel<BS, REC>;                                                \
+    auto kfn = triplet_basis_project_packed_kernel<BS>;                                                     \
     const size_t smem = sizeof(PrjPackSmem<BS>);                                                            \
     if (cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) { \
       set_error("triplet_basis_project: cannot reserve %zu bytes of shared memory", smem);                  \
@@ -1677,11 +1471,8 @@ int dig3d_triplet_basis_project_lists(const float* bess, const float* angle, con
                                             batch, (int)n_edges, (int)n_triplets, w_sbf1, w_t1, sbf_p, t_p, \
                                             out_ptr, out_list, pos_in);                                     \
   }
-#define DIG3D_PRJ(BS)                                                  \
-  if (tors && h_project_mode == 2) DIG3D_PRJP_ONE(BS, true)            \
-  else if (tors && h_project_mode == 1) DIG3D_PRJP_ONE(BS, false)      \
-  else if (tors) DIG3D_PRJ_ONE(BS, true)                               \
-  else DIG3D_PRJ_ONE(BS, false)
+#define DIG3D_PRJ(BS) \
+  if (tors) DIG3D_PRJP_ONE(BS) else DIG3D_PRJ_ONE(BS)
   switch (basis_id) {
     case 0: DIG3D_PRJ(B76); break;
     case 1: DIG3D_PRJ(B36); break;
@@ -1690,54 +1481,6 @@ int dig3d_triplet_basis_project_lists(const float* bess, const float* angle, con
 #undef DIG3D_PRJ_ONE
 #undef DIG3D_PRJP_ONE
 #undef DIG3D_PRJ
-  DIG3D_LAUNCH_CHECK();
-  return DIG3D_OK;
-}
-
-int dig3d_triplet_basis_project_set_mode(int32_t mode) {
-  DIG3D_REQUIRE(mode >= 0 && mode <= 2, "triplet_basis_project_set_mode: mode must be 0, 1 or 2");
-  h_project_mode = mode;
-  return DIG3D_OK;
-}
-
-int dig3d_triplet_basis_project_node(const float* bess, const float* angle, const float* torsion, const int32_t* src,
-                                     const int32_t* row_ptr, const int32_t* trip_ptr, const int32_t* graph_ptr,
-                                     const int64_t* batch, int64_t n_nodes, int64_t n_triplets, int32_t cap,
-                                     int32_t basis_id, int32_t n_layers, int32_t basis_emb, const float* w_sbf1,
-                                     const float* w_t1, float* sbf_p, float* t_p, void* stream) {
-  DIG3D_REQUIRE(bess && angle && src && row_ptr && trip_ptr && graph_ptr && batch && w_sbf1 && sbf_p,
-                "triplet_basis_project_node: null pointer");
-  DIG3D_REQUIRE(n_layers * basis_emb == 32, "triplet_basis_project_node: n_layers*basis_emb must be 32, got %d*%d",
-                n_layers, basis_emb);
-  DIG3D_REQUIRE(cap >= 1 && cap <= PN_MAXIN, "triplet_basis_project_node: cap=%d outside [1,%d]", cap, PN_MAXIN);
-  const bool tors = (t_p != nullptr);
-  DIG3D_REQUIRE(!tors || (torsion && w_t1), "triplet_basis_project_node: torsion path needs torsion and w_t1");
-  if (n_nodes == 0 || n_triplets == 0) return DIG3D_OK;
-  cudaStream_t st = (cudaStream_t)stream;
-  int dev = 0, n_sm = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
-  const int grid = (int)(n_nodes < 2 * n_sm ? n_nodes : 2 * n_sm);
-#define DIG3D_PRJN_ONE(BS, TORS)                                                                            \
-  {                                                                                                         \
-    auto kfn = triplet_basis_project_node_kernel<BS, TORS>;                                                 \
-    const size_t smem = sizeof(PrjNodeSmem<BS, TORS>);                                                      \
-    if (cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) { \
-      set_error("triplet_basis_project_node: cannot reserve %zu bytes of shared memory", smem);             \
-      return DIG3D_ECUDA;                                                                                   \
-    }                                                                                                       \
-    kfn<<<grid, PN_THREADS, smem, st>>>(bess, angle, torsion, src, row_ptr, trip_ptr, graph_ptr, batch,     \
-                                        (int)n_nodes, (int)n_triplets, w_sbf1, w_t1, sbf_p, t_p);           \
-  }
-#define DIG3D_PRJN(BS) \
-  if (tors) DIG3D_PRJN_ONE(BS, true) else DIG3D_PRJN_ONE(BS, false)
-  switch (basis_id) {
-    case 0: DIG3D_PRJN(B76); break;
-    case 1: DIG3D_PRJN(B36); break;
-    default: set_error("triplet_basis_project_node: unsupported basis_id %d", basis_id); return DIG3D_EUNSUPPORTED;
-  }
-#undef DIG3D_PRJN_ONE
-#undef DIG3D_PRJN
   DIG3D_LAUNCH_CHECK();
   return DIG3D_OK;
 }

@@ -645,11 +645,6 @@ int dig3d_triplet_count_out(const int32_t* nbr, const int32_t* deg, int64_t n_no
   return DIG3D_OK;
 }
 
-int dig3d_triplet_count(const int32_t* nbr, const int32_t* deg, int64_t n_nodes, int32_t cap, int32_t* tcnt,
-                        void* stream) {
-  return dig3d_triplet_count_out(nbr, deg, n_nodes, cap, tcnt, nullptr, stream);
-}
-
 int dig3d_scan_counts3(const int32_t* deg, const int32_t* tcnt, const int32_t* out_cnt, int64_t n_nodes,
                        int32_t* row_ptr, int32_t* node_trip_ptr, int32_t* out_ptr, int32_t* totals, void* stream) {
   DIG3D_REQUIRE(deg && tcnt && row_ptr && node_trip_ptr && totals, "scan_counts: null pointer");
@@ -658,11 +653,6 @@ int dig3d_scan_counts3(const int32_t* deg, const int32_t* tcnt, const int32_t* o
                                                          out_ptr, totals);
   DIG3D_LAUNCH_CHECK();
   return DIG3D_OK;
-}
-
-int dig3d_scan_counts(const int32_t* deg, const int32_t* tcnt, int64_t n_nodes, int32_t* row_ptr,
-                      int32_t* node_trip_ptr, int32_t* totals, void* stream) {
-  return dig3d_scan_counts3(deg, tcnt, nullptr, n_nodes, row_ptr, node_trip_ptr, nullptr, totals, stream);
 }
 
 int dig3d_edge_fill_out(const float* pos, const int32_t* nbr, const int32_t* deg, const int32_t* row_ptr,
@@ -680,14 +670,6 @@ int dig3d_edge_fill_out(const float* pos, const int32_t* nbr, const int32_t* deg
       trip_ptr, graph_ptr, batch, out_ptr, out_list, pos_in);
   DIG3D_LAUNCH_CHECK();
   return DIG3D_OK;
-}
-
-int dig3d_edge_fill(const float* pos, const int32_t* nbr, const int32_t* deg, const int32_t* row_ptr,
-                    const int32_t* node_trip_ptr, int64_t n_nodes, int32_t cap, int64_t n_edges,
-                    int64_t* edge_index, int32_t* src, int32_t* dst, float* dist, float* vec,
-                    int32_t* trip_ptr, void* stream) {
-  return dig3d_edge_fill_out(pos, nbr, deg, row_ptr, node_trip_ptr, n_nodes, cap, n_edges, edge_index, src, dst, dist,
-                             vec, trip_ptr, nullptr, nullptr, nullptr, nullptr, nullptr, stream);
 }
 
 int dig3d_triplet_geometry(const float* pos, const int32_t* src, const int32_t* dst, const int32_t* row_ptr,

@@ -1358,228 +1358,6 @@ linear_h16_kernel(const float* __restrict__ x, int n_rows, int ldx, HLinParams P
   h_finish(s, epi ? &c : nullptr);
 }
 
-// ---------------------------------------------------------------------------------- triplet gather on the tensor cores
-// m[e] = sum_{t in trip(e)} x_down[kj(t)] * lin_sbf2(sbf_p[t]) * lin_t2(t_p[t])            spherenet.py:163-171
-// The node-centred SIMT kernel (sphere_triplet_gather_node_kernel) is FP32-issue bound: 35 of its ~58 instructions per
-// triplet and channel pair are the two 8 -> 64 expansions.  Here those expansions run as wgmma on one warpgroup:
-//   * one CTA per source node j (all out-edges (j -> i) sum over the same in-edges (k -> j)); the x_down rows of the
-//     in-edges are staged in shared memory (padded rows, no L2 gather);
-//   * whole out-edges are packed into tiles of <= 128 triplet rows; per tile the projected bases S [128 x 8] and
-//     T [128 x 8] are split into fp16 hi / lo planes (K padded to 16 with zeros) and multiplied with the packed
-//     lin_sbf2 / lin_t2 weights: G_s, G_t [128 x 64] in registers (two m64 halves, 3 MMAs each, N = 64, K = 16);
-//   * epilogue on the accumulator fragments: y = x * g_s * g_t into a shared tile, then lane = channel sums the rows
-//     of each out-edge and writes m[e] as one 256-byte row.
-// The protocol is sequential per tile (build planes -> MMAs -> epilogue): no roles, no rings; two to three CTAs per
-// SM overlap each other's phases.
-constexpr int GT_ROWS = 128;
-constexpr int GT_XLD = 68;                  // floats per staged x_down row (16-byte aligned, spreads the banks)
-constexpr int GT_YLD = 65;
-constexpr int GT_MAXIN = 64, GT_MAXOUT = 256, GT_MAXSEG = 128;
-constexpr float GT_SS = 8.0f, GT_SW = 64.0f;      // operand pre-scales (same rationale as H_SA / H_SW)
-
-struct GTSmem {
-  unsigned char s_hi[2 * GT_ROWS * 16], s_lo[2 * GT_ROWS * 16];     // [k-unit][row][8 halves]; k-unit 1 stays zero
-  unsigned char t_hi[2 * GT_ROWS * 16], t_lo[2 * GT_ROWS * 16];
-  unsigned char ws_hi[2 * 64 * 16], ws_lo[2 * 64 * 16], wt_hi[2 * 64 * 16], wt_lo[2 * 64 * 16];
-  float x[GT_MAXIN * GT_XLD];
-  float y[GT_ROWS * GT_YLD];
-  int in_src[GT_MAXIN];
-  int out_e[GT_MAXOUT], out_pos[GT_MAXOUT];
-  int seg_row[GT_MAXSEG + 1], seg_out[GT_MAXSEG];   // tile: first row / out-edge slot of each packed out-edge
-  int row_seg[GT_ROWS];
-  int row_src[GT_ROWS];                             // tile row -> in-edge slot of its x_down row
-  int n_out, n_seg, next_u;
-};
-
-template <bool TORSION>
-__global__ void __launch_bounds__(GT_ROWS)
-sphere_triplet_gather_tc_kernel(const float* __restrict__ x_down, const float* __restrict__ sbf_p,
-                                const float* __restrict__ t_p, const int32_t* __restrict__ src,
-                                const int32_t* __restrict__ row_ptr, const int32_t* __restrict__ trip_ptr,
-                                const int32_t* __restrict__ graph_ptr, const int64_t* __restrict__ batch,
-                                int n_nodes, const float* __restrict__ w_sbf2, const float* __restrict__ w_t2,
-                                float* __restrict__ m) {
-  extern __shared__ __align__(1024) unsigned char gt_raw[];
-  GTSmem& s = *reinterpret_cast<GTSmem*>(gt_raw);
-  const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
-  // zero the operand planes once (k-unit 1 and unused rows must read as zero), pack the two small weight matrices
-  for (int i = tid; i < (int)(4 * 2 * GT_ROWS * 16 / 16); i += GT_ROWS) reinterpret_cast<uint4*>(s.s_hi)[i] = make_uint4(0, 0, 0, 0);
-  for (int i = tid; i < 64 * 8; i += GT_ROWS) {
-    const int n = i >> 3, k = i & 7;
-    {
-      const float v = __ldg(w_sbf2 + i) * GT_SW;
-      const __half h = __float2half_rn(v);
-      reinterpret_cast<__half*>(s.ws_hi)[n * 8 + k] = h;
-      reinterpret_cast<__half*>(s.ws_lo)[n * 8 + k] = __float2half_rn(v - __half2float(h));
-    }
-    if (TORSION) {
-      const float v = __ldg(w_t2 + i) * GT_SW;
-      const __half h = __float2half_rn(v);
-      reinterpret_cast<__half*>(s.wt_hi)[n * 8 + k] = h;
-      reinterpret_cast<__half*>(s.wt_lo)[n * 8 + k] = __float2half_rn(v - __half2float(h));
-    }
-  }
-  for (int i = tid; i < 64 * 8; i += GT_ROWS) {          // k-unit 1 of the weights: zeros
-    reinterpret_cast<__half*>(s.ws_hi)[64 * 8 + i] = __float2half_rn(0.f);
-    reinterpret_cast<__half*>(s.ws_lo)[64 * 8 + i] = __float2half_rn(0.f);
-    reinterpret_cast<__half*>(s.wt_hi)[64 * 8 + i] = __float2half_rn(0.f);
-    reinterpret_cast<__half*>(s.wt_lo)[64 * 8 + i] = __float2half_rn(0.f);
-  }
-  __syncthreads();
-  for (int j = blockIdx.x; j < n_nodes; j += gridDim.x) {
-    const int base = row_ptr[j], d = row_ptr[j + 1] - base;
-    const int g = (int)batch[j], lo = graph_ptr[g], hi = graph_ptr[g + 1];
-    __syncthreads();
-    // in-neighbour list and x_down rows of j's in-edges
-    for (int k = tid; k < d; k += GT_ROWS) s.in_src[k] = src[base + k];
-    for (int i = tid; i < d * 16; i += GT_ROWS) {
-      const int r = i >> 4, c4 = i & 15;
-      *reinterpret_cast<float4*>(&s.x[r * GT_XLD + 4 * c4]) =
-          __ldg(reinterpret_cast<const float4*>(x_down + (size_t)(base + r) * 64) + c4);
-    }
-    for (int c0 = lo; c0 < hi; c0 += GT_MAXOUT) {
-      if (tid == 0) s.n_out = 0;
-      __syncthreads();
-      for (int i = c0 + tid; i < min(hi, c0 + GT_MAXOUT); i += GT_ROWS) {
-        if (i == j) continue;
-        const int ib = row_ptr[i], di = row_ptr[i + 1] - ib;
-        int a = 0, b = di;
-        while (a < b) { const int mid = (a + b) >> 1; if (src[ib + mid] < j) a = mid + 1; else b = mid; }
-        if (a < di && src[ib + a] == j) {
-          int pa = 0, pb = d;
-          while (pa < pb) { const int mid = (pa + pb) >> 1; if (s.in_src[mid] < i) pa = mid + 1; else pb = mid; }
-          const int slot = atomicAdd(&s.n_out, 1);
-          s.out_e[slot] = ib + a;
-          s.out_pos[slot] = (pa < d && s.in_src[pa] == i) ? pa : d;
-        }
-      }
-      __syncthreads();
-      const int no = s.n_out;
-      int u0 = 0;
-      while (u0 < no) {                                  // uniform loop: one tile of packed out-edges per iteration
-        // pack whole out-edges [u0, u1) while they fit in 128 rows (an out-edge has at most d <= 64 rows)
-        if (tid == 0) {
-          int rows = 0, u = u0, ns = 0;
-          while (u < no && ns < GT_MAXSEG) {
-            const int nt = d - (s.out_pos[u] < d ? 1 : 0);
-            if (rows + nt > GT_ROWS) break;
-            s.seg_row[ns] = rows; s.seg_out[ns] = u;
-            rows += nt; ++ns; ++u;
-          }
-          s.seg_row[ns] = rows;
-          s.n_seg = ns;
-          s.next_u = u;
-        }
-        __syncthreads();
-        const int ns = s.n_seg, rows = s.seg_row[ns];
-        // row -> segment map (warp-parallel fill)
-        for (int sg = w; sg < ns; sg += GT_ROWS / 32)
-          for (int r = s.seg_row[sg] + lane; r < s.seg_row[sg + 1]; r += 32) s.row_seg[r] = sg;
-        __syncthreads();
-        // operand planes of this tile: thread = triplet row
-        int srow = 0;      // in-edge slot whose x_down row this triplet uses
-        {
-          const int p = tid;
-          float sv[8], tv[8];
-#pragma unroll
-          for (int i = 0; i < 8; ++i) sv[i] = tv[i] = 0.f;
-          if (p < rows) {
-            const int sg = s.row_seg[p], u = s.seg_out[sg], r = p - s.seg_row[sg];
-            const int pos_i = s.out_pos[u];
-            srow = r + (r >= pos_i ? 1 : 0);
-            const size_t t = (size_t)trip_ptr[s.out_e[u]] + r;
-            const float4 a0 = __ldg(reinterpret_cast<const float4*>(sbf_p + t * 8));
-            const float4 a1 = __ldg(reinterpret_cast<const float4*>(sbf_p + t * 8) + 1);
-            sv[0] = a0.x; sv[1] = a0.y; sv[2] = a0.z; sv[3] = a0.w; sv[4] = a1.x; sv[5] = a1.y; sv[6] = a1.z; sv[7] = a1.w;
-            if (TORSION) {
-              const float4 b0 = __ldg(reinterpret_cast<const float4*>(t_p + t * 8));
-              const float4 b1 = __ldg(reinterpret_cast<const float4*>(t_p + t * 8) + 1);
-              tv[0] = b0.x; tv[1] = b0.y; tv[2] = b0.z; tv[3] = b0.w; tv[4] = b1.x; tv[5] = b1.y; tv[6] = b1.z; tv[7] = b1.w;
-            }
-          }
-          uint32_t h[4], l[4];
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const float a = sv[2 * i] * GT_SS, b = sv[2 * i + 1] * GT_SS;
-            const __half2 hh = __floats2half2_rn(a, b);
-            const float2 hf = __half22float2(hh);
-            const __half2 ll = __floats2half2_rn(a - hf.x, b - hf.y);
-            h[i] = *reinterpret_cast<const uint32_t*>(&hh); l[i] = *reinterpret_cast<const uint32_t*>(&ll);
-          }
-          *reinterpret_cast<uint4*>(s.s_hi + p * 16) = make_uint4(h[0], h[1], h[2], h[3]);
-          *reinterpret_cast<uint4*>(s.s_lo + p * 16) = make_uint4(l[0], l[1], l[2], l[3]);
-          if (TORSION) {
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const float a = tv[2 * i] * GT_SS, b = tv[2 * i + 1] * GT_SS;
-              const __half2 hh = __floats2half2_rn(a, b);
-              const float2 hf = __half22float2(hh);
-              const __half2 ll = __floats2half2_rn(a - hf.x, b - hf.y);
-              h[i] = *reinterpret_cast<const uint32_t*>(&hh); l[i] = *reinterpret_cast<const uint32_t*>(&ll);
-            }
-            *reinterpret_cast<uint4*>(s.t_hi + p * 16) = make_uint4(h[0], h[1], h[2], h[3]);
-            *reinterpret_cast<uint4*>(s.t_lo + p * 16) = make_uint4(l[0], l[1], l[2], l[3]);
-          }
-        }
-        s.row_src[tid] = srow;
-        fence_async_smem();
-        __syncthreads();
-        // G_s = S Ws^T and G_t = T Wt^T on the warpgroup (two m64 halves): lo*hi + hi*lo + hi*hi, K = 16 (upper half
-        // zero); epilogue y[p][c] = x[srow][c] * g_s[p][c] * g_t[p][c] straight from the accumulator fragments
-        {
-          const float scale = TORSION ? 1.0f / (GT_SS * GT_SW * GT_SS * GT_SW) : 1.0f / (GT_SS * GT_SW);
-          const uint64_t dwh = smem_desc(smem_u32(s.ws_hi), 64 * 16, 128), dwl = smem_desc(smem_u32(s.ws_lo), 64 * 16, 128);
-          const uint64_t dvh = smem_desc(smem_u32(s.wt_hi), 64 * 16, 128), dvl = smem_desc(smem_u32(s.wt_lo), 64 * 16, 128);
-#pragma unroll 1
-          for (int mh = 0; mh < 2; ++mh) {
-            const uint32_t mo = (uint32_t)(mh * 64 * 16);
-            float gs[32], gt[32];
-            wg_fence();
-            const uint64_t dsh = smem_desc(smem_u32(s.s_hi) + mo, GT_ROWS * 16, 128), dsl = smem_desc(smem_u32(s.s_lo) + mo, GT_ROWS * 16, 128);
-            mma_f16(gs, dsl, dwh, 0);
-            mma_f16(gs, dsh, dwl, 1);
-            mma_f16(gs, dsh, dwh, 1);
-            if (TORSION) {
-              const uint64_t dth = smem_desc(smem_u32(s.t_hi) + mo, GT_ROWS * 16, 128), dtl = smem_desc(smem_u32(s.t_lo) + mo, GT_ROWS * 16, 128);
-              mma_f16(gt, dtl, dvh, 0);
-              mma_f16(gt, dth, dvl, 1);
-              mma_f16(gt, dth, dvh, 1);
-            }
-            wg_commit();
-            wg_wait0();
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              const int r = 64 * mh + frag_row(tid) + 8 * h;
-              const float* xr = &s.x[s.row_src[r] * GT_XLD];
-#pragma unroll
-              for (int j = 0; j < 8; ++j)
-#pragma unroll
-                for (int e = 0; e < 2; ++e) {
-                  const int cc = 8 * j + frag_col(tid) + e, i = 4 * j + 2 * h + e;
-                  float y = (xr[cc] * scale) * gs[i];
-                  if (TORSION) y *= gt[i];
-                  s.y[r * GT_YLD + cc] = y;
-                }
-            }
-          }
-        }
-        __syncthreads();
-        // segmented sums: one warp per packed out-edge, lane = channel (c, c + 32)
-        for (int sg = w; sg < ns; sg += GT_ROWS / 32) {
-          const int r0 = s.seg_row[sg], r1 = s.seg_row[sg + 1];
-          float a0 = 0.f, a1 = 0.f;
-          for (int r = r0; r < r1; ++r) { a0 += s.y[r * GT_YLD + lane]; a1 += s.y[r * GT_YLD + lane + 32]; }
-          const size_t e = (size_t)s.out_e[s.seg_out[sg]];
-          m[e * 64 + lane] = a0;
-          m[e * 64 + lane + 32] = a1;
-        }
-        u0 = s.next_u;
-        __syncthreads();
-      }
-    }
-  }
-}
-
 static int h_smem_attr(const void* fn);
 template <int NPANEL, int KU, int N>
 static int launch_linear_h16(const float* x, int64_t rows, int ldx, const unsigned char* packed, const float* bias,
@@ -1615,8 +1393,6 @@ static int h_smem_attr(const void* fn) {
 using namespace dig3d;
 
 extern "C" {
-
-int64_t dig3d_h16_packed_bytes(int32_t n, int32_t k) { return (int64_t)4 * n * k; }
 
 static int h16_pack_impl(const float* const* weights, const int32_t* n, const int32_t* k, const int32_t* trans,
                          void* const* outs, int32_t count, void* stream) {
@@ -1783,39 +1559,6 @@ int dig3d_sphere_update_e_ba_h16(const float* m, const float* e1_in, const float
   P.w_rbf1 = w_next->w_rbf1; P.w_rbf2 = w_next->w_rbf2;
   P.x_ji = x_ji_next; P.x_down = x_down_next;
   return launch_update_e_h16<RE_BA>(m, x_ji, e1_in, rbf0, dst, n_edges, P, e1_out, v_in, (cudaStream_t)stream);
-}
-
-int dig3d_sphere_triplet_gather_tc(const float* x_down, const float* sbf_p, const float* t_p, int32_t ld_p,
-                                   const int32_t* src, const int32_t* row_ptr, const int32_t* trip_ptr,
-                                   const int32_t* graph_ptr, const int64_t* batch, int64_t n_nodes, int32_t cap,
-                                   const float* w_sbf2, const float* w_t2, float* m, void* stream) {
-  DIG3D_REQUIRE(x_down && sbf_p && src && row_ptr && trip_ptr && graph_ptr && batch && w_sbf2 && m,
-                "sphere_triplet_gather_tc: null pointer");
-  DIG3D_REQUIRE((t_p != nullptr) == (w_t2 != nullptr), "sphere_triplet_gather_tc: t_p and w_t2 must agree");
-  DIG3D_REQUIRE(ld_p == 8, "sphere_triplet_gather_tc: expects the layer-major [T, 8] slices (ld_p == 8), got %d", ld_p);
-  DIG3D_REQUIRE(cap >= 1 && cap <= GT_MAXIN, "sphere_triplet_gather_tc: cap=%d outside [1,%d]", cap, GT_MAXIN);
-  DIG3D_REQUIRE((((uintptr_t)x_down | (uintptr_t)sbf_p | (uintptr_t)t_p) & 15) == 0, "sphere_triplet_gather_tc: 16-byte alignment");
-  if (n_nodes == 0) return DIG3D_OK;
-  cudaStream_t st = (cudaStream_t)stream;
-  int dev = 0, n_sm = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
-  const int grid = (int)(n_nodes < 2 * n_sm ? n_nodes : 2 * n_sm);   // 79 KB of shared memory per CTA: two per SM
-  cudaError_t e;
-  if (t_p) {
-    e = cudaFuncSetAttribute(sphere_triplet_gather_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(GTSmem));
-    if (e == cudaSuccess)
-      sphere_triplet_gather_tc_kernel<true><<<grid, GT_ROWS, sizeof(GTSmem), st>>>(
-          x_down, sbf_p, t_p, src, row_ptr, trip_ptr, graph_ptr, batch, (int)n_nodes, w_sbf2, w_t2, m);
-  } else {
-    e = cudaFuncSetAttribute(sphere_triplet_gather_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(GTSmem));
-    if (e == cudaSuccess)
-      sphere_triplet_gather_tc_kernel<false><<<grid, GT_ROWS, sizeof(GTSmem), st>>>(
-          x_down, sbf_p, t_p, src, row_ptr, trip_ptr, graph_ptr, batch, (int)n_nodes, w_sbf2, w_t2, m);
-  }
-  if (e != cudaSuccess) { set_error("sphere_triplet_gather_tc: %s", cudaGetErrorString(e)); return DIG3D_ECUDA; }
-  DIG3D_LAUNCH_CHECK();
-  return DIG3D_OK;
 }
 
 int dig3d_linear_h16_supported(int32_t k, int32_t nout) {

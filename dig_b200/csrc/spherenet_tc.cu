@@ -223,7 +223,7 @@ __device__ __forceinline__ void epi_bar() { asm volatile("bar.sync 1, %0;" ::"n"
 
 // ---------------------------------------------------------------------------------- triplet gather (SIMT)
 // m[e] = sum_{t in trip(e)} x_down[kj(t)] * lin_sbf2(sbf_p[t]) * lin_t2(t_p[t])      spherenet.py:163-171
-// ---- packed inner loop shared by the edge-centred and the node-centred gather ------------------------------------
+// ---- packed inner loop shared by the edge-centred and the warp-per-node gather ------------------------------------
 // A lane owns channels `lane` and `lane + 32`.  Per triplet and channel the work is two 8-term expansions
 // (lin_sbf2, lin_t2) and three products; the expansions run as paired FFMA chains (common.cuh):
 //   TORSION   : the halves of a pair are the sbf and the t expansion of the SAME triplet and channel -- weights
@@ -370,124 +370,17 @@ sphere_triplet_gather_kernel(const float* __restrict__ x_down, const float* __re
   m[(size_t)e * 64 + lane + 32] = a1;
 }
 
-// ---------------------------------------------------------------------------------- triplet gather, node-centred
-// Same result as sphere_triplet_gather_kernel, organised around the SOURCE node j of the edges: every out-edge
-// (j -> i) sums over the same in-edges (k -> j) of j, whose x_down rows are CONTIGUOUS in the target-sorted edge
-// list.  One CTA per node j stages those rows (<= 33 x 256 B) in shared memory with ONE bulk copy (cp.async.bulk,
-// mbarrier completion) and then serves all out-edges of j from it: the per-triplet 256-byte L2 gathers of the
-// edge-centred kernel (one per triplet and edge) become
-// E x 256 B of coalesced staging.  The out-edges of j are discovered on the fly (one binary search per atom of
-// the molecule); their order does not matter, every m[e] is produced by exactly one warp (no atomics).
-constexpr int TGN_THREADS = 128;
-constexpr int TGN_MAXIN = 64;     // in-degree supported (cap + 1 <= 64, same bound as GEO_MAXDEG in graph.cu)
-constexpr int TGN_LIST = 256;     // out-edges handled per pass
-
-template <bool TORSION>
-__global__ void __launch_bounds__(TGN_THREADS)
-sphere_triplet_gather_node_kernel(const float* __restrict__ x_down, const float* __restrict__ sbf_p,
-                                  const float* __restrict__ t_p, const int32_t* __restrict__ src,
-                                  const int32_t* __restrict__ row_ptr, const int32_t* __restrict__ trip_ptr,
-                                  const int32_t* __restrict__ graph_ptr, const int64_t* __restrict__ batch,
-                                  int n_nodes, const float* __restrict__ w_sbf2, const float* __restrict__ w_t2,
-                                  float* __restrict__ m) {
-  extern __shared__ __align__(128) float tgn_rows[];          // [cap][64]: x_down rows of j's in-edges
-  float (*rows)[64] = reinterpret_cast<float (*)[64]>(tgn_rows);
-  __shared__ __align__(16) float2 stage[TGN_THREADS / 32][64];
-  __shared__ int in_src[TGN_MAXIN];
-  __shared__ int out_e[TGN_LIST], out_p[TGN_LIST];
-  __shared__ int n_out;
-  __shared__ uint64_t bar;
-  const int j = blockIdx.x;
-  const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
-  const int base = row_ptr[j], d = row_ptr[j + 1] - base;
-  const int g = (int)batch[j], lo = graph_ptr[g], hi = graph_ptr[g + 1];
-  if (tid == 0) {
-    mbar_init(&bar, 1);
-    mbar_fence_init();
-    n_out = 0;
-  }
-  __syncthreads();
-  if (tid == 0 && d > 0) {
-    mbar_arrive_expect_tx(&bar, (uint32_t)d * 256u);
-    bulk_g2s(&rows[0][0], x_down + (size_t)base * 64, (uint32_t)d * 256u, &bar);
-  }
-  for (int k = tid; k < d; k += TGN_THREADS) in_src[k] = src[base + k];
-  float2 wq[2][8];
-  tg_load_weights<TORSION>(wq, w_sbf2, w_t2, lane);
-  __syncthreads();
-  bool staged = false;
-  for (int c0 = lo; c0 < hi; c0 += TGN_LIST) {
-    // out-edges (j -> i) with i in [c0, c0 + TGN_LIST): edge id and the position of i among j's in-neighbours
-    for (int i = c0 + tid; i < min(hi, c0 + TGN_LIST); i += TGN_THREADS) {
-      if (i == j) continue;
-      const int ib = row_ptr[i], di = row_ptr[i + 1] - ib;
-      int a = 0, b = di;
-      while (a < b) { const int mid = (a + b) >> 1; if (src[ib + mid] < j) a = mid + 1; else b = mid; }
-      if (a < di && src[ib + a] == j) {
-        int pa = 0, pb = d;
-        while (pa < pb) { const int mid = (pa + pb) >> 1; if (in_src[mid] < i) pa = mid + 1; else pb = mid; }
-        const int slot = atomicAdd(&n_out, 1);
-        out_e[slot] = ib + a;
-        out_p[slot] = (pa < d && in_src[pa] == i) ? pa : d;
-      }
-    }
-    __syncthreads();
-    const int no = n_out;
-    if (!staged && no > 0 && d > 0) { mbar_wait(&bar, 0); staged = true; }
-    // The projected-basis values of a chunk (8 triplets) are fetched one chunk AHEAD of their use -- the next chunk of
-    // this edge, or the first chunk of the warp's next edge -- so the L2 latency hides under the paired FFMA chains.
-    auto fetch = [&](int t_first, int left, float& sa, float& sb, float& ta, float& tb) {
-      const int lim = min(8, left) * 8;
-      const float* sp = sbf_p + (size_t)t_first * 8;
-      sa = lane < lim ? __ldg(sp + lane) : 0.f; sb = lane + 32 < lim ? __ldg(sp + lane + 32) : 0.f;
-      ta = 0.f; tb = 0.f;
-      if (TORSION) {
-        const float* tp = t_p + (size_t)t_first * 8;
-        ta = lane < lim ? __ldg(tp + lane) : 0.f; tb = lane + 32 < lim ? __ldg(tp + lane + 32) : 0.f;
-      }
-    };
-    int idx = w, e = 0, p_i = 0, t0 = 0, nt = 0;
-    float sa = 0.f, sb = 0.f, ta = 0.f, tb = 0.f;
-    bool fetched = false;
-    if (idx < no) { e = out_e[idx]; p_i = out_p[idx]; t0 = trip_ptr[e]; nt = d - (p_i < d ? 1 : 0); }
-    while (idx < no) {
-      const int idx_n = idx + TGN_THREADS / 32;
-      int e_n = 0, p_n = 0, t0_n = 0, nt_n = 0;
-      if (idx_n < no) { e_n = out_e[idx_n]; p_n = out_p[idx_n]; t0_n = trip_ptr[e_n]; nt_n = d - (p_n < d ? 1 : 0); }
-      if (!fetched && nt > 0) fetch(t0, nt, sa, sb, ta, tb);
-      fetched = false;
-      float a0 = 0.f, a1 = 0.f;
-      for (int r0 = 0; r0 < nt; r0 += 8) {
-        const int n8 = min(8, nt - r0);
-        __syncwarp();
-        tg_stage<TORSION>(stage[w], lane, sa, sb, ta, tb);
-        __syncwarp();
-        if (r0 + 8 < nt) fetch(t0 + r0 + 8, nt - r0 - 8, sa, sb, ta, tb);
-        else if (idx_n < no && nt_n > 0) { fetch(t0_n, nt_n, sa, sb, ta, tb); fetched = true; }
-        tg_accumulate<TORSION>(stage[w], n8, wq, [=](int u, float& xa, float& xb) {
-          const int r = r0 + u, row = r + (r >= p_i ? 1 : 0);
-          xa = rows[row][lane]; xb = rows[row][lane + 32];
-        }, a0, a1);
-      }
-      m[(size_t)e * 64 + lane] = a0;
-      m[(size_t)e * 64 + lane + 32] = a1;
-      idx = idx_n; e = e_n; p_i = p_n; t0 = t0_n; nt = nt_n;
-    }
-    __syncthreads();
-    if (tid == 0) n_out = 0;
-    __syncthreads();
-  }
-}
-
 // ---------------------------------------------------------------------------------- triplet gather, one WARP per node
-// The node-centred kernel above spends a quarter of its warp time in CTA barriers (one warp searches the out-edges
-// while three wait; the four warps finish their 3-4 out-edges at different times) and pays the CTA set-up once per
-// node.  Here every warp is independent: it owns (node j, share `sub` of `split`), stages the rows of j's in-edges in
-// its OWN shared-memory buffer with one bulk copy (own mbarrier), finds the out-edges with lane = candidate atom,
-// keeps the in-neighbour list in two registers per lane (position look-ups are ballots) and walks its out-edges with the
-// same chunk pipeline.  No __syncthreads after the set-up.  split > 1 spreads a heavy node over several warps (each
-// stages its own copy of the rows; out-edge r of the node goes to share r % split).
+// Same result as sphere_triplet_gather_kernel, bit for bit, organised around the SOURCE node j of the edges: every
+// out-edge (j -> i) sums over the same in-edges (k -> j) of j, whose x_down rows are CONTIGUOUS in the target-sorted
+// edge list, so the per-triplet 256-byte L2 gathers of the edge-centred kernel become one coalesced staging of those
+// rows.  Every warp is independent: it owns (node j, share `sub` of `split`), stages the rows of j's in-edges in its
+// OWN shared-memory buffer with one bulk copy (cp.async.bulk, own mbarrier), finds the out-edges with lane = candidate
+// atom, keeps the in-neighbour list in two registers per lane (position look-ups are ballots) and walks its out-edges,
+// fetching the projected-basis values one chunk ahead.  No __syncthreads after the set-up.  split > 1 spreads a heavy
+// node over several warps (each stages its own copy of the rows; out-edge r of the node goes to share r % split).
 constexpr int TGW_WARPS = 4;
+constexpr int TGW_MAXIN = 64;     // in-degree supported (cap + 1 <= 64, same bound as GEO_MAXDEG in graph.cu)
 
 template <bool TORSION>
 __global__ void __launch_bounds__(TGW_WARPS * 32)
@@ -1108,8 +1001,6 @@ using namespace dig3d;
 
 extern "C" {
 
-int dig3d_tc_packed_floats(int32_t n, int32_t k) { return 2 * n * k; }
-
 int dig3d_tc_pack(const float* const* weights, const int32_t* n, const int32_t* k, float* const* outs, int32_t count,
                   void* stream) {
   DIG3D_REQUIRE(weights && n && k && outs && count >= 1 && count <= 16, "tc_pack: bad arguments");
@@ -1240,28 +1131,6 @@ int dig3d_sphere_triplet_gather(const float* x_down, const float* sbf_p, const f
   return DIG3D_OK;
 }
 
-int dig3d_sphere_triplet_gather_node(const float* x_down, const float* sbf_p, const float* t_p, int32_t ld_p,
-                                     const int32_t* src, const int32_t* row_ptr, const int32_t* trip_ptr,
-                                     const int32_t* graph_ptr, const int64_t* batch, int64_t n_nodes, int32_t cap,
-                                     const float* w_sbf2, const float* w_t2, float* m, void* stream) {
-  DIG3D_REQUIRE(x_down && sbf_p && src && row_ptr && trip_ptr && graph_ptr && batch && w_sbf2 && m,
-                "sphere_triplet_gather_node: null pointer");
-  DIG3D_REQUIRE((t_p != nullptr) == (w_t2 != nullptr), "sphere_triplet_gather_node: t_p and w_t2 must agree");
-  DIG3D_REQUIRE(ld_p == 8, "sphere_triplet_gather_node: expects the layer-major [T, 8] slices (ld_p == 8), got %d", ld_p);
-  DIG3D_REQUIRE(cap >= 1 && cap <= TGN_MAXIN, "sphere_triplet_gather_node: cap=%d outside [1,%d]", cap, TGN_MAXIN);
-  DIG3D_REQUIRE(((uintptr_t)x_down & 15) == 0, "sphere_triplet_gather_node: x_down must be 16-byte aligned");
-  if (n_nodes == 0) return DIG3D_OK;
-  cudaStream_t st = (cudaStream_t)stream;
-  if (t_p)
-    sphere_triplet_gather_node_kernel<true><<<(int)n_nodes, TGN_THREADS, (size_t)cap * 256, st>>>(
-        x_down, sbf_p, t_p, src, row_ptr, trip_ptr, graph_ptr, batch, (int)n_nodes, w_sbf2, w_t2, m);
-  else
-    sphere_triplet_gather_node_kernel<false><<<(int)n_nodes, TGN_THREADS, (size_t)cap * 256, st>>>(
-        x_down, sbf_p, t_p, src, row_ptr, trip_ptr, graph_ptr, batch, (int)n_nodes, w_sbf2, w_t2, m);
-  DIG3D_LAUNCH_CHECK();
-  return DIG3D_OK;
-}
-
 int dig3d_sphere_triplet_gather_warp(const float* x_down, const float* sbf_p, const float* t_p, int32_t ld_p,
                                      const int32_t* src, const int32_t* row_ptr, const int32_t* trip_ptr,
                                      const int32_t* graph_ptr, const int64_t* batch, int64_t n_nodes, int32_t cap,
@@ -1274,7 +1143,7 @@ int dig3d_sphere_triplet_gather_warp(const float* x_down, const float* sbf_p, co
                 "sphere_triplet_gather_warp: out_ptr, out_list and pos_in come together");
   DIG3D_REQUIRE((t_p != nullptr) == (w_t2 != nullptr), "sphere_triplet_gather_warp: t_p and w_t2 must agree");
   DIG3D_REQUIRE(ld_p == 8, "sphere_triplet_gather_warp: expects the layer-major [T, 8] slices (ld_p == 8), got %d", ld_p);
-  DIG3D_REQUIRE(cap >= 1 && cap <= TGN_MAXIN, "sphere_triplet_gather_warp: cap=%d outside [1,%d]", cap, TGN_MAXIN);
+  DIG3D_REQUIRE(cap >= 1 && cap <= TGW_MAXIN, "sphere_triplet_gather_warp: cap=%d outside [1,%d]", cap, TGW_MAXIN);
   DIG3D_REQUIRE(split >= 1 && split <= 32, "sphere_triplet_gather_warp: split=%d outside [1,32]", split);
   DIG3D_REQUIRE(((uintptr_t)x_down & 15) == 0, "sphere_triplet_gather_warp: x_down must be 16-byte aligned");
   if (n_nodes == 0) return DIG3D_OK;

@@ -297,23 +297,6 @@ def triplet_basis(bess, angle, torsion, idx_kj, basis_id, ns, nr, want_tbf):
     return sbf, tbf
 
 
-# "edge" (default): one warp per (k -> j) edge, persistent CTAs.  "node": one CTA per middle node of the triplets -- all
-# threads busy in the harmonics phase and no repeated out-edge search, bit-identical output, but slower at the headline
-# size on an earlier GPU (three CTA-wide barriers per pass and only ~15 in-edges to spread over the eight contraction
-# warps; not measured on the H100); kept as the starting point for a version that keeps several nodes in flight per CTA.
-PROJECT_MODE = ["edge"]
-
-# Kernel behind the "edge" mode for the torsion models (dig3d_triplet_basis_project_set_mode, process-wide):
-# "scalar" = round 1's kernel (reference-rounded closed-form harmonics, scalar FMA chains), "packed" = FFMA2 chains on
-# pairs of outputs with the same closed forms, "recurrence" (default) = packed + harmonics from the Legendre / angle-addition
-# recurrences (csrc/harmonics.cuh).
-PROJECT_KERNELS = {"scalar": 0, "packed": 1, "recurrence": 2}
-
-
-def set_project_kernel(name):
-    call("dig3d_triplet_basis_project_set_mode", PROJECT_KERNELS[name])
-
-
 def triplet_basis_project(g, bess, basis_id, w_sbf1_rows, w_t1_rows):
     """w_sbf1_rows: [32, ns*nr], w_t1_rows: [32, ns*ns*nr] or None.
     Returns sbf_p [4, T, 8], t_p [4, T, 8] | None (layer-major: layer l's rows are contiguous)."""
@@ -323,14 +306,7 @@ def triplet_basis_project(g, bess, basis_id, w_sbf1_rows, w_t1_rows):
     t_p = torch.empty(4, max(t, 1), 8, dtype=torch.float32, device=dev) if w_t1_rows is not None else None
     if t == 0:
         return sbf_p[:, :0], (t_p[:, :0] if t_p is not None else None)
-    if t and g.n_edges and PROJECT_MODE[0] == "node":
-        call("dig3d_triplet_basis_project_node", _p(bess, torch.float32), _p(g.angle),
-             _p(g.torsion) if w_t1_rows is not None else None, _p(g.src), _p(g.row_ptr), _p(g.trip_ptr),
-             _p(g.graph_ptr), _p(g.batch, torch.int64), g.n_nodes, t, g.cap, int(basis_id), 4, 8,
-             _p(w_sbf1_rows, torch.float32, "w_sbf1"),
-             _p(w_t1_rows, torch.float32, "w_t1") if w_t1_rows is not None else None,
-             _p(sbf_p), _p(t_p) if t_p is not None else None, _stream())
-    elif t and g.n_edges:
+    if g.n_edges:
         call("dig3d_triplet_basis_project_lists", _p(bess, torch.float32), _p(g.angle),
              _p(g.torsion) if w_t1_rows is not None else None, _p(g.src), _p(g.dst), _p(g.row_ptr),
              _p(g.trip_ptr), _p(g.graph_ptr), _p(g.batch, torch.int64), g.n_edges, t, int(basis_id), 4, 8,
@@ -872,18 +848,8 @@ def sphere_update_e_tc(e1, g, rbf0, sbf_p, t_p, col0, w, hidden, int_emb, v_in=N
     return e1_out, v_in, x_ji, x_down
 
 
-# "warp" (default): one warp per (source node, share) -- rows staged in the warp's own shared memory by one bulk copy, no
-# CTA-wide barrier; "node": one CTA per source node (round 2's first node-centred kernel); "tc": the node organisation
-# with the 8 -> 64 expansions on wgmma (3xFP16 operands); "edge": one warp per edge.  "warp" / "node" / "edge" are
-# bit-identical.
-GATHER_MODE = ["warp"]
-# warps sharing one node in "warp" mode; None = by the average number of triplets per node
-GATHER_SPLIT = [None]
-
-
 def gather_split(g):
-    if GATHER_SPLIT[0] is not None:
-        return int(GATHER_SPLIT[0])
+    """Warps sharing one source node in dig3d_sphere_triplet_gather_warp: by the average number of triplets per node."""
     per_node = g.n_triplets / max(g.n_nodes, 1)
     return max(1, min(8, int(per_node // 384) + 1))
 
@@ -893,21 +859,13 @@ def _ptr(x):
     return x if type(x) is int else _p(x)
 
 
-def triplet_gather(x_down, sp, tp, g, w_sbf2, w_t2, m_out, st):
+def triplet_gather(x_down, sp, tp, g, w_sbf2, w_t2, m_out, st, split=None):
     """m[e] = sum_t x_down[kj] * lin_sbf2(sbf_p) * lin_t2(t_p)  (spherenet.py:163-171); sp / tp are layer slices.
-    x_down / m_out: tensors or raw device addresses."""
-    mode = GATHER_MODE[0]
-    if mode == "warp":
-        call("dig3d_sphere_triplet_gather_warp", _ptr(x_down), sp, tp, 8, _p(g.src), _p(g.row_ptr), _p(g.trip_ptr),
-             _p(g.graph_ptr), _p(g.batch, torch.int64), g.n_nodes, g.cap, gather_split(g), w_sbf2, w_t2, _ptr(m_out),
-             *_out_lists(g), st)
-    elif mode in ("node", "tc"):
-        call("dig3d_sphere_triplet_gather_tc" if mode == "tc" else "dig3d_sphere_triplet_gather_node", _ptr(x_down), sp,
-             tp, 8, _p(g.src), _p(g.row_ptr), _p(g.trip_ptr), _p(g.graph_ptr), _p(g.batch, torch.int64), g.n_nodes, g.cap,
-             w_sbf2, w_t2, _ptr(m_out), st)
-    else:
-        call("dig3d_sphere_triplet_gather", _ptr(x_down), sp, tp, 8, _p(g.src), _p(g.dst), _p(g.row_ptr),
-             _p(g.trip_ptr), g.n_edges, w_sbf2, w_t2, _ptr(m_out), st)
+    One warp per (source node, share of `split` warps; None = gather_split(g)), bit-identical to the edge-centred
+    dig3d_sphere_triplet_gather for every split.  x_down / m_out: tensors or raw device addresses."""
+    call("dig3d_sphere_triplet_gather_warp", _ptr(x_down), sp, tp, 8, _p(g.src), _p(g.row_ptr), _p(g.trip_ptr),
+         _p(g.graph_ptr), _p(g.batch, torch.int64), g.n_nodes, g.cap, gather_split(g) if split is None else int(split),
+         w_sbf2, w_t2, _ptr(m_out), *_out_lists(g), st)
 
 
 def init_e_tables(init_e, cache):
@@ -1181,7 +1139,7 @@ def sphere_triplet_gather(x_down, sbf_p, t_p, g, w_sbf2, w_t2):
         return torch.zeros(e, x_down.size(1), device=x_down.device, dtype=F32)
     m = torch.empty(e, x_down.size(1), device=x_down.device, dtype=F32)
     if (x_down.size(1) == 64 and g.cap is not None and g.cap <= 64 and g.graph_ptr is not None and g.batch is not None
-            and (x_down.data_ptr() & 15) == 0 and GATHER_MODE[0] != "edge"):
+            and (x_down.data_ptr() & 15) == 0):
         # the inference organisation (warp per source node, out-edge lists): bit-identical to the edge-centred kernel
         triplet_gather(_p(x_down, F32, "x_down").value, _p(sbf_p, F32, "sbf_p"), _p(t_p, F32, "t_p"), g,
                        _p(w_sbf2, F32, "w_sbf2"), _p(w_t2, F32, "w_t2"), _p(m).value, _stream())

@@ -58,7 +58,7 @@ int dig3d_radius_neighbors(const float* pos, const int64_t* batch, const int32_t
                            int64_t n_graphs, double cutoff, int32_t cap, int32_t* nbr, int32_t* deg, void* stream);
 
 /* Radius graph for any max_num_neighbors, without the nbr[N][cap] table (csrc/graph_dense.cu): the semantics of
- * dig3d_radius_neighbors + dig3d_edge_fill at cap = max_num_neighbors + 1, in two passes.
+ * dig3d_radius_neighbors + dig3d_edge_fill_out at cap = max_num_neighbors + 1, in two passes.
  * _count: counts[n_nodes] (workspace), row_ptr[n_nodes+1]; info [2] int64 on the device, zeroed by the caller, whose
  * info[1] may carry dig3d_validate_nodes' flags (int32 at byte offset 8).  The stream is synchronised once and
  * info_host[0] = E, info_host[1] = those flags; E >= 2^31 returns DIG3D_EINVAL (info_host still written).
@@ -76,35 +76,24 @@ int dig3d_radius_graph_dense_fill(const float* pos, const int64_t* batch, const 
 int dig3d_validate_nodes(const int64_t* batch, const int64_t* z, int64_t n_nodes, int64_t n_graphs, int32_t z_rows,
                          int32_t* flags, void* stream);
 
-/* tcnt[i] = number of triplets (k->j->i, k != i) over the in-edges of node i. */
-int dig3d_triplet_count(const int32_t* nbr, const int32_t* deg, int64_t n_nodes, int32_t cap,
-                        int32_t* tcnt, void* stream);
-
-/* The same, also counting the OUT-degree of every node into out_cnt[n_nodes] (zero-initialised by the caller, nullable):
- * the radius graph caps the in-degree only, so the out-degree is not the in-degree. */
+/* tcnt[i] = number of triplets (k->j->i, k != i) over the in-edges of node i; also counts the OUT-degree of every node
+ * into out_cnt[n_nodes] (zero-initialised by the caller, nullable): the radius graph caps the in-degree only, so the
+ * out-degree is not the in-degree. */
 int dig3d_triplet_count_out(const int32_t* nbr, const int32_t* deg, int64_t n_nodes, int32_t cap, int32_t* tcnt,
                             int32_t* out_cnt, void* stream);
 
-/* Exclusive scans: row_ptr[0..n] of deg, node_trip_ptr[0..n] of tcnt; totals[0]=E, totals[1]=T. */
-int dig3d_scan_counts(const int32_t* deg, const int32_t* tcnt, int64_t n_nodes, int32_t* row_ptr,
-                      int32_t* node_trip_ptr, int32_t* totals, void* stream);
-
-/* dig3d_scan_counts plus out_ptr[0..n] = exclusive scan of out_cnt (both nullable together). */
+/* Exclusive scans: row_ptr[0..n] of deg, node_trip_ptr[0..n] of tcnt; totals[0]=E, totals[1]=T; out_ptr[0..n] of
+ * out_cnt (both nullable together). */
 int dig3d_scan_counts3(const int32_t* deg, const int32_t* tcnt, const int32_t* out_cnt, int64_t n_nodes,
                        int32_t* row_ptr, int32_t* node_trip_ptr, int32_t* out_ptr, int32_t* totals, void* stream);
 
 /* Per-edge arrays, edges sorted by (target i, source j):
  *   edge_index[2,E] int64 (row 0 = source j, row 1 = target i), src/dst int32, dist[E],
  *   vec[E,3] = pos[j]-pos[i] (nullable), trip_ptr[E+1] (first triplet of each edge).
- *   dist = sqrt(sum((pos_i-pos_j)^2)) with ATen-CUDA rounding (geometric_computing.py:25). */
-int dig3d_edge_fill(const float* pos, const int32_t* nbr, const int32_t* deg, const int32_t* row_ptr,
-                    const int32_t* node_trip_ptr, int64_t n_nodes, int32_t cap, int64_t n_edges,
-                    int64_t* edge_index, int32_t* src, int32_t* dst, float* dist, float* vec,
-                    int32_t* trip_ptr, void* stream);
-
-/* dig3d_edge_fill plus the OUT-edge lists (CSR by source; all three nullable together): out_list[out_ptr[j] ..
- * out_ptr[j+1]) = the edges (j -> i) in ascending i, pos_in[e] for e = (j -> i) = position of i among j's own
- * in-neighbours (deg[j] if i is not one).  The triplet kernels (projection: per (k -> j) edge; gather: per node and
+ *   dist = sqrt(sum((pos_i-pos_j)^2)) with ATen-CUDA rounding (geometric_computing.py:25).
+ * And the OUT-edge lists (CSR by source; out_list, out_ptr and pos_in nullable together, graph_ptr and batch needed
+ * with them): out_list[out_ptr[j] .. out_ptr[j+1]) = the edges (j -> i) in ascending i, pos_in[e] for e = (j -> i) =
+ * position of i among j's own in-neighbours (deg[j] if i is not one).  The triplet kernels (projection: per (k -> j) edge; gather: per node and
  * layer) read them instead of searching the nodes of j's graph for j's out-edges. */
 int dig3d_edge_fill_out(const float* pos, const int32_t* nbr, const int32_t* deg, const int32_t* row_ptr,
                         const int32_t* node_trip_ptr, int64_t n_nodes, int32_t cap, int64_t n_edges,
@@ -163,9 +152,6 @@ int dig3d_triplet_geometry_any_degree_arg(const float* pos, const int32_t* src, 
 int dig3d_edge_basis(const float* dist, int64_t n_edges, double cutoff, int32_t envelope_exponent,
                      const float* freq, int32_t basis_id, int32_t envelope_on_bessel, float* rbf0,
                      float* bess, void* stream);
-/* 1 (default): one thread per (edge, Bessel order) -- 8x the warps of the one-thread-per-edge kernel, bit-identical
- * output; 0: the round-1 kernel (kept as the comparison twin for tests). */
-int dig3d_edge_basis_set_split(int32_t on);
 
 /* Materialise sbf[T, ns*nr] and (nullable) tbf[T, ns*ns*nr] exactly as the reference's angle_emb /
  * torsion_emb do (test / API-parity path; the fused model path never materialises them). */
@@ -175,14 +161,11 @@ int dig3d_triplet_basis(const float* bess, const float* angle, const float* tors
 /* Fused basis evaluation + first basis projection for ALL layers:
  *   sbf_p[L, T, B] = lin_sbf1_l(sbf),  t_p[L, T, B] = lin_t1_l(tbf) (nullable => DimeNet++), layer-major
  * w_sbf1: [L][B][ns*nr], w_t1: [L][B][ns*ns*nr] (PyTorch [out,in] per layer, layers concatenated).
- * Requires L*B == 32.                                     spherenet.py:163,167  dimenetpp.py:146 */
-int dig3d_triplet_basis_project(const float* bess, const float* angle, const float* torsion,
-                                const int32_t* src, const int32_t* dst, const int32_t* row_ptr,
-                                const int32_t* trip_ptr, const int32_t* graph_ptr, const int64_t* batch,
-                                int64_t n_edges, int64_t n_triplets, int32_t basis_id, int32_t n_layers,
-                                int32_t basis_emb, const float* w_sbf1, const float* w_t1, float* sbf_p,
-                                float* t_p, void* stream);
-/* The same with the out-edge lists of dig3d_edge_fill_out (nullable together; used by the packed torsion kernels). */
+ * Requires L*B == 32.                                     spherenet.py:163,167  dimenetpp.py:146
+ * out_ptr / out_list / pos_in: the out-edge lists of dig3d_edge_fill_out (nullable together: the out-edges are then
+ * searched among the nodes of each graph; read by the torsion models' kernel).  The torsion models' harmonics come from
+ * the recurrences the reference derives its closed forms from (features.py:74-148; csrc/harmonics.cuh); DimeNet++
+ * (no torsion) uses the reference-rounded closed forms. */
 int dig3d_triplet_basis_project_lists(const float* bess, const float* angle, const float* torsion,
                                       const int32_t* src, const int32_t* dst, const int32_t* row_ptr,
                                       const int32_t* trip_ptr, const int32_t* graph_ptr, const int64_t* batch,
@@ -190,18 +173,6 @@ int dig3d_triplet_basis_project_lists(const float* bess, const float* angle, con
                                       int32_t basis_emb, const float* w_sbf1, const float* w_t1, float* sbf_p,
                                       float* t_p, const int32_t* out_ptr, const int32_t* out_list,
                                       const int32_t* pos_in, void* stream);
-/* Process-wide experiment switch for the torsion models' projection (spherenet.py:163,167): 0 = scalar kernel with the
- * reference-rounded closed-form harmonics (round 1), 1 = paired-FFMA kernel with the same closed forms, 2 (default) =
- * packed kernel with the harmonics evaluated from the recurrences the reference derives its closed forms from
- * (features.py:74-148; csrc/harmonics.cuh).  DimeNet++ (no torsion) always takes the scalar kernel. */
-int dig3d_triplet_basis_project_set_mode(int32_t mode);
-/* Same outputs (bit-identical to mode 0) with one CTA per MIDDLE node j of the triplets: the out-edges of j are found once, the
- * harmonics of up to 256 triplets are evaluated with all threads busy, then contracted per (k -> j) edge. */
-int dig3d_triplet_basis_project_node(const float* bess, const float* angle, const float* torsion, const int32_t* src,
-                                     const int32_t* row_ptr, const int32_t* trip_ptr, const int32_t* graph_ptr,
-                                     const int64_t* batch, int64_t n_nodes, int64_t n_triplets, int32_t cap,
-                                     int32_t basis_id, int32_t n_layers, int32_t basis_emb, const float* w_sbf1,
-                                     const float* w_t1, float* sbf_p, float* t_p, void* stream);
 
 /* ------------------------------------------------------------------ segmented reductions
  * scatter(src, index, dim=0, dim_size, reduce='sum') with a SORTED index given as CSR pointers
@@ -278,7 +249,6 @@ int dig3d_graph_readout(const float* v, const int32_t* graph_ptr, int64_t n_grap
  * Same math as dig3d_sphere_update_e_a/_b with the dense chain on wgmma tf32 (3xTF32 split, one K-chunk per
  * tensor-core accumulation, chunks summed in fp32).  Weights are pre-split / pre-arranged once per parameter update:
  *   dig3d_tc_pack: W [N,K] (nn.Linear layout) -> [K/32][hi|lo][8][N][4] floats (2*N*K floats per matrix). */
-int dig3d_tc_packed_floats(int32_t n, int32_t k);
 int dig3d_tc_pack(const float* const* weights, const int32_t* n, const int32_t* k, float* const* outs,
                   int32_t count, void* stream);
 /* number of mbarrier waits that hit the bounded-spin limit since library load (0 = healthy) */
@@ -305,17 +275,11 @@ int dig3d_sphere_triplet_gather(const float* x_down, const float* sbf_p, const f
                                 const int32_t* src, const int32_t* dst, const int32_t* row_ptr,
                                 const int32_t* trip_ptr, int64_t n_edges, const float* w_sbf2, const float* w_t2,
                                 float* m, void* stream);
-/* The same sums organised around the SOURCE node: one CTA per node j stages the x_down rows of j's in-edges
- * (contiguous in the target-sorted edge list, <= cap x 256 B) in shared memory with one cp.async.bulk and serves
- * every out-edge (j -> i) of j from it.  Every edge that has a source is written (all of m[E, 64]); cap = the
- * max_num_neighbors + 1 the graph was built with. */
-int dig3d_sphere_triplet_gather_node(const float* x_down, const float* sbf_p, const float* t_p, int32_t ld_p,
-                                     const int32_t* src, const int32_t* row_ptr, const int32_t* trip_ptr,
-                                     const int32_t* graph_ptr, const int64_t* batch, int64_t n_nodes, int32_t cap,
-                                     const float* w_sbf2, const float* w_t2, float* m, void* stream);
-/* Same result (bit-identical) with one WARP per (source node, share): no CTA-wide barrier, the warp's own bulk copy /
- * mbarrier, in-neighbour positions by ballot.  split >= 1 warps share a node (out-edge r of the node goes to share
- * r % split); cap = max in-degree + 1 <= 64.  out_ptr / out_list / pos_in: the out-edge lists of dig3d_edge_fill_out
+/* The same sums (bit-identical) organised around the SOURCE node, one WARP per (source node j, share): the warp stages
+ * the x_down rows of j's in-edges (contiguous in the target-sorted edge list, <= cap x 256 B) in its own shared memory
+ * with one cp.async.bulk (own mbarrier) and serves every out-edge (j -> i) of its share from it; in-neighbour positions
+ * by ballot, no CTA-wide barrier.  Every edge that has a source is written (all of m[E, 64]).  split >= 1 warps share
+ * a node (out-edge r of the node goes to share r % split); cap = max in-degree + 1 <= 64.  out_ptr / out_list / pos_in: the out-edge lists of dig3d_edge_fill_out
  * (nullable together: without them the warp searches the nodes of the graph). */
 int dig3d_sphere_triplet_gather_warp(const float* x_down, const float* sbf_p, const float* t_p, int32_t ld_p,
                                      const int32_t* src, const int32_t* row_ptr, const int32_t* trip_ptr,
@@ -340,7 +304,6 @@ int dig3d_tc_set_fast_swish(int32_t on);
  * raise the flag returned by dig3d_h16_overflow -- every 3xFP16 entry point (init_e, update_e parts A / B / BA,
  * update_v, linear_h16) raises it in the launch whose outputs became non-finite (the *_tc chain has fp32 range and
  * is the fallback). */
-int64_t dig3d_h16_packed_bytes(int32_t n, int32_t k);
 int dig3d_h16_pack(const float* const* weights, const int32_t* n, const int32_t* k, void* const* outs, int32_t count,
                    void* stream);
 int dig3d_sphere_init_e_h16(const int64_t* z, const int32_t* src, const int32_t* dst, const float* rbf0,
@@ -387,14 +350,6 @@ int dig3d_sphere_update_v_h16_supported(int32_t hidden, int32_t out_emb, int32_t
 int dig3d_sphere_update_v_h16(const float* v_in_all, int64_t n_nodes, int32_t n_blocks, int32_t out_channels,
                               int32_t n_lins, const void* const* packed, const dig3d_update_v_weights* w,
                               float* v_out_all, void* stream);
-/* The triplet gather with the two 8 -> 64 expansions (lin_sbf2, lin_t2) on the tensor cores: one CTA per source node,
- * x_down rows of its in-edges staged in shared memory, whole out-edges packed into tiles of <= 128 triplet rows, G_s / G_t
- * in registers (3xFP16 operands, K = 16 zero padded), products + per-edge sums in the epilogue.  Same contract as
- * dig3d_sphere_triplet_gather_node (every edge that has a source is written); fp32-level accuracy (~3e-7), not bit-equal. */
-int dig3d_sphere_triplet_gather_tc(const float* x_down, const float* sbf_p, const float* t_p, int32_t ld_p,
-                                   const int32_t* src, const int32_t* row_ptr, const int32_t* trip_ptr,
-                                   const int32_t* graph_ptr, const int64_t* batch, int64_t n_nodes, int32_t cap,
-                                   const float* w_sbf2, const float* w_t2, float* m, void* stream);
 /* Training-path linears on the same engine: y[rows, nout] = x[rows, k] W^T + bias, optionally also swish(y);
  * dig3d_h16_pack_t: trans[i] = 0 packs weights[i] as a row-major [n, k] matrix; trans[i] = ld > 0 packs the TRANSPOSE of
  * a [k, n] block whose rows are ld floats apart (a column slice of W for the input-gradient GEMM dX = dY W). */
@@ -619,7 +574,7 @@ int dig3d_scatter_add_rows(const float* y, const void* idx, int32_t idx_is_64, i
  * spherenet/features.py:180-182); dfreq initialised by the caller. */
 int dig3d_rbf_freq_grad(const float* dist, int64_t n_edges, double cutoff, int32_t envelope_exponent,
                         const float* freq, int32_t num_radial, const float* drbf0, float* dfreq, void* stream);
-/* Backward of dig3d_triplet_basis_project w.r.t. the projection weights: dw_sbf1[32, ns*nr] / dw_t1[32, ns*ns*nr]
+/* Backward of dig3d_triplet_basis_project_lists w.r.t. the projection weights: dw_sbf1[32, ns*nr] / dw_t1[32, ns*ns*nr]
  * (rows = layer*8 + basis row, same row order as the forward's w_sbf1 / w_t1; zero-initialised by the caller) from
  * the per-layer gradients d_sbf_p[l] / d_t_p[l] ([T, 8] each, HOST arrays of 4 device pointers, entries may be NULL).
  * The [T, ns*ns*nr] basis is recomputed on chip, never materialised.  dw_t1 NULL = no torsion (DimeNet++). */
@@ -663,8 +618,8 @@ int dig3d_graphnorm_tangent_bwd(const float* h, const float* h_dot, const float*
  *   (enveloped, when envelope_on_bessel) Bessel basis of dig3d_edge_basis; either output may be NULL.
  * triplet_torsion_bwd: dpos += d torsion[t] through the minimising candidate (geometric_computing.py:53-75).
  * triplet_basis_project_bwd_geom: dangle[T], ddist_kj[E] (and dtorsion[T] when the torsion arguments are given; every
- *   row written) of dig3d_triplet_basis_project given d_sbf_p / d_t_p (host arrays of 4 device pointers, NULL entries
- *   allowed) and the forward's w_sbf1 / w_t1 rows.
+ *   row written) of dig3d_triplet_basis_project_lists given d_sbf_p / d_t_p (host arrays of 4 device pointers, NULL
+ *   entries allowed) and the forward's w_sbf1 / w_t1 rows.
  * triplet_basis_bwd: reverse mode of dig3d_triplet_basis (materialised sbf [T, ns*nr] / tbf [T, ns*ns*nr]) given
  *   d_sbf / d_tbf (either NULL = zero): dangle[T], dtorsion[T] (NULL: skip) and ddist[E], the k->j edge's share through
  *   bess, with bess_dx from dig3d_edge_basis_bwd.  Every row of every output written (0 for an edge that is no

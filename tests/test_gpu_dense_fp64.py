@@ -1,14 +1,14 @@
 """The SphereNet / DimeNet++ inference dense chains, element by element against an fp64 restatement.
 
-Every kernel boundary -- init_e (three-panel and table form), update_e part A, the triplet gather (all four
-GATHER_MODEs), part B, part B + next part A, update_v, linear_h16 -- is restated in fp64 from the KERNEL'S OWN fp32
-inputs (spherenet.py:79-91, 150-182, 209-216; the op sequence of oracle/restated.py:229-262), so only the kernel's
-arithmetic is under test.  Each output element y must satisfy |y - y64| <= e, the running error bound of
-tests/fp64_bound.py: TOL * M + FLOOR per layer, with M the magnitude chain and TOL / FLOOR derived from the operand
-split (11-bit hi, fp16 subnormal spacing 2^-24 / H_SA and / H_SW), the truncating wgmma accumulation of the K = 64
-chunks and their fp32 sums -- the derivation is that module's docstring.  The same bound is checked for the 3xTF32
-chains and the exact-fp32 FFMA twins (their own constants), so the references the older parity tests lean on are
-pinned too.
+Every kernel boundary -- init_e (three-panel and table form), update_e part A, the triplet gather (warp per source
+node, at the graph's split and at pinned ones, and warp per edge), part B, part B + next part A, update_v, linear_h16
+-- is restated in fp64 from the KERNEL'S OWN fp32 inputs (spherenet.py:79-91, 150-182, 209-216; the op sequence of
+oracle/restated.py:229-262), so only the kernel's arithmetic is under test.  Each output element y must satisfy
+|y - y64| <= e, the running error bound of tests/fp64_bound.py: TOL * M + FLOOR per layer, with M the magnitude chain
+and TOL / FLOOR derived from the operand split (11-bit hi, fp16 subnormal spacing 2^-24 / H_SA and / H_SW), the
+truncating wgmma accumulation of the K = 64 chunks and their fp32 sums -- the derivation is that module's docstring.
+The same bound is checked for the 3xTF32 chains and the exact-fp32 FFMA twins (their own constants), so the references
+the older parity tests lean on are pinned too.
 
 Regimes: formula weights; molecules stretched so that many edges lie at 0.9-1.0 x cutoff (rbf0 -> 0: tiny rbf gates
 and e2 rows); inputs scaled until the largest operand a 3xFP16 layer splits is ~4000, then ~8100 (4000 / 8100 x 1.005 at most) (the flag must stay
@@ -192,16 +192,19 @@ def _h16_part_b(m, e1, x_ji, rbf0, dst, n, n_nodes, w, w_next=None):
 
 
 def _gather_kernel(x_down, geo, w, mode):
+    """mode: "warp" (the inference gather, split by the graph), "warp_split<n>" (the same kernel at split n) or "edge"
+    (dig3d_sphere_triplet_gather, one warp per edge)."""
     from dig_b200 import ops
     g = geo["g"]
     m = torch.zeros(g.n_edges, 64, device=x_down.device)
+    sp = ctypes.c_void_p(geo["sbf"].data_ptr())
     tp = ctypes.c_void_p(geo["tp"].data_ptr()) if geo["tp"] is not None else None
-    old = ops.GATHER_MODE[0]
-    ops.GATHER_MODE[0] = mode
-    try:
-        ops.triplet_gather(x_down, ctypes.c_void_p(geo["sbf"].data_ptr()), tp, g, w.w_sbf2, w.w_t2, m, _st())
-    finally:
-        ops.GATHER_MODE[0] = old
+    if mode == "edge":
+        _call("dig3d_sphere_triplet_gather", _p(x_down), sp, tp, 8, _p(g.src), _p(g.dst), _p(g.row_ptr),
+              _p(g.trip_ptr), g.n_edges, w.w_sbf2, w.w_t2, _p(m), _st())
+    else:
+        split = int(mode[len("warp_split"):]) if mode.startswith("warp_split") else None
+        ops.triplet_gather(x_down, sp, tp, g, w.w_sbf2, w.w_t2, m, _st(), split=split)
     return m
 
 
@@ -248,7 +251,7 @@ def _update_e_inputs(cls_name, regime):
 
 @pytest.mark.parametrize("regime", list(REGIMES))
 @pytest.mark.parametrize("cls_name", ["SphereNet", "DimeNetPP"])
-def test_update_e_register_engine_against_fp64(cls_name, regime):
+def test_update_e_register_engine_and_gather_against_fp64(cls_name, regime):
     """Part A, the default triplet gather, part B and the fused part B + next part A on the 128-molecule batch."""
     from dig_b200 import ops
     model, geo, e1_base, r = _update_e_inputs(cls_name, regime)
@@ -298,7 +301,7 @@ def test_update_e_register_engine_against_fp64(cls_name, regime):
 
 @pytest.mark.parametrize("n_edges", [1, 63, 64, 65, 129])
 @pytest.mark.parametrize("cls_name", ["SphereNet", "DimeNetPP"])
-def test_update_e_edge_prefixes_against_fp64(cls_name, n_edges):
+def test_update_e_partial_units_against_fp64(cls_name, n_edges):
     """Single partial unit, one full unit, one past it, two units and one edge: the first n_edges edges of the batch."""
     from dig_b200 import ops
     model, geo, e1, _ = _update_e_inputs(cls_name, "formula")
@@ -328,10 +331,10 @@ def test_update_e_edge_prefixes_against_fp64(cls_name, n_edges):
     ref_down2.check(x_down2, "fused x_down")
 
 
-@pytest.mark.parametrize("mode", ["warp", "node", "edge", "tc"])
+@pytest.mark.parametrize("mode", ["warp", "warp_split1", "warp_split2", "warp_split3", "edge"])
 @pytest.mark.parametrize("stretch", [1.0, 1.3])
 @pytest.mark.parametrize("cls_name", ["SphereNet", "DimeNetPP"])
-def test_triplet_gather_modes_against_fp64(cls_name, stretch, mode):
+def test_triplet_gather_kernels_against_fp64(cls_name, stretch, mode):
     from dig_b200 import ops
     model = _model(cls_name)
     geo = _geom(cls_name, stretch)
@@ -343,8 +346,7 @@ def test_triplet_gather_modes_against_fp64(cls_name, stretch, mode):
         torch.rand(g.n_edges, 1, device="cuda:0", generator=gen) * 4 - 3)      # rows over four decades
     m = _gather_kernel(x_down, geo, w, mode)
     torch.cuda.synchronize()
-    _gather(x_down, geo["sbf"], geo["tp"], g.idx_kj64, g.idx_ji64, g.n_edges, ue,
-            "h16" if mode == "tc" else "fp32").check(m, f"gather {mode}")
+    _gather(x_down, geo["sbf"], geo["tp"], g.idx_kj64, g.idx_ji64, g.n_edges, ue, "fp32").check(m, f"gather {mode}")
 
 
 # ------------------------------------------------------------------------------------------------ init_e
@@ -438,7 +440,7 @@ def test_update_v_against_fp64(layers, out_channels, regime):
 # ------------------------------------------------------------------------------------------------ 3xTF32 and fp32 twins
 @pytest.mark.parametrize("target", [None, 3.0e4], ids=["formula", "act_3e4"])
 @pytest.mark.parametrize("cls_name", ["SphereNet", "DimeNetPP"])
-def test_tf32_chain_against_fp64(cls_name, target):
+def test_tf32_fallback_chain_against_fp64(cls_name, target):
     """The 3xTF32 chain (init_e, part A, part B) is the fallback with fp32 operand range: it holds the bound at
     activations ~3e4, where the 3xFP16 split would overflow."""
     from dig_b200 import ops

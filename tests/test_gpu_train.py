@@ -667,9 +667,10 @@ def test_flat_adam_matches_torch_adam():
     assert opt_c.steps == 5 and torch.equal(opt_c.exp_avg, opt_a.exp_avg)
 
 
-def test_node_centred_triplet_gather_equals_edge_centred():
-    """The shared-memory staged gather (one CTA per source node) sums the same triplets in the same order as the
-    one-warp-per-edge kernel: m is BITWISE equal, with and without the torsion factor, incl. isolated atoms."""
+def test_warp_triplet_gather_splits_equal_edge_centred():
+    """The warp-per-source-node gather (x_down rows staged in the warp's shared memory) sums the same triplets in the
+    same order as the one-warp-per-edge kernel: m is BITWISE equal at splits 1, 2, 3 and the graph's own split, with
+    and without the torsion factor, incl. isolated atoms."""
     import ctypes
     from dig_b200 import ops
     from dig_b200.data import synthetic_batch, collate, Molecule
@@ -685,59 +686,17 @@ def test_node_centred_triplet_gather_equals_edge_centred():
     x_down = torch.randn(e, 64, device=dev)
     sbf_p, t_p = torch.randn(t, 8, device=dev), torch.randn(t, 8, device=dev)
     w_s, w_t = torch.randn(64, 8, device=dev), torch.randn(64, 8, device=dev)
-    default_mode = ops.GATHER_MODE[0]
-    try:
-        for tors in (True, False):
-            outs = {}
-            for mode, split in (("edge", None), ("node", None), ("warp", 1), ("warp", 2), ("warp", 3), ("warp", None)):
-                ops.GATHER_MODE[0], ops.GATHER_SPLIT[0] = mode, split
-                m = torch.full((e, 64), float("nan"), device=dev)
-                ops.triplet_gather(x_down, ctypes.c_void_p(sbf_p.data_ptr()),
-                                   ctypes.c_void_p(t_p.data_ptr()) if tors else None, g,
-                                   w_s.data_ptr(), w_t.data_ptr() if tors else None, m, ops._stream())
-                outs[(mode, split)] = m
-            for key, m in outs.items():
-                assert torch.isfinite(m).all() and torch.equal(outs[("edge", None)], m), (tors, key)
-    finally:
-        ops.GATHER_MODE[0], ops.GATHER_SPLIT[0] = default_mode, None
-
-
-def test_tensor_core_triplet_gather_matches_the_exact_one():
-    """ops.GATHER_MODE 'tc' (lin_sbf2 / lin_t2 expansions as 3xFP16 wgmma MMAs, out-edges packed into 128-row tiles)
-    against the exact FP32 'node' kernel on the same inputs: fp32-level agreement (the operand split keeps ~22 bits),
-    every edge written, with and without torsion, incl. an isolated atom and the 128-molecule headline batch."""
-    import ctypes
-    from dig_b200 import ops
-    from dig_b200.data import synthetic_batch, collate, Molecule
-    dev = torch.device("cuda:0")
-    mols = synthetic_batch(9, "qm9", seed=4, variable=True)
-    far = torch.tensor([[50.0, 50.0, 50.0]])
-    small = collate([Molecule(mols.z[:7], mols.pos[:7]), Molecule(torch.tensor([6]), far),
-                     Molecule(mols.z[7:40], mols.pos[7:40])]).to(dev)
-    big = synthetic_batch(128, "qm9", seed=5).to(dev)
-    for b, ng in ((small, 3), (big, 128)):
-        g = ops.build_graph(b.pos, b.batch, 5.0, num_graphs=ng)
-        ops.triplet_geometry(g, b.pos, use_torsion=True, want_idx=False)
-        e, t = g.n_edges, g.n_triplets
-        torch.manual_seed(1)
-        x_down = torch.randn(e, 64, device=dev)
-        sbf_p, t_p = torch.randn(t, 8, device=dev), torch.randn(t, 8, device=dev)
-        w_s, w_t = torch.randn(64, 8, device=dev) * 0.3, torch.randn(64, 8, device=dev) * 0.3
-        for tors in (True, False):
-            outs = []
-            for mode in ("node", "tc"):
-                ops.GATHER_MODE[0] = mode
-                m = torch.full((e, 64), float("nan"), device=dev)
-                ops.triplet_gather(x_down, ctypes.c_void_p(sbf_p.data_ptr()),
-                                   ctypes.c_void_p(t_p.data_ptr()) if tors else None, g,
-                                   w_s.data_ptr(), w_t.data_ptr() if tors else None, m, ops._stream())
-                outs.append(m)
-            ops.GATHER_MODE[0] = "warp"
-            torch.cuda.synchronize()
-            assert ops.tc_timeouts() == 0
-            assert torch.isfinite(outs[1]).all(), (ng, tors)
-            err = (outs[1] - outs[0]).abs().max().item() / outs[0].abs().max().item()
-            assert err < 2e-6, (ng, tors, err)
+    for tors in (True, False):
+        sp, tp = ctypes.c_void_p(sbf_p.data_ptr()), ctypes.c_void_p(t_p.data_ptr()) if tors else None
+        ws, wt = w_s.data_ptr(), w_t.data_ptr() if tors else None
+        edge = torch.full((e, 64), float("nan"), device=dev)
+        ops.call("dig3d_sphere_triplet_gather", ops._p(x_down), sp, tp, 8, ops._p(g.src), ops._p(g.dst),
+                 ops._p(g.row_ptr), ops._p(g.trip_ptr), e, ws, wt, ops._p(edge), ops._stream())
+        assert torch.isfinite(edge).all(), tors
+        for split in (1, 2, 3, None):
+            m = torch.full((e, 64), float("nan"), device=dev)
+            ops.triplet_gather(x_down, sp, tp, g, ws, wt, m, ops._stream(), split=split)
+            assert torch.equal(edge, m), (tors, split)
 
 
 def test_training_step_parity_at_the_headline_size():

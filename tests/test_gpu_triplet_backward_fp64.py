@@ -1,6 +1,6 @@
 """The triplet-stage backward kernels of SphereNet / DimeNet++ training, one by one and element by element against fp64.
 
-    ops.sphere_triplet_gather (both organisations) / ops.sphere_triplet_gather_bwd     ag.triplet_gather
+    ops.sphere_triplet_gather (warp and edge kernels) / ops.sphere_triplet_gather_bwd  ag.triplet_gather
     ops.triplet_basis_project_bwd                                                      ag.basis_project
     ops.rbf_freq_grad                                                                  ag.edge_basis
 
@@ -111,21 +111,19 @@ def _check_gather_bwd(outs, exact, counts, tors, tag):
 # ------------------------------------------------------------------------------------------------ the gather
 @pytest.mark.parametrize("tors", [True, False], ids=["torsion", "no_torsion"])
 @pytest.mark.parametrize("graph", GRAPHS)
-def test_triplet_gather_forward_both_organisations(graph, tors):
+def test_triplet_gather_forward_warp_and_edge_kernels(graph, tors):
     from dig_b200 import ops
     G = _graph(graph)
     x, s, tp, ws, wt, _ = _gather_inputs(G, tors)
     exact, counts = _gather_ref(G, tors)
     v, m = exact["m"]
-    old = ops.GATHER_MODE[0]
-    got = {}
-    try:
-        for mode in ("warp", "edge"):
-            ops.GATHER_MODE[0] = mode
-            got[mode] = ops.sphere_triplet_gather(x, s, tp, G["g"], ws, wt)
-            _note("gather_fwd.m", ref.check(got[mode], v, ref.bound(m, counts["m"]), f"{graph} m ({mode})"))
-    finally:
-        ops.GATHER_MODE[0] = old
+    g = G["g"]
+    got = {"warp": ops.sphere_triplet_gather(x, s, tp, g, ws, wt), "edge": torch.empty(g.n_edges, 64, device="cuda:0")}
+    ops.call("dig3d_sphere_triplet_gather", ops._p(x), ops._p(s), ops._p(tp), 8, ops._p(g.src), ops._p(g.dst),
+             ops._p(g.row_ptr), ops._p(g.trip_ptr), g.n_edges, ops._p(ws), ops._p(wt), ops._p(got["edge"]),
+             ops._stream())
+    for mode in ("warp", "edge"):
+        _note("gather_fwd.m", ref.check(got[mode], v, ref.bound(m, counts["m"]), f"{graph} m ({mode})"))
     assert torch.equal(got["warp"], got["edge"])
     torch.cuda.synchronize()
     assert ops.tc_timeouts() == 0

@@ -11,7 +11,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SO = os.path.join(ROOT, "dig_b200", "libdig3d.so")
-pat = re.compile(sys.argv[1] if len(sys.argv) > 1 else r"h16|_tc_kernel|gather_node|linear_tc")
+pat = re.compile(sys.argv[1] if len(sys.argv) > 1 else r"h16|_tc_kernel|gather_warp|linear_tc")
 KEY = ("UTCHMMA", "UTCQMMA", "UTCBAR", "LDTM", "STTM", "UBLKCP", "UTMALDG", "SYNCS", "USETMAXREG", "HMMA", "MUFU", "FFMA2", "FMUL2", "FADD2",
        "F2FP", "LDL", "STL", "ATOMS", "RED", "ATOMG")
 out = subprocess.run(["cuobjdump", "-sass", SO], capture_output=True, text=True).stdout
