@@ -201,6 +201,9 @@ SIGNATURES = {
     "dig3d_mmd_terms": [P, c_int64, c_int64, c_double, c_int32, c_double, P, c_int64, P, P],
     "dig3d_xyz2mol": [P, P, c_int64, c_int32, P, P, P],
     "dig3d_gen_traj": [P, P, P, P, c_int64, P, P, P, P, P, P, P, P, P, P, P, P, P],
+    "dig3d_fire_step": [P, P, P, P, c_int32, P, P, P, c_int64, P, P, P, P, P, P, P, P, P, c_double, c_int32,
+                        c_double, c_double, P],
+    "dig3d_relax_compact": [P, P, c_int64, P, P, P, P, P, P],
 }
 _RESTYPES = {"dig3d_last_error": c_char_p}
 
@@ -234,8 +237,8 @@ def load():
 
 
 # Launch accounting (bench.py's `gpu_launches`) and optional per-kernel CUDA-event timing
-# (bench.py's roofline pass).  Every entry point except scan/ptr helpers and dig3d_mmd_terms (three kernels) launches
-# exactly one kernel.
+# (bench.py's roofline pass).  Every entry point except scan/ptr helpers, dig3d_mmd_terms (three kernels) and
+# dig3d_relax_compact (two) launches exactly one kernel.
 launch_count = 0
 _timing = None            # None, or dict name -> list of (start_event, stop_event)
 

@@ -5,6 +5,7 @@ is a hand-written sm_90a kernel in libdig3d.so.  Inputs are validated here (dtyp
 contiguity / alignment), the C side only returns codes.  Nothing in this module has a CPU path.
 """
 import ctypes
+from types import SimpleNamespace
 
 import torch
 
@@ -2054,3 +2055,65 @@ def gen_traj(atom_type, pos, con, n_atoms, device=None):
                                                                "new_angle", "new_torsion")),
              _p(status), _stream())
     return out, ptr, status
+
+
+# ---------------------------------------------------------------------------------------------------- FIRE relaxation
+FIRE_ALPHA_START = 0.1
+
+
+def fire_state(n_graphs, n_atoms, dt, device):
+    """Initial FIRE state for `fire_step`: velocities vel [N, 3] = 0; per structure dt [B] fp64 = dt, alpha [B] fp64 =
+    0.1, n_pos / steps [B] int32 = 0, status [B] int32 = 0 (running); the outputs fmax [B] fp64, energy [B] fp32 and
+    forces [N, 3] fp32."""
+    z = lambda *shape, dtype: torch.zeros(shape, dtype=dtype, device=device)
+    return SimpleNamespace(vel=z(n_atoms, 3, dtype=F32), dt=torch.full((n_graphs,), float(dt), dtype=F64, device=device),
+                           alpha=torch.full((n_graphs,), FIRE_ALPHA_START, dtype=F64, device=device),
+                           n_pos=z(n_graphs, dtype=torch.int32), steps=z(n_graphs, dtype=torch.int32),
+                           status=z(n_graphs, dtype=torch.int32), fmax=z(n_graphs, dtype=F64),
+                           energy=z(n_graphs, dtype=F32), forces=z(n_atoms, 3, dtype=F32))
+
+
+def fire_step(pos, grad, graph_ptr, active, sub_ptr, state, fmax, max_steps, dt_max, max_step, fixed=None,
+              energy=None):
+    """One FIRE step (dig3d_fire_step) of the structures `active` [A] int32 of a batch with graph_ptr [B + 1] int32:
+    pos [N, 3] fp32 and state.vel move in place; grad [sum n_a, 3] fp32 = dE/dpos of the active structures back to back
+    (sub_ptr [A + 1] int32 their offsets), energy [A, out] fp32 (optional) their model outputs, fixed [N] bool
+    (optional).  Writes state.fmax / energy / forces / status for the active structures and advances their FIRE state
+    (see `fire_state`).  One launch, no host synchronisation."""
+    n_act = active.numel()
+    if tuple(pos.shape) != (state.vel.size(0), 3) or tuple(grad.shape) != (grad.size(0), 3) or \
+            sub_ptr.numel() != n_act + 1 or graph_ptr.numel() != state.dt.numel() + 1:
+        raise ValueError(f"fire_step: inconsistent shapes pos {tuple(pos.shape)}, grad {tuple(grad.shape)}, active "
+                         f"[{n_act}], sub_ptr [{sub_ptr.numel()}], graph_ptr [{graph_ptr.numel()}]")
+    if fixed is not None and (fixed.dtype != torch.bool or tuple(fixed.shape) != (pos.size(0),)):
+        raise ValueError(f"fire_step: fixed must be a bool [{pos.size(0)}] mask")
+    if energy is not None and (energy.dim() != 2 or energy.size(0) != n_act):
+        raise ValueError(f"fire_step: energy must be [{n_act}, out], got {tuple(energy.shape)}")
+    i32 = torch.int32
+    call("dig3d_fire_step", _p(pos, F32, "pos"), _p(state.vel, F32, "vel"), _p(grad, F32, "grad"),
+         _p(energy, F32, "energy"), energy.size(1) if energy is not None else 0, _p(graph_ptr, i32, "graph_ptr"),
+         _p(active, i32, "active"), _p(sub_ptr, i32, "sub_ptr"), n_act,
+         _p(fixed.view(torch.uint8) if fixed is not None else None, torch.uint8, "fixed", align=1),
+         _p(state.dt, F64), _p(state.alpha, F64), _p(state.n_pos, i32), _p(state.steps, i32), _p(state.status, i32),
+         _p(state.fmax, F64), _p(state.energy, F32), _p(state.forces, F32), float(fmax), int(max_steps),
+         float(dt_max), float(max_step), _stream())
+
+
+def relax_compact(status, graph_ptr, n_atoms):
+    """The structures with status 0 of a batch of n_atoms atoms (dig3d_relax_compact): returns (active [A] int32, new_ptr [A + 1] int32, atom_map
+    [M] int32 sub-batch atom -> batch atom, new_batch [M] int64), views of buffers sized for the whole batch.  Reads
+    the 8-byte count pair (A, M) back: one host synchronisation."""
+    nb = status.numel()
+    if graph_ptr.numel() != nb + 1:
+        raise ValueError(f"relax_compact: graph_ptr must have {nb + 1} entries, got {graph_ptr.numel()}")
+    dev, i32 = status.device, torch.int32
+    n = int(n_atoms)
+    active = torch.empty(max(nb, 1), dtype=i32, device=dev)
+    new_ptr = torch.empty(nb + 1, dtype=i32, device=dev)
+    atom_map = torch.empty(max(n, 1), dtype=i32, device=dev)
+    new_batch = torch.empty(max(n, 1), dtype=I64, device=dev)
+    counts = torch.empty(2, dtype=i32, device=dev)
+    call("dig3d_relax_compact", _p(status, i32, "status"), _p(graph_ptr, i32, "graph_ptr"), nb, _p(active),
+         _p(new_ptr), _p(atom_map), _p(new_batch), _p(counts), _stream())
+    a, m = counts.tolist()
+    return active[:a], new_ptr[:a + 1], atom_map[:m], new_batch[:m]

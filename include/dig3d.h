@@ -861,6 +861,30 @@ int dig3d_gen_traj(const int64_t* atom_type, const float* pos, const int64_t* co
                    int64_t* out_c1, int64_t* out_c2, int64_t* out_new_type, double* out_dist, double* out_angle,
                    double* out_torsion, int32_t* status, void* stream);
 
+/* ------------------------------------------------------------------ FIRE relaxation (csrc/relax.cu)
+ * One FIRE step (N_min 5, f_inc 1.1, f_dec 0.5, alpha_start 0.1, f_alpha 0.99) for n_active structures, one CTA each.
+ * Structure a of the active list is batch structure s = active[a], atoms graph_ptr[s] .. graph_ptr[s + 1] of
+ * pos / vel [N, 3] fp32 (batch order, updated in place); grad [sum n_a, 3] = dE/dpos of the active structures back to
+ * back, structure a at sub_ptr[a] (the force is -grad); energy [n_active, n_out] (nullable) their model outputs.
+ * fixed [N] (nullable, 0 / 1): fixed atoms feel no force, count in no reduction and are never written.  Per batch
+ * structure, fp64 dt / alpha and int32 n_pos / steps hold the FIRE state; the step writes fmax_out[s] = max over free
+ * atoms of |F_i| (fp64), energy_out[s] = the row sum of energy, force_out (nullable) the structure's forces with zero
+ * rows on fixed atoms, and status[s] = 1 if fmax_out < fmax (no free atom: converged), else 2 if steps >= max_steps
+ * (neither moves), else 0 and the structure takes its step: the power check (skipped while steps = 0), velocity mixing
+ * or reset, v += dt F, dr = dt v clipped to |dr| <= max_step over the structure, steps += 1.  Every reduction is fp64 in
+ * a fixed order that depends only on the structure's atom count: bit-identical between runs and batch compositions. */
+int dig3d_fire_step(float* pos, float* vel, const float* grad, const float* energy, int32_t n_out,
+                    const int32_t* graph_ptr, const int32_t* active, const int32_t* sub_ptr, int64_t n_active,
+                    const uint8_t* fixed, double* dt, double* alpha, int32_t* n_pos, int32_t* steps, int32_t* status,
+                    double* fmax_out, float* energy_out, float* force_out, double fmax, int32_t max_steps,
+                    double dt_max, double max_step, void* stream);
+/* The structures of a batch with status[s] == 0, in batch order: active[A], new_ptr[A + 1] (their graph_ptr in the
+ * sub-batch), atom_map[M] (sub-batch atom -> batch atom), new_batch[M] int64 (sub-batch structure of each atom) and
+ * counts[2] = (A, M).  Buffers are sized for every structure (n_graphs, n_graphs + 1, N, N); only the first A / A + 1 /
+ * M entries are written.  Two launches: one CTA scans, then one warp per active structure fills. */
+int dig3d_relax_compact(const int32_t* status, const int32_t* graph_ptr, int64_t n_graphs, int32_t* active,
+                        int32_t* new_ptr, int32_t* atom_map, int64_t* new_batch, int32_t* counts, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
